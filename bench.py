@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark: sites/s of popgenWindows (pi + Fst + Dxy) on B200.
+"""bench.py — headline benchmark: sites/s of popgenWindows (pi + Fst + Dxy) on H100.
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # the UNMODIFIED reference command line on the host cores
+    python bench.py --gpus 1 --steps K --dump-outputs DIR     # + the rows of the last timed step as DIR/<name>.npy
 
 Workload (BASELINE.json configs[1], "C2"): 4 populations x 50 diploid samples (H = 400 haplotypes), 10 M synthetic sites per
 GPU, -w 50000 coordinate windows (~5000 sites each), -m 100, minData 0.01.  A "step" is one pass of the hot path (site pass ->
@@ -11,7 +12,7 @@ window statistics -> rows on the host) over that batch.
   value           whole-job sites/s, matrix resident in HBM, NO missing genotypes: every window takes the closed-form
                   allele-count path (K1, the HBM-roofline kernel)
   value_missing   the same with 2 % missing genotypes — what real data looks like: every window is "ragged" and takes the
-                  pairwise path (K2: tcgen05 int8 Gram kernels); roofline_missing describes its kernels
+                  pairwise path (K2: wgmma int8 Gram kernels); roofline_missing describes its kernels
   e2e             value's workload through the public API from pinned HOST buffers (H2D + transcode + statistics + D2H)
   c3 / c4 / c5    the other BASELINE.json configs as first-class legs: C3 ABBABABAwindows strong scaling (10 M sites over the
                   N GPUs), C4 distMat 500 diploid samples x 2 M sites (N = 1), C5 freq.py + popgenWindows 8 x 100 samples,
@@ -20,6 +21,10 @@ window statistics -> rows on the host) over that batch.
   cpu_baseline    the unmodified reference command line (oracle/_ref/popgenWindows.py, staged by oracle/build_ref.py) on a
                   bounded sample of the workload, best of -T in {1, 8, all cores}; falls back to the loop-faithful port
                   (oracle/ref_port.py) only if the staged scripts are missing
+
+Every leg times --steps steps.  The inputs are synthetic and seeded: the same arguments give the same inputs on every run,
+so the arrays written by --dump-outputs (float64, one per statistic of the headline and the missing-data leg) can be
+compared between two builds.
 
 Multi-GPU: one process per GPU (torchrun); every rank owns its own shard, no data-path collective, the per-window records are
 all-gathered once per step by the engine's native NCCL call.  Time = max over ranks.
@@ -297,6 +302,17 @@ def rows_equal(a: dict, b: dict, keys, rtol=0.0):
     return True
 
 
+DUMP_KEYS = ("sites", "pos_sum", "path", "pi", "dxy", "fst")
+
+
+def dump_outputs(out_dir, legs):
+    """The per-window rows a caller of the timed path receives, as float64 .npy files (a few MB at the default size)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for prefix, rows in legs.items():
+        for k in DUMP_KEYS:
+            np.save(os.path.join(out_dir, prefix + k + ".npy"), np.ascontiguousarray(np.asarray(rows[k], dtype=np.float64)))
+
+
 def main():
     quiet_stdout()
     ap = argparse.ArgumentParser()
@@ -308,6 +324,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-legs", action="store_true", help="skip the C3 / C4 / C5 / text legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the per-window rows of the last timed step of the headline and missing-data legs as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
@@ -399,12 +417,7 @@ def main():
                     keys.append(k)
         return {k: float(np.mean([t[k]["ms"] for t in tms if k in t])) for k in keys}
 
-    peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
-    try:
-        mp_ = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
-        peak, peak_src = float(mp_["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    except Exception:
-        pass
+    peak, peak_src = 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)"
 
     # =============== C2, resident matrix ===============
     def c2_leg(miss, steps, warmup):
@@ -470,8 +483,12 @@ def main():
                 eng.set_windows(lo, hi)
             barrier()
         paths = np.bincount(eng.popgen(MIN_SITES, MIN_DATA)["path"], minlength=3).tolist()
+        # copied out of the pinned gather slot, which the next pipelined run reuses
+        rows_tab = multigpu.gathered_rows(np.asarray(last), counts, w_max) if dist is not None else np.asarray(last)[:len(lo)]
+        rows = {k: np.array(v) for k, v in multigpu.unpack_device_records(rows_tab, P).items()}
         return dict(dt=dt, tms=tms, launches=launches, steps=steps, W=len(lo), lo=lo, hi=hi, step=step, equal=equal,
-                    paths=paths, table=table, dt_pipe=dt_pipe, launches_pipe=launches_pipe, pipe_equal=pipe_equal)
+                    paths=paths, table=table, dt_pipe=dt_pipe, launches_pipe=launches_pipe, pipe_equal=pipe_equal,
+                    rows=rows)
 
     A = c2_leg(0.0, args.steps, args.warmup)
     value_sync = world * S * args.steps / A["dt"]
@@ -494,7 +511,7 @@ def main():
             eng.set_windows(A["lo"], A["hi"])
             return A["step"]()                        # statistics + D2H of the rows (+ all-gather when N > 1)
 
-        e_steps = max(3, min(args.steps, 10))
+        e_steps = args.steps
         dt_e, _, _ = timed(step_e2e, e_steps, 1)
         npairs = P * (P - 1) // 2
         e2e = {"value": world * S * e_steps / dt_e, "unit": "sites/s", "h2d_bytes_per_step": int(S) * (H + 4),
@@ -504,8 +521,8 @@ def main():
         hp.close()
 
     # =============== C2 with 2 % missing genotypes: the pairwise path ===============
-    m_steps = max(3, min(args.steps, 10))
-    B = c2_leg(0.02, m_steps, 2)
+    m_steps = args.steps
+    B = c2_leg(0.02, m_steps, args.warmup)
     value_missing = world * S * m_steps / B["dt_pipe"]
     value_missing_sync = world * S * m_steps / B["dt"]
     kernel_ms_missing = mean_ms(B["tms"])
@@ -519,8 +536,7 @@ def main():
         n_var = None
         macs_n = tiles(208) * S                                            # 200 sample rows (padded to 208), K = every site
         gram_ms = km.get("k2t_gram_n", 0.0) + km.get("k2t_gram_diff", 0.0)
-        sm_clock = 1.965e9
-        int8_peak = 148 * 8192 * sm_clock                                   # measured: M128 N256 K32 per 128 cycles per SM
+        int8_peak = 1979e12 / 2                                             # H100 SXM data sheet: 1979 dense INT8 TOPS
         vc = "k2t_valid_class"                                              # the chain's HBM-bound kernel
         roofline_missing = {
             "bound": "hbm", "kernel": vc, "kernel_ms": km[vc], "longest_kernel": dom,
@@ -529,13 +545,12 @@ def main():
             "frac": S * (H + 4) / (km[vc] * 1e-3) / 1e9 / peak,
             "traffic": None, "peak_source": peak_src,
             "algorithmic_bytes_per_launch": S * (H + 4),
-            "note": "the pairwise path is a chain of kernels, none above 0.9 ms: k2t_valid_class re-reads the resident matrix "
-                    "(algorithmic bytes = S x (H + 4); issue-bound below the HBM roofline), the tcgen05 Gram kernels are paced by "
-                    "the per-stage chain TMA -> bit-to-byte expansion -> proxy fence -> MMA -> commit (tensor pipe 19-31 % busy, "
-                    "issue slots 50-62 %, no single resource saturated: profiles/r02b_k2t_gram_ncu.txt)",
-            "tensor": {"kernels": "k2t_gram_n + k2t_gram_diff (tcgen05.mma kind::i8, cta_group::1, M128)", "kernel_ms": gram_ms,
+            "note": "the pairwise path is a chain of kernels: k2t_valid_class re-reads the resident matrix (algorithmic "
+                    "bytes = S x (H + 4)); the wgmma Gram kernels are paced by the per-stage chain TMA -> bit-to-byte "
+                    "expansion -> proxy fence -> barrier -> MMA",
+            "tensor": {"kernels": "k2t_gram_n + k2t_gram_diff (wgmma.mma_async u8 x u8 -> s32, M64 per warpgroup)", "kernel_ms": gram_ms,
                        "n_macs": macs_n, "peak_int8_macs_per_s": int8_peak,
-                       "peak_source": "tools/mma_bench.cu on B200: 128 cycles per M128 N256 K32 instruction per SM",
+                       "peak_source": "H100 SXM data sheet: 1979 dense INT8 TOPS at up to 700 W (not measured)",
                        "n_frac_of_int8_peak": macs_n / (km.get("k2t_gram_n", float("nan")) * 1e-3) / int8_peak}}
         del n_var, pair_macs
     except Exception as exc:
@@ -562,8 +577,8 @@ def main():
                     eng.abbababa_allgather(0, 1, 2, 3, 0.5, w3, tab3.array)
                     return tab3.array
                 return eng.abbababa(0, 1, 2, 3, 0.5)
-            c_steps = max(3, min(args.steps, 10))
-            dt3, tms3, _ = timed(step3, c_steps, 2)
+            c_steps = args.steps
+            dt3, tms3, _ = timed(step3, c_steps, args.warmup)
             equal3 = None
             if dist is not None:
                 g3 = multigpu.unpack_abba_records(multigpu.gathered_rows(tab3.array.copy(), counts3, w3))
@@ -617,7 +632,7 @@ def main():
                         eng.popgen_allgather(w5, tab5.array, MIN_SITES, MIN_DATA)
                         return tab5.array
                     return eng.popgen(MIN_SITES, MIN_DATA)
-                s5 = 5 if tag == "popgen" else 2
+                s5 = args.steps
                 dt5_sync, tms5, _ = timed(step5, s5, 1)
                 # pipelined like the headline: exchange + read-back of batch k under the site pass of batch k+1
                 def pipe5():
@@ -789,16 +804,10 @@ def main():
     alg_bytes = S * (H + 4)
     achieved = alg_bytes / (k1_ms * 1e-3) / 1e9
     traffic = None
-    try:
-        traffic = json.load(open(os.path.join(REPO, "profiles", "k1_traffic.json")))["dram_bytes_per_launch"]
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "kernel": "k1_site_pass<POPGEN,4>", "achieved": achieved, "peak": peak, "unit": "GB/s",
                 "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": k1_ms,
-                "note": "the kernel only READS (4.04 GB in, a few MB out); the peak is the driver's copy figure (read + write "
-                        "traffic), so a fraction slightly above 1 is a read-only stream beating a copy, not a measurement error: "
-                        "ncu reports 4.050 GB of DRAM traffic for the 4.040 GB of algorithmic bytes (profiles/k1_traffic.json)",
+                "note": "the kernel only READS (S x (H + 4) bytes in, a few MB out); achieved = algorithmic bytes over kernel time",
                 "missing": roofline_missing}
 
     # ---------------- CPU baseline: the unmodified reference command line on a bounded sample ----------------
@@ -835,6 +844,8 @@ def main():
             "c3": legs.get("c3"), "c4": legs.get("c4"), "c5": legs.get("c5"), "from_text": legs.get("from_text"),
             "variants": variants}
     emit(line)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"": A["rows"], "missing_": B["rows"]})
     eng.close()
     if dist is not None:
         dist.destroy_process_group()

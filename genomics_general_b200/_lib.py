@@ -1,7 +1,7 @@
 """ctypes binding of libpgwin.so (C-ABI: include/pgwin.h).
 
 There is no CPU fallback: if the shared library is missing, or no CUDA device is present when a
-context is created, this raises.  ``build()`` compiles the library in-tree with nvcc for sm_100a.
+context is created, this raises.  ``build()`` compiles the library in-tree with nvcc for sm_90a (H100).
 """
 from __future__ import annotations
 
@@ -21,7 +21,7 @@ class PgError(RuntimeError):
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/*.cu -> libpgwin.so (nvcc, -gencode arch=compute_100a,code=sm_100a -lineinfo)."""
+    """Compile csrc/*.cu -> libpgwin.so (nvcc, -gencode arch=compute_90a,code=sm_90a -lineinfo)."""
     srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".h", ".cpp"))]
     srcs.append(os.path.join(_HERE, "..", "include", "pgwin.h"))
     if not force and os.path.exists(LIB_PATH):
@@ -33,7 +33,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if verbose or r.returncode != 0:
         print(r.stdout)
     if r.returncode != 0:
-        raise PgError("building libpgwin.so failed (nvcc for sm_100a)")
+        raise PgError("building libpgwin.so failed (nvcc for sm_90a)")
     return LIB_PATH
 
 

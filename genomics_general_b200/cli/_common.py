@@ -1,5 +1,5 @@
 """Shared pieces of the four drop-in command lines (flag handling that the reference repeats in every
-script: windows, populations, ploidy, files).  Citations are /root/reference/<file>:<line>."""
+script: windows, populations, ploidy, files).  Citations are genomics_general/<file>:<line>."""
 from __future__ import annotations
 
 import gzip

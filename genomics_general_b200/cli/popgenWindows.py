@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Drop-in for the reference's popgenWindows.py (same flags, header and rows), computed on the GPU.
 
-Reference: /root/reference/popgenWindows.py — argparse 170-213, sample/pop parsing 253-307, header 319-354,
+Reference: genomics_general/popgenWindows.py — argparse 170-213, sample/pop parsing 253-307, header 319-354,
 worker stats_wrapper 28-75.  The process pipeline (producer / -T workers / sorter / writer) is replaced by:
 parse the whole file once -> dense int8 matrix -> all windows in one engine call -> rows.
 All six --analysis modes run on the GPU.  The reference caches one haplotype distance matrix per window and its

@@ -56,8 +56,8 @@ extern "C" int pg_ctx_create(int device, pg_ctx** out) {
     PG_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     PG_CUDA(cudaGetDeviceProperties(&prop, device));
-    PG_CHECK(prop.major >= 10, "pg_ctx_create: device %d is sm_%d%d; libpgwin is built for sm_100a only", device,
-             prop.major, prop.minor);
+    PG_CHECK(prop.major == 9 && prop.minor == 0, "pg_ctx_create: device %d is sm_%d%d; libpgwin is built for sm_90a only",
+             device, prop.major, prop.minor);
     pg_ctx* ctx = new pg_ctx();
     ctx->device = device;
     ctx->sm_count = prop.multiProcessorCount;
@@ -279,7 +279,7 @@ K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw, 
     const int smem_cap = 227 * 1024 - 2048 - table_bytes;   // per-CTA dynamic smem we allow ourselves
     const int tile_target = env_int("PG_K1_TILE_KB", 64) * 1024;
     int G = 1, wpt = 1, I = 1;
-    // lanes per site: keep one lane's walk below ~64 chunks (measured: 1600-haplotype rows run 20 % faster with G = 2),
+    // lanes per site: keep one lane's walk below ~64 chunks (long rows are shared by G lanes; PG_K1_G overrides),
     // and a 32/G-site slab inside the tile target
     while (G < 32 && (p.chunks / G > 64 || (32 / G) * p.pitch > tile_target)) G *= 2;
     if (force_G > 0) G = force_G;           // lane-per-population variant: G = number of populations
@@ -316,7 +316,7 @@ K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw, 
 extern "C" int pg_debug_k1_plan(int64_t S, int32_t H, int32_t* pitch, int32_t* lanes_per_site, int32_t* tile_sites,
                                 int32_t* stages, int32_t* smem_bytes) {
     PG_CHECK(S >= 0 && H > 0, "pg_debug_k1_plan: bad shape");
-    K1Plan p = pg_make_k1_plan(S, H, 148, 4096);
+    K1Plan p = pg_make_k1_plan(S, H, 132, 4096);     // H100 SXM: 132 SMs (the fields reported do not depend on it)
     if (pitch) *pitch = p.pitch;
     if (lanes_per_site) *lanes_per_site = p.G;
     if (tile_sites) *tile_sites = p.T;

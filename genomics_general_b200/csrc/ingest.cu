@@ -413,8 +413,8 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
     // H2D of the text: host threads fill two pinned staging buffers in turn, the copy engine drains them
     {
         const size_t slab = (size_t)64 << 20;
-        // measured on the B200 box (tools/ingest_threads.py, 815 MB of text from memory / page cache): 4 threads 16.6 / 15.1 GB/s,
-        // 8: 14.3 / 15.3, 16: 13.9 / 11.1, 32 and more: ~11 — a few threads saturate the copy into pinned memory, more only contend
+        // a few threads saturate the copy into pinned memory, more only contend (PG_INGEST_THREADS overrides; tools/ingest_threads.py
+        // sweeps it)
         int n_threads = std::max(1, std::min(4, (int)std::thread::hardware_concurrency() / 2));
         if (const char* e = getenv("PG_INGEST_THREADS")) n_threads = std::max(1, std::min(128, atoi(e)));
         if (!ctx->h_text[0]) {

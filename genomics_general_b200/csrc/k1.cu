@@ -26,7 +26,7 @@ constexpr int K1_MAX_WARPS = 12;
 
 enum { MODE_POPGEN = 0, MODE_ABBA = 1, MODE_COUNTS = 2, MODE_POPGEN_FREQ = 3, MODE_FOURPOP = 4,   // FREQ = POPGEN + popFreq counters
        MODE_FOURPOP_Q = 5 };   // FOURPOP with the informative sites of a warp queued and evaluated 32 at a time (site pass only;
-                               // experimental, PG_K1_FOURPOP_QUEUE: measured slower, see the comment in k1_site_pass)
+                               // experimental, PG_K1_FOURPOP_QUEUE: see the comment in k1_site_pass)
 
 struct K1Params {
     const uint8_t* geno;
@@ -636,10 +636,9 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass(const __grid_co
                     // About a third of the lanes hold an informative site, and the ~1000 instructions of the evaluation
                     // run for the whole warp whenever one does.  Here the informative sites move into free queue slots of
                     // the warp (one per lane) and are evaluated when the next ones no longer fit, i.e. with (nearly) all
-                    // 32 lanes at work.  MEASURED on B200 (profiles/r02c_fourpop_queue.jsonl, C2 shape): identical sums,
-                    // but 1.15 ms against 0.90 ms for the default / polarize modes (the ballot / rank / __fns / four
-                    // shuffles of every iteration cost more than the evaluations they save) and 0.70 against 0.78 ms for
-                    // `fixed`, where informative sites are rare — so it stays an experiment (PG_K1_FOURPOP_QUEUE).
+                    // 32 lanes at work.  The sums are identical, but the ballot / rank / __fns / four shuffles of every
+                    // iteration can cost more than the evaluations they save, so it stays an experiment
+                    // (PG_K1_FOURPOP_QUEUE; tools/fourpop_time.py times both).
                     const unsigned full_m = 0xffffffffu;
                     const int seg0 = __shfl_sync(full_m, cur_seg, 0);
                     if (!__all_sync(full_m, cur_seg == seg0)) {
@@ -1348,7 +1347,8 @@ int launch_site_pass_nw(pg_ctx* ctx, const K1Launch& L, const char* name) {
 }
 
 // consumer warps per CTA: 12 (+ the producer = 416 threads, 128 registers each) for rows below 1 KiB; 8 (up to 168
-// registers, no spills) for longer rows, where the 8-population instantiations measured 3-10 % faster (tools/k1_sweep2.py)
+// registers, no spills) for longer rows, where the 8-population instantiations need the registers (tools/k1_sweep2.py
+// compares the two)
 int k1_env_nw12() {
     const char* e = getenv("PG_K1_NW");
     return (e && *e && atoi(e) == 8) ? 8 : 12;

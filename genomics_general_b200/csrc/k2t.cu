@@ -1,4 +1,4 @@
-// K2T — the pairwise path on the 5th-generation tensor cores (tcgen05.mma kind::i8, int32 accumulators in TMEM).
+// K2T — the pairwise path on the Hopper tensor cores (wgmma.mma_async u8 x u8 -> s32, int32 accumulators in registers).
 //
 // Reference semantics (genomics.py:903-916, 1042-1047, 1219-1221): for every haplotype pair of a window
 //   n_ij    = #sites where both are non-missing                 = (V V^T)_ij          V  = 0/1 valid indicator
@@ -17,11 +17,10 @@
 //                     presence nibble + pseudo-site count per chunk                       (one pass, HBM-bound)
 //   k2t_scan / k2t_inv : exclusive scan -> cps[site] (pseudo-site prefix) + inverse map pseudo-site -> (site, P bit, Q mask)
 //   k2t_build_pq    : gathers the variable sites' rows -> P / Q planes (64 pseudo-site chunks)
-//   k2t_gram<NPL>   : persistent CTAs (one per SM) over (window, tile group) items: TMA warps bring plane words into a raw
-//                     ring, three groups of warps expand them to 0/1 bytes in the K-major no-swizzle core-matrix layout
-//                     in shared memory, one warp issues tcgen05.mma (M=128, N<=256, K=32 per instruction) into TMEM,
-//                     tcgen05.commit releases the stage; epilogue warps read the accumulators back with tcgen05.ld and
-//                     write the upper triangle of the symmetric int32 matrix.
+//   k2t_gram<NPL>   : persistent CTAs (one per SM) over (window, tile group) items: a TMA warp brings plane words into a
+//                     raw ring, two consumer warpgroups expand them to 0/1 bytes in the K-major no-swizzle core-matrix
+//                     layout in shared memory and issue wgmma (M=64 per warpgroup, N<=256, K=32 per instruction) on them,
+//                     then write the upper triangle of the symmetric int32 matrix from their accumulator registers.
 #include <stdlib.h>
 
 #include <algorithm>
@@ -385,7 +384,7 @@ __global__ void __launch_bounds__(256, 4) k2t_build_pq(const __grid_constant__ P
 struct GramGroup {
     int a_row0;       // first row of the 128-row A tile
     int b_row0;       // first row of the B range
-    int nb_rows;      // rows of the B range: multiple of 16, <= 512
+    int nb_rows;      // rows of the B range: multiple of 16, <= GRAM_BMAX
     int pad;
 };
 struct GramParams {
@@ -398,30 +397,27 @@ struct GramParams {
     const GramGroup* groups;
     int ngroups;
     int nb;                     // windows
-    int nbmax;                  // max nb_rows over the groups (shared-memory geometry)
+    int brows;                  // rows of the B region of a block: max(128, max nb_rows rounded up to 64)
     int a_sep;                  // some group's A tile lies outside its B range: blocks carry a separate 128-row A region
-    int nstages;                // operand ring depth (a multiple of xg)
-    int nraw;                   // raw plane-word ring depth (a multiple of xg)
-    int xg;                     // expanding groups at work (3, or 2 when only two operand stages fit)
+    int nstages;                // operand ring depth (1 or 2)
+    int nraw;                   // raw plane-word ring depth
     int64_t nchunks;            // chunks of the plane (a stage of CH chunks may reach past the last one: clamped, masked to 0)
     int32_t* out;               // [nb][Hk][Hk], upper triangle (i <= j) only
 };
 
-// Warp roles of the persistent CTA (one per SM), geometry <GW, EW>:
-//   3 GW warps  expand: three groups of GW warps (GW / 4 per scheduler each); group k owns the stages k, k+3, k+6, ... so
-//               that while one group waits (shared-memory loads, the proxy fence) the other two keep the ALUs busy
-//   1 warp      TMEM allocation + MMA issue (warp-uniform loop, an elected lane issues)
-//   3 warps     TMA: warp t brings the plane words of group t's stages into group t's raw slots
-//   EW warps    epilogue: TMEM -> registers -> global (EW = 4 or 8; with 8, warps w and w+4 share TMEM lane quarter w % 4)
-// <8, 4> = 32 warps (the default: 64 registers), <4, 8> = 24 warps (80 registers; PG_K2T_GW=4).
-constexpr int GRAM_XGROUPS = 3;
-constexpr int gram_threads(int GW, int EW) { return (GW * GRAM_XGROUPS + 1 + GRAM_XGROUPS + EW) * 32; }
-constexpr int GRAM_MAX_STAGES = 9;
-constexpr int GRAM_MAX_RAW = 48;           // depth of the raw plane-word ring (TMA runs this many chunks ahead)
+// Warp roles of the persistent CTA (one per SM):
+//   warps 0-7   two consumer warpgroups: they expand the plane words of a stage into 0/1 bytes (K-major, no-swizzle core
+//               matrices) and issue wgmma on it; warpgroup w owns rows 64 w .. 64 w + 63 of the 128-row A tile and keeps its
+//               64 x N int32 accumulators in registers (N <= 256: 128 registers per thread)
+//   warp 8      TMA: plane words of every stage -> raw ring (1-D bulk copies completing on an mbarrier)
+// The MMAs of stage k run while the consumers expand stage k + 1; one named barrier per stage hands the stage over.
+constexpr int GRAM_CTHREADS = 256;
+constexpr int GRAM_THREADS = GRAM_CTHREADS + 32;
+constexpr int GRAM_MAX_RAW = 48;           // depth of the raw plane-word ring (TMA runs this many stages ahead)
+constexpr int GRAM_BMAX = 256;             // B rows of a tile group (the largest wgmma N)
+constexpr int GRAM_ACC = GRAM_BMAX / 2;    // accumulator registers per thread
 
-// 16 bits -> 16 bytes of 0/1 (byte k = bit k): 4 bits -> 4 bytes is one IMAD + LOP3.  (A 256-entry shared-memory table,
-// 8 bits -> 8 bytes per LDS.64, was measured and dropped: the kernel is short of shared-memory bandwidth — the SS-mode MMAs
-// read (128 + N) x 32 bytes per instruction — not of integer issue slots; gram_diff went from 1.07 to 1.35 ms with it.)
+// 16 bits -> 16 bytes of 0/1 (byte k = bit k): 4 bits -> 4 bytes is one IMAD + LOP3
 __device__ __forceinline__ uint4 expand16(uint32_t x) {
     uint4 r;
     r.x = ((x & 0xfu) * 0x00204081u) & 0x01010101u;
@@ -431,48 +427,114 @@ __device__ __forceinline__ uint4 expand16(uint32_t x) {
     return r;
 }
 
-// shared-memory matrix descriptor: K-major, no swizzle; core matrix = 8 rows x 16 bytes stored as 128 contiguous bytes;
-// LBO = byte distance between the two K cores of a K=32 slab (128), SBO = byte distance between 8-row groups (256)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)(128u >> 4) << 16) | ((uint64_t)(256u >> 4) << 32) |
-           (1ull << 46);
+// wgmma shared-memory matrix descriptor: K-major, no swizzle; core matrix = 8 rows x 16 bytes stored as 128 contiguous
+// bytes; LBO = byte distance between the two K cores of a K=32 slab (128), SBO = byte distance between 8-row groups (256)
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)(128u >> 4) << 16) | ((uint64_t)(256u >> 4) << 32);
 }
-// instruction descriptor: D = S32, A = B = UINT8, both K-major, M = 128
-__device__ __forceinline__ uint32_t umma_idesc(int N) {
-    return (2u << 4) | ((uint32_t)(N >> 3) << 17) | ((128u >> 4) << 24);
-}
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t accumulate) {
+
+// D[64 x N] (s32, registers) += A[64 x 32] (u8, shared) * B[N x 32]^T (u8, shared)
+template <int N>
+__device__ __forceinline__ void wgmma_u8(uint32_t (&d)[GRAM_ACC], uint64_t a, uint64_t b);
+template <>
+__device__ __forceinline__ void wgmma_u8<64>(uint32_t (&d)[GRAM_ACC], uint64_t a, uint64_t b) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(a), "l"(b), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n64k32.s32.u8.u8 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+        "}, %32, %33, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(a), "l"(b));
 }
-// one lane of a converged warp (the MMA warp runs its loop with all 32 lanes so that addresses and descriptors stay in
-// uniform registers; only the elected lane issues)
+template <>
+__device__ __forceinline__ void wgmma_u8<128>(uint32_t (&d)[GRAM_ACC], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+        "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+        "}, %64, %65, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(a), "l"(b));
+}
+template <>
+__device__ __forceinline__ void wgmma_u8<192>(uint32_t (&d)[GRAM_ACC], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n192k32.s32.u8.u8 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+        "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+        "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+        "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95"
+        "}, %96, %97, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),
+          "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),
+          "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),
+          "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),
+          "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95])
+        : "l"(a), "l"(b));
+}
+template <>
+__device__ __forceinline__ void wgmma_u8<256>(uint32_t (&d)[GRAM_ACC], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n256k32.s32.u8.u8 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+        "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+        "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+        "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+        "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,"
+        "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+        "}, %128, %129, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),
+          "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),
+          "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),
+          "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),
+          "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),
+          "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]),
+          "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]),
+          "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]),
+          "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+        : "l"(a), "l"(b));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(GRAM_CTHREADS) : "memory"); }
+
+// one lane of a converged warp (the TMA warp runs its loop with all 32 lanes so that addresses stay warp-uniform)
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// position in a ring of `n` slots + the parity of the current pass; advances by small steps
-struct RingPos {
-    int s;
-    uint32_t ph;
-    __device__ __forceinline__ void advance(int delta, int n) {
-        s += delta;
-        while (s >= n) {
-            s -= n;
-            ph ^= 1u;
-        }
-    }
-};
 
 // work item j of this launch -> (window, group) and the chunk range of the window in plane coordinates
 struct GramItem {
@@ -498,26 +560,38 @@ __device__ __forceinline__ GramItem gram_item(const GramParams& gp, int64_t j) {
     return it;
 }
 
-// Shared memory: [raw ring: nraw slots of NPL x RROWS plane words, filled by 1-D TMA bulk copies]
-//                [operand ring: nstages stages of 2 K steps x NPL planes x RROWS rows x 32 bytes] [+ slack]
-// RROWS = (128 rows of a separate A tile, only when some group needs one) + nbmax rows of the B range.
-// CH = chunks per stage (1, 2 or 4): every per-stage hand-over (TMA wait, proxy fence, MMA issue, commit) serves CH x 64 sites.
-template <int NPL, int GW, int EW, int CH = 1>
-__global__ void __launch_bounds__(gram_threads(GW, EW), 1) k2t_gram(const __grid_constant__ GramParams gp) {
+// the MMAs of one stage for one warpgroup: 2 CH K steps of 32 (pseudo-)sites
+template <int NPL, int CH, int N>
+__device__ __forceinline__ void gram_stage_mma(uint32_t (&acc)[GRAM_ACC], uint32_t st, uint32_t a_off, uint32_t b_off,
+                                               uint32_t blk) {
+#pragma unroll
+    for (int ks = 0; ks < 2 * CH; ++ks) {
+        if (NPL == 1) {
+            const uint32_t bk = st + ks * blk;
+            wgmma_u8<N>(acc, gmma_desc(bk + a_off), gmma_desc(bk + b_off));
+        } else {
+            const uint32_t bp = st + (ks * 2) * blk, bq = bp + blk;
+            wgmma_u8<N>(acc, gmma_desc(bp + a_off), gmma_desc(bq + b_off));
+            wgmma_u8<N>(acc, gmma_desc(bq + a_off), gmma_desc(bp + b_off));
+        }
+    }
+}
+
+// Shared memory: [raw ring: nraw slots of CH x NPL x RROWS plane words, filled by 1-D TMA bulk copies]
+//                [operand ring: nstages stages of 2 CH K steps x NPL planes x RROWS rows x 32 bytes]
+// RROWS = (128 rows of a separate A tile, only when some group needs one) + brows rows of the B range.  Rows of a block
+// beyond the item's B range hold stale bytes: they only reach accumulator rows / columns that are not stored.
+// CH = chunks per stage (1, 2 or 4): every per-stage hand-over (TMA wait, proxy fence, barrier, MMA issue) serves CH x 64 sites.
+template <int NPL, int CH>
+__global__ void __launch_bounds__(GRAM_THREADS, 1) k2t_gram(const __grid_constant__ GramParams gp) {
     static_assert(CH == 1 || CH == 2 || CH == 4, "chunks per stage");
-    constexpr int GRAM_XWARPS = GW * GRAM_XGROUPS, GTHREADS = GW * 32;
-    constexpr int GRAM_WARP_MMA = GRAM_XWARPS, GRAM_WARP_TMA = GRAM_XWARPS + 1, GRAM_WARP_EPI = GRAM_WARP_TMA + GRAM_XGROUPS;
-    constexpr int GRAM_EPI_WARPS = EW;
-    constexpr int GRAM_MAX_ITEMS = ((128 + 512) * NPL + GTHREADS - 1) / GTHREADS;    // plane rows per expanding thread and stage
-    static_assert(GW % 4 == 0 && (EW == 4 || EW == 8) , "warp roles");
+    constexpr int GRAM_MAX_ITEMS = ((128 + GRAM_BMAX) * NPL + GRAM_CTHREADS - 1) / GRAM_CTHREADS;   // plane rows per thread
     extern __shared__ __align__(128) uint8_t gsm[];
-    __shared__ __align__(8) uint64_t full[GRAM_MAX_STAGES], empty[GRAM_MAX_STAGES], raw_full[GRAM_MAX_RAW],
-        raw_empty[GRAM_MAX_RAW], tmem_full, tmem_empty;
-    __shared__ uint32_t s_tmem;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    __shared__ __align__(8) uint64_t raw_full[GRAM_MAX_RAW], raw_empty[GRAM_MAX_RAW];
+    const int tid = threadIdx.x, warp = tid >> 5;
     const int NS = gp.nstages, RD = gp.nraw;
     const int AOFF = gp.a_sep ? 128 : 0;                // rows of the separate A region in front of the B rows
-    const int RROWS = AOFF + gp.nbmax;                  // rows of one plane in a raw slot / operand block
+    const int RROWS = AOFF + gp.brows;                  // rows of one plane in a raw slot / operand block
     const int RAW1 = NPL * RROWS * 8;                   // plane words of ONE chunk in a raw slot
     const int RAW = CH * RAW1;                          // bytes of one raw slot
     const int BLK = RROWS * 32;                         // one (K step, plane) operand block
@@ -529,301 +603,167 @@ __global__ void __launch_bounds__(gram_threads(GW, EW), 1) k2t_gram(const __grid
     const int64_t n_items = (int64_t)gp.nb * gp.ngroups;
     const int64_t j0 = n_items * blockIdx.x / gridDim.x, j1 = n_items * (blockIdx.x + 1) / gridDim.x;
 
-    if (warp == GRAM_WARP_MMA) {
-        if (lane == 0) {
-            for (int s = 0; s < NS; ++s) {
-                mbar_init(&full[s], GW);                // the warps of the expanding group that owns the slot
-                mbar_init(&empty[s], 1);
-            }
-            for (int s = 0; s < RD; ++s) {
-                mbar_init(&raw_full[s], 1);
-                mbar_init(&raw_empty[s], GW);
-            }
-            mbar_init(&tmem_full, 1);
-            mbar_init(&tmem_empty, GRAM_EPI_WARPS);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    if (tid == 0) {
+        for (int s = 0; s < RD; ++s) {
+            mbar_init(&raw_full[s], 1);
+            mbar_init(&raw_empty[s], 1);
         }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&s_tmem)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = s_tmem;
 
-    if (warp >= GRAM_WARP_TMA && warp < GRAM_WARP_EPI) {
-        // ---------------- TMA: plane words of every chunk of every item -> raw ring ----------------
-        // One warp per expanding group: warp t loads exactly the stages group t expands (gs % XG == t) into that group's raw
-        // slots, walking the same slot / parity sequence as the group.  (ONE thread issuing every stage's copies — ~60
-        // dependent instructions per stage — was what paced the whole kernel; the loop runs warp-uniform and an elected lane
-        // issues, so addresses stay in uniform registers.)
-        const int XG = gp.xg;
-        const int t = warp - GRAM_WARP_TMA;
-        if (t < XG) {
-            const int RM = RD / XG;
-            int n_done = 0, rm = 0;
-            uint32_t rph = 0;
-            int64_t gbase = 0;
-            for (int64_t j = j0; j < j1; ++j) {
-                const GramItem im = gram_item<NPL, CH>(gp, j);
-                const bool a_in_b = (im.g.a_row0 == im.g.b_row0);
-                const int a_rows = a_in_b ? 0 : min(128, gp.R - im.g.a_row0);
-                const uint32_t bytes_a = (uint32_t)a_rows * 8u, bytes_b = (uint32_t)im.g.nb_rows * 8u;
-                int it = (int)(((int64_t)t - gbase % XG + XG) % XG);
-                for (; it < im.nst; it += XG) {
-                    const int rslot = t + XG * rm;
-                    if (n_done >= RM) mbar_wait(&raw_empty[rslot], rph ^ 1u);
-                    if (elect_one()) {
-                        mbar_expect_tx(&raw_full[rslot], CH * NPL * (bytes_a + bytes_b));
-#pragma unroll
-                        for (int h = 0; h < CH; ++h) {
-                            // a chunk past the end of the plane is read from the last one; its mask is 0
-                            const int64_t chunk = min((im.c_first + it) * CH + h, gp.nchunks - 1);
-#pragma unroll
-                            for (int pl = 0; pl < NPL; ++pl) {
-                                const uint64_t* src = gp.plane + (chunk * NPL + pl) * gp.R;
-                                uint8_t* dst = raw_base + (size_t)rslot * RAW + (size_t)h * RAW1 + (size_t)pl * RROWS * 8;
-                                if (bytes_a) bulk_g2s(dst, src + im.g.a_row0, bytes_a, &raw_full[rslot]);
-                                bulk_g2s(dst + AOFF * 8, src + im.g.b_row0, bytes_b, &raw_full[rslot]);
-                            }
-                        }
-                    }
-                    __syncwarp();
-                    ++n_done;
-                    if (++rm == RM) {
-                        rm = 0;
-                        rph ^= 1u;
-                    }
-                }
-                gbase += im.nst;
-            }
-        }
-    } else if (warp < GRAM_XWARPS) {
-        // ---------------- expand: plane words -> 0/1 bytes in the core-matrix layout ----------------
-        // Group xg owns the global stages gs with gs % XG == xg.  NS and RD are multiples of XG, so a group always cycles
-        // through the same operand slots (xg, xg + XG, ...) and the same raw slots in the same order: every barrier it waits on
-        // is one whose previous phase the same group consumed, and a parity wait can never alias with an older phase.
-        // Several slots per group matter: a slot comes back only after the MMAs that read it have completed (the tensor
-        // pipe's latency), and with one slot per group that latency sat in every group's critical path.
-        const int XG = gp.xg;
-        const int xg = warp / GW, xt = tid % GTHREADS;     // expanding group, thread inside the group
-        const int SM_ = NS / XG, RM = RD / XG;             // operand / raw slots of this group
-        int n_done = 0;                                    // stages this group has processed: stage n is gs = xg + n XG
-        int sm = 0, rm = 0;                                // n_done % SM_, n_done % RM
-        uint32_t sph = 0, rph = 0;                         // (n_done / SM_) & 1, (n_done / RM) & 1
-        int64_t gbase = 0;                                 // global stage index of the item's first stage
-        for (int64_t j = j0; j < j1 && xg < XG; ++j) {
+    if (__shfl_sync(0xffffffffu, warp, 0) == GRAM_CTHREADS / 32) {      // (warp-uniform, visibly so to the compiler)
+        // ---------------- TMA: plane words of every stage of every item -> raw ring ----------------
+        int n_done = 0, rs = 0;
+        uint32_t rph = 0;
+        for (int64_t j = j0; j < j1; ++j) {
             const GramItem im = gram_item<NPL, CH>(gp, j);
             const bool a_in_b = (im.g.a_row0 == im.g.b_row0);
-            // rows expanded per plane: [separate A tile (128 rows)] + B range
-            const int skip_a = a_in_b ? 128 : 0;
-            const int rows_tot = 128 + im.g.nb_rows - skip_a;
-            const int nitems = rows_tot * NPL;
-            int r_idx[GRAM_MAX_ITEMS], d_off[GRAM_MAX_ITEMS];      // raw word index (-1 none, -2 zero row) / byte offset in a block
+            const int a_rows = a_in_b ? 0 : min(128, gp.R - im.g.a_row0);
+            const uint32_t bytes_a = (uint32_t)a_rows * 8u, bytes_b = (uint32_t)im.g.nb_rows * 8u;
+            for (int it = 0; it < im.nst; ++it) {
+                if (n_done >= RD) mbar_wait(&raw_empty[rs], rph ^ 1u);
+                if (elect_one()) {
+                    mbar_expect_tx(&raw_full[rs], CH * NPL * (bytes_a + bytes_b));
 #pragma unroll
-            for (int q = 0; q < GRAM_MAX_ITEMS; ++q) {
-                const int item = xt + q * GTHREADS;
-                r_idx[q] = -1;
-                d_off[q] = 0;
-                if (item < nitems) {
-                    const int pl = (NPL == 2 && item >= rows_tot) ? 1 : 0;
-                    const int rr = item - pl * rows_tot + skip_a;          // < 128: row of the separate A tile
-                    const int x = (rr < 128) ? rr : rr - 128;
-                    const int row = (rr < 128) ? x : AOFF + x;             // row inside the block / raw slot
-                    r_idx[q] = (rr < 128 && im.g.a_row0 + x >= gp.R) ? -2 : pl * RROWS + row;
-                    d_off[q] = pl * BLK + (row >> 3) * 256 + (row & 7) * 16;
-                }
-            }
-            // first local stage of this group: (gbase + it) % XG == xg
-            int it = (int)(((int64_t)xg - gbase % XG + XG) % XG);
-            for (; it < im.nst; it += XG) {
-                const int rslot = xg + XG * rm, sslot = xg + XG * sm;
-                uint64_t mask[CH];
+                    for (int h = 0; h < CH; ++h) {
+                        // a chunk past the end of the plane is read from the last one; its mask is 0
+                        const int64_t chunk = min((im.c_first + it) * CH + h, gp.nchunks - 1);
 #pragma unroll
-                for (int h = 0; h < CH; ++h) {
-                    const int64_t b0 = ((im.c_first + it) * CH + h) << 6;
-                    uint64_t m = 0ull;                                  // a chunk outside the window (CH > 1 only)
-                    if (b0 < im.hi && b0 + 64 > im.lo) {
-                        m = ~0ull;
-                        if (im.lo > b0) m &= ~0ull << (int)(im.lo - b0);
-                        if (im.hi < b0 + 64) m &= ~0ull >> (int)(b0 + 64 - im.hi);
-                    }
-                    mask[h] = m;
-                }
-                mbar_wait(&raw_full[rslot], rph);
-                const uint64_t* rw = reinterpret_cast<const uint64_t*>(raw_base + (size_t)rslot * RAW);
-                uint64_t v[GRAM_MAX_ITEMS][CH];
-#pragma unroll
-                for (int q = 0; q < GRAM_MAX_ITEMS; ++q)
-#pragma unroll
-                    for (int h = 0; h < CH; ++h) v[q][h] = (r_idx[q] >= 0) ? (rw[h * (RAW1 / 8) + r_idx[q]] & mask[h]) : 0ull;
-                if (n_done >= SM_) mbar_wait(&empty[sslot], sph ^ 1u);
-                uint8_t* sb = op_base + (size_t)sslot * STAGE;
-#pragma unroll
-                for (int q = 0; q < GRAM_MAX_ITEMS; ++q) {
-                    if (q * GTHREADS < nitems) {            // warp-uniform: no instructions for item slots nobody uses
-                        if (r_idx[q] != -1) {
-#pragma unroll
-                            for (int h = 0; h < CH; ++h) {
-                                const uint32_t wlo = (uint32_t)v[q][h], whi = (uint32_t)(v[q][h] >> 32);
-                                uint8_t* d0 = sb + (size_t)h * 2 * NPL * BLK + d_off[q];      // K steps 2h, 2h + 1
-                                uint8_t* d1 = d0 + NPL * BLK;
-                                *reinterpret_cast<uint4*>(d0) = expand16(wlo & 0xffffu);
-                                *reinterpret_cast<uint4*>(d0 + 128) = expand16(wlo >> 16);
-                                *reinterpret_cast<uint4*>(d1) = expand16(whi & 0xffffu);
-                                *reinterpret_cast<uint4*>(d1 + 128) = expand16(whi >> 16);
-                            }
+                        for (int pl = 0; pl < NPL; ++pl) {
+                            const uint64_t* src = gp.plane + (chunk * NPL + pl) * gp.R;
+                            uint8_t* dst = raw_base + (size_t)rs * RAW + (size_t)h * RAW1 + (size_t)pl * RROWS * 8;
+                            if (bytes_a) bulk_g2s(dst, src + im.g.a_row0, bytes_a, &raw_full[rs]);
+                            bulk_g2s(dst + AOFF * 8, src + im.g.b_row0, bytes_b, &raw_full[rs]);
                         }
                     }
                 }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
                 __syncwarp();
-                if (lane == 0) {
-                    mbar_arrive(&full[sslot]);
-                    // released only now: the stores above consumed the words, so the loads from the slot have completed
-                    // before the TMA (async proxy) may overwrite it — an arrive right after issuing the loads raced with
-                    // the refill
-                    mbar_arrive(&raw_empty[rslot]);
-                }
                 ++n_done;
-                if (++rm == RM) {
-                    rm = 0;
+                if (++rs == RD) {
+                    rs = 0;
                     rph ^= 1u;
                 }
-                if (++sm == SM_) {
-                    sm = 0;
-                    sph ^= 1u;
-                }
-            }
-            gbase += im.nst;
-        }
-    } else if (warp == GRAM_WARP_MMA) {
-        // ---------------- MMA issue ----------------
-        // The whole warp runs the loop (waits included) so that everything stays warp-uniform — the compiler keeps ring
-        // positions, shared-memory addresses and descriptors in uniform registers, which is what UTCIMMA takes; one elected lane
-        // issues.  Everything that does not change per stage is hoisted and a descriptor is one 32-bit add (the shared-memory
-        // address field sits in the low word).  (Earlier versions ran the loop in lane 0 alone: ~450, then ~110 dependent
-        // instructions per stage through R2UR moves — the issuing thread, not the tensor pipe, set the pace.)
-        {
-            const uint32_t sbase16 = smem_u32(op_base) >> 4;
-            const uint32_t DLO = (128u >> 4) << 16;                       // LBO
-            const uint32_t DHI = (256u >> 4) | (1u << 14);                // SBO | descriptor version 1
-            const uint32_t stage16 = (uint32_t)STAGE >> 4, blk16 = (uint32_t)BLK >> 4;
-            auto D = [&](uint32_t a16) { return ((uint64_t)DHI << 32) | (uint64_t)(DLO + a16); };
-            RingPos sp = {0, 0u};
-            int64_t k = 0;                                  // items done by this CTA
-            for (int64_t j = j0; j < j1; ++j, ++k) {
-                const GramItem im = gram_item<NPL, CH>(gp, j);
-                // A tile inside the B rows for a diagonal group, else the separate A region in front of them
-                const uint32_t a16 = (im.g.a_row0 == im.g.b_row0) ? (uint32_t)AOFF * 2u : 0u;
-                const uint32_t b16 = (uint32_t)AOFF * 2u;                 // 32 bytes per row = 2 units of 16 bytes
-                const int n_a = min(256, im.g.nb_rows), n_b = im.g.nb_rows - n_a;
-                const uint32_t id_a = umma_idesc(n_a), id_b = umma_idesc(n_b > 0 ? n_b : 16);
-                if (k > 0) {                                // the epilogue must have drained the previous accumulators
-                    mbar_wait(&tmem_empty, (uint32_t)((k - 1) & 1));
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                }
-                for (int it = 0; it < im.nst; ++it) {
-                    mbar_wait(&full[sp.s], sp.ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t st16 = sbase16 + (uint32_t)sp.s * stage16;
-                    if (elect_one()) {
-#pragma unroll
-                        for (int ks = 0; ks < 2 * CH; ++ks) {
-                            const uint32_t acc0 = (it > 0 || ks > 0) ? 1u : 0u;
-                            if (NPL == 1) {
-                                const uint32_t blk = st16 + ks * blk16;
-                                umma_i8(tmem, D(blk + a16), D(blk + b16), id_a, acc0);
-                                if (n_b > 0) umma_i8(tmem + 256, D(blk + a16), D(blk + b16 + 512), id_b, acc0);
-                            } else {
-                                const uint32_t bp = st16 + (ks * 2) * blk16, bq = bp + blk16;
-                                umma_i8(tmem, D(bp + a16), D(bq + b16), id_a, acc0);
-                                umma_i8(tmem, D(bq + a16), D(bp + b16), id_a, 1u);
-                                if (n_b > 0) {
-                                    umma_i8(tmem + 256, D(bp + a16), D(bq + b16 + 512), id_b, acc0);
-                                    umma_i8(tmem + 256, D(bq + a16), D(bp + b16 + 512), id_b, 1u);
-                                }
-                            }
-                        }
-                        umma_commit(&empty[sp.s]);  // arrives when the MMAs above have read the stage
-                    }
-                    __syncwarp();
-                    sp.advance(1, NS);
-                }
-                if (elect_one()) umma_commit(&tmem_full);   // arrives when every MMA of the item has completed
-                __syncwarp();
             }
         }
-    } else {
-        // ---------------- epilogue: TMEM -> registers -> symmetric int32 matrix ----------------
-        // Lane = matrix row in TMEM (a warp may touch lanes 32 (warp % 4) ..): the two warps of a quarter take alternate
-        // 32-column blocks; a lane stores its 32 consecutive columns (128 contiguous bytes of its row) with 16-byte stores.
-        // Only [i][j] with i in the A tile and j in the B range is written — the upper triangle of the symmetric matrix
-        // (readers index it through (min, max)).
-        const int ew = warp - GRAM_WARP_EPI;
-        const int qd = warp & 3;
-        const bool vec_ok = (gp.Hk & 3) == 0;              // rows are 16-byte aligned: a lane stores its 32 columns as 8 x 16 bytes
-        int64_t k = 0;
-        for (int64_t j = j0; j < j1; ++j, ++k) {
-            const GramItem im = gram_item<NPL, CH>(gp, j);
-            mbar_wait(&tmem_full, (uint32_t)(k & 1));
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int i = im.g.a_row0 + qd * 32 + lane;     // this lane's matrix row
-            int32_t* orow = gp.out + (size_t)im.wb * gp.Hk * gp.Hk + (size_t)i * gp.Hk;
-            const int cfirst = (ew >> 2) * 32;
-            int c_last = cfirst;                            // last block this warp reads
-            constexpr int CSTEP = (EW / 4) * 32;          // the warps of a lane quarter take alternate 32-column blocks
-            while (c_last + CSTEP < im.g.nb_rows) c_last += CSTEP;
-            if (cfirst >= im.g.nb_rows) {                   // nothing to read: release the accumulators right away
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tmem_empty);
-            }
-            for (int c0 = cfirst; c0 < im.g.nb_rows; c0 += CSTEP) {
-                uint32_t v[32];
-                if (im.nst > 0) {
-                    const uint32_t taddr = tmem + ((uint32_t)(qd * 32) << 16) + (uint32_t)c0;
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,"
-                        "%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-                          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-                          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                        : "r"(taddr)
-                        : "memory");
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) v[e] = 0u;
-                }
-                if (c0 == c_last) {                         // last read of the accumulators: the next item's MMAs may start
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tmem_empty);
-                }
-                if (i < gp.Hk) {
-                    const int jb = im.g.b_row0 + c0;        // first column of the block (multiple of 16)
-                    if (vec_ok) {
-#pragma unroll
-                        for (int e = 0; e < 32; e += 4)
-                            if (jb + e + 4 <= gp.Hk)
-                                *reinterpret_cast<uint4*>(orow + jb + e) = make_uint4(v[e], v[e + 1], v[e + 2], v[e + 3]);
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 32; ++e)
-                            if (jb + e < gp.Hk) orow[jb + e] = (int32_t)v[e];
-                    }
-                }
-            }
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == GRAM_WARP_MMA) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
+
+    // ---------------- consumers: expand + wgmma + store ----------------
+    const int wg = warp >> 2, lane = tid & 31, wq = warp & 3;
+    const uint32_t op16 = smem_u32(op_base);
+    int rs = 0, os = 0;                                 // raw / operand ring positions
+    uint32_t rph = 0;
+    uint32_t acc[GRAM_ACC];
+    for (int64_t j = j0; j < j1; ++j) {
+        const GramItem im = gram_item<NPL, CH>(gp, j);
+        const bool a_in_b = (im.g.a_row0 == im.g.b_row0);
+        // rows expanded per plane: [separate A tile (128 rows)] + B range
+        const int skip_a = a_in_b ? 128 : 0;
+        const int rows_tot = 128 + im.g.nb_rows - skip_a;
+        const int nitems = rows_tot * NPL;
+        int r_idx[GRAM_MAX_ITEMS], d_off[GRAM_MAX_ITEMS];      // raw word index (-1 none, -2 zero row) / byte offset in a block
+#pragma unroll
+        for (int q = 0; q < GRAM_MAX_ITEMS; ++q) {
+            const int item = tid + q * GRAM_CTHREADS;
+            r_idx[q] = -1;
+            d_off[q] = 0;
+            if (item < nitems) {
+                const int pl = (NPL == 2 && item >= rows_tot) ? 1 : 0;
+                const int rr = item - pl * rows_tot + skip_a;          // < 128: row of the separate A tile
+                const int x = (rr < 128) ? rr : rr - 128;
+                const int row = (rr < 128) ? x : AOFF + x;             // row inside the block / raw slot
+                r_idx[q] = (rr < 128 && im.g.a_row0 + x >= gp.R) ? -2 : pl * RROWS + row;
+                d_off[q] = pl * BLK + (row >> 3) * 256 + (row & 7) * 16;
+            }
+        }
+        // operand offsets inside a block: this warpgroup's 64 A rows (inside the B rows for a diagonal group), the B rows
+        const uint32_t a_off = (uint32_t)((a_in_b ? AOFF : 0) + 64 * wg) * 32u, b_off = (uint32_t)AOFF * 32u;
+        const int nsel = __shfl_sync(0xffffffffu, (min(im.g.nb_rows, GRAM_BMAX) + 63) / 64, 0);    // wgmma N = 64 nsel
+#pragma unroll
+        for (int e = 0; e < GRAM_ACC; ++e) acc[e] = 0u;
+        for (int it = 0; it < im.nst; ++it) {
+            uint64_t mask[CH];
+#pragma unroll
+            for (int h = 0; h < CH; ++h) {
+                const int64_t b0 = ((im.c_first + it) * CH + h) << 6;
+                uint64_t m = 0ull;                                  // a chunk outside the window (CH > 1 only)
+                if (b0 < im.hi && b0 + 64 > im.lo) {
+                    m = ~0ull;
+                    if (im.lo > b0) m &= ~0ull << (int)(im.lo - b0);
+                    if (im.hi < b0 + 64) m &= ~0ull >> (int)(b0 + 64 - im.hi);
+                }
+                mask[h] = m;
+            }
+            mbar_wait(&raw_full[rs], rph);
+            const uint64_t* rw = reinterpret_cast<const uint64_t*>(raw_base + (size_t)rs * RAW);
+            uint64_t v[GRAM_MAX_ITEMS][CH];
+#pragma unroll
+            for (int q = 0; q < GRAM_MAX_ITEMS; ++q)
+#pragma unroll
+                for (int h = 0; h < CH; ++h) v[q][h] = (r_idx[q] >= 0) ? (rw[h * (RAW1 / 8) + r_idx[q]] & mask[h]) : 0ull;
+            if (NS == 1) {                      // the only stage may still be read by the previous stage's MMAs
+                wgmma_wait_all();
+                consumers_sync();
+            }
+            uint8_t* sb = op_base + (size_t)os * STAGE;
+#pragma unroll
+            for (int q = 0; q < GRAM_MAX_ITEMS; ++q) {
+                if (q * GRAM_CTHREADS < nitems && r_idx[q] != -1) {
+#pragma unroll
+                    for (int h = 0; h < CH; ++h) {
+                        const uint32_t wlo = (uint32_t)v[q][h], whi = (uint32_t)(v[q][h] >> 32);
+                        uint8_t* d0 = sb + (size_t)h * 2 * NPL * BLK + d_off[q];      // K steps 2h, 2h + 1
+                        uint8_t* d1 = d0 + NPL * BLK;
+                        *reinterpret_cast<uint4*>(d0) = expand16(wlo & 0xffffu);
+                        *reinterpret_cast<uint4*>(d0 + 128) = expand16(wlo >> 16);
+                        *reinterpret_cast<uint4*>(d1) = expand16(whi & 0xffffu);
+                        *reinterpret_cast<uint4*>(d1 + 128) = expand16(whi >> 16);
+                    }
+                }
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
+            // this warpgroup's MMAs of the previous stage are complete; after the barrier every warpgroup's are, so the
+            // other operand slot may be overwritten next, and every row of this stage has been written
+            wgmma_wait_all();
+            consumers_sync();
+            // the loads from the raw slot were consumed by the stores above: the TMA may refill it
+            if (tid == 0) mbar_arrive(&raw_empty[rs]);
+            wgmma_fence();
+            const uint32_t st = op16 + (uint32_t)os * (uint32_t)STAGE;
+            switch (nsel) {
+                case 1: gram_stage_mma<NPL, CH, 64>(acc, st, a_off, b_off, (uint32_t)BLK); break;
+                case 2: gram_stage_mma<NPL, CH, 128>(acc, st, a_off, b_off, (uint32_t)BLK); break;
+                case 3: gram_stage_mma<NPL, CH, 192>(acc, st, a_off, b_off, (uint32_t)BLK); break;
+                default: gram_stage_mma<NPL, CH, 256>(acc, st, a_off, b_off, (uint32_t)BLK); break;
+            }
+            wgmma_commit();
+            if (++rs == RD) {
+                rs = 0;
+                rph ^= 1u;
+            }
+            if (++os == NS) os = 0;
+        }
+        wgmma_wait_all();
+        // ---------------- epilogue: registers -> upper triangle of the symmetric int32 matrix ----------------
+        // Accumulator e of a thread: row 16 wq + lane / 4 + 8 ((e / 2) & 1) of the warpgroup's 64, column 8 (e / 4) + 2 (lane % 4)
+        // + (e & 1).  Only [i][j] with i in the A tile and j in the B range is written (readers index through (min, max)).
+        const int i0 = im.g.a_row0 + 64 * wg + 16 * wq + (lane >> 2);
+        const bool pair_ok = (gp.Hk & 1) == 0;          // two adjacent columns are one aligned 8-byte store
+#pragma unroll
+        for (int e = 0; e < GRAM_ACC; e += 2) {
+            const int c = 8 * (e >> 2) + 2 * (lane & 3);
+            const int i = i0 + 8 * ((e >> 1) & 1), jc = im.g.b_row0 + c;
+            if (c < im.g.nb_rows && i < gp.Hk && jc < gp.Hk) {
+                int32_t* o = gp.out + (size_t)im.wb * gp.Hk * gp.Hk + (size_t)i * gp.Hk + jc;
+                if (pair_ok) {
+                    *reinterpret_cast<int2*>(o) = make_int2((int32_t)acc[e], (int32_t)acc[e + 1]);
+                } else {
+                    o[0] = (int32_t)acc[e];
+                    if (jc + 1 < gp.Hk) o[1] = (int32_t)acc[e + 1];
+                }
+            }
+        }
     }
 }
 
@@ -1041,51 +981,44 @@ int pg_k2t_build(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int
 
 // diff [nb][Hk^2] and n [nb][Hk^2] for nb windows (absolute site ranges on the device)
 namespace {
-// tile groups of an R-row Gram: one 128-row A tile x up to 512 B rows (TMEM has 512 int32 columns per SM)
-void gram_groups(int R, std::vector<GramGroup>& groups, int& nbmax, int& a_sep) {
+// tile groups of an R-row Gram: one 128-row A tile x up to GRAM_BMAX B rows (the accumulators live in registers)
+void gram_groups(int R, std::vector<GramGroup>& groups, int& brows, int& a_sep) {
     groups.clear();
-    nbmax = 16;
+    int nbmax = 16;
     a_sep = 0;
     for (int a0 = 0; a0 < R; a0 += 128)
-        for (int c = a0; c < R; c += 512) {
+        for (int c = a0; c < R; c += GRAM_BMAX) {
             GramGroup g;
             g.a_row0 = a0;
             g.b_row0 = c;
-            g.nb_rows = std::min(512, R - c);
+            g.nb_rows = std::min(GRAM_BMAX, R - c);
             g.pad = 0;
             nbmax = std::max(nbmax, g.nb_rows);
             if (c != a0) a_sep = 1;
             groups.push_back(g);
         }
+    // the B region holds the widest wgmma N of any group, and the 128-row A tile of a diagonal group
+    brows = std::max(128, (nbmax + 63) / 64 * 64);
 }
 }  // namespace
 
 int pg_k2t_pairs(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const int64_t* d_hi, int nb, int32_t* d_diff,
                  int32_t* d_n) {
+    const int budget = 227 * 1024 - 1024;      // dynamic shared memory; the barriers are static
     static bool attr_dev[64] = {};
     if (!attr_dev[ctx->device & 63]) {
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 4, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<2, 4, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 8, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<2, 8, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 8, 4, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 8, 4, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, budget));
+        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, budget));
+        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, budget));
+        PG_CUDA(cudaFuncSetAttribute(k2t_gram<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, budget));
         attr_dev[ctx->device & 63] = true;
     }
-    // expanding groups of 8 warps + 4 epilogue warps (30 warps) or 4 + 8 (22 warps): PG_K2T_GW = 4 | 8, per kernel
-    // PG_K2T_GW_N / PG_K2T_GW_D
-    auto gw_of = [](const char* name, int dflt) {
-        const char* e = getenv(name);
-        if (!e) e = getenv("PG_K2T_GW");
-        return e ? atoi(e) : dflt;
-    };
-    const bool wide_n = gw_of("PG_K2T_GW_N", 8) == 8, wide_d = gw_of("PG_K2T_GW_D", 8) == 8;
     // n_ij over the mask rows (one per sample when the haplotypes of a sample share their missingness), diff_ij over all rows
     const int Rn = ps.vpair ? ps.R2 : ps.R;
     std::vector<GramGroup> gn, gd;
-    int nbmax_n, asep_n, nbmax_d, asep_d;
-    gram_groups(Rn, gn, nbmax_n, asep_n);
-    gram_groups(ps.R, gd, nbmax_d, asep_d);
+    int brows_n, asep_n, brows_d, asep_d;
+    gram_groups(Rn, gn, brows_n, asep_n);
+    gram_groups(ps.R, gd, brows_d, asep_d);
     PG_TRY(ctx->misc4.ensure((gn.size() + gd.size()) * sizeof(GramGroup) + 64));
     GramGroup* d_gn = (GramGroup*)ctx->misc4.p;
     GramGroup* d_gd = d_gn + gn.size();
@@ -1096,59 +1029,44 @@ int pg_k2t_pairs(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const in
     gp.win_lo = d_lo;
     gp.win_hi = d_hi;
     gp.nb = nb;
-    // shared memory: an operand ring of (ideally) one stage per expanding group + the raw plane-word ring + 4 KB slack (the
-    // 128-row A tile of a diagonal group may reach past a short B range)
-    const int budget = 222 * 1024;            // + 2.3 KB of static shared memory (barriers, the expansion table) <= 227 KB
-    const int fixed = 4096;
-    auto geometry = [&](int npl, int nbmax, int a_sep, int& nstages, int& nraw, int& xg, int ch = 1) {
-        const int rrows = (a_sep ? 128 : 0) + nbmax;
+    // shared memory: two operand stages (the MMAs of one overlap the expansion of the next) + as deep a raw plane-word ring
+    // as fits.  PG_K2T_NSTAGES = 1 and PG_K2T_NRAW cap both (the smallest rings stress the hand-overs).
+    auto geometry = [&](int npl, int brows, int a_sep, int ch, int& nstages, int& nraw) {
+        const int rrows = (a_sep ? 128 : 0) + brows;
         const int stage = ch * 2 * npl * rrows * 32, raw = ch * npl * rrows * 8;
-        // operand stages: 9, 6 or 3 (three expanding groups with 3 / 2 / 1 slots each), else 2 (two groups); raw slots a
-        // multiple of the group count too, so that every slot has ONE consumer group
-        const int avail = budget - fixed;
         nstages = 2;
-        for (int cand : {9, 6, 3})
-            if (cand * stage + 3 * raw <= avail) {
-                nstages = cand;
-                break;
-            }
         if (const char* e = getenv("PG_K2T_NSTAGES")) nstages = std::max(1, std::min(nstages, atoi(e)));
-        xg = (nstages % 3 == 0) ? 3 : (nstages % 2 == 0 ? 2 : 1);
-        int mult = std::min(GRAM_MAX_RAW / xg, (avail - nstages * stage) / (raw * xg));
-        if (const char* e = getenv("PG_K2T_NRAW")) mult = std::min(mult, atoi(e));
-        nraw = std::max(1, mult) * xg;
-        return (size_t)nstages * stage + (size_t)nraw * raw + fixed;
+        nraw = std::min(GRAM_MAX_RAW, (budget - nstages * stage) / raw);
+        if (const char* e = getenv("PG_K2T_NRAW")) nraw = std::min(nraw, atoi(e));
+        nraw = std::max(1, nraw);
+        return (size_t)nstages * stage + (size_t)nraw * raw;
     };
     {   // persistent CTAs: one per SM, each works through a contiguous range of (window, group) items
         gp.R = Rn;
         gp.Hk = ps.Hm;
         gp.groups = d_gn;
         gp.ngroups = (int)gn.size();
-        gp.nbmax = nbmax_n;
+        gp.brows = brows_n;
         gp.a_sep = asep_n;
-        // 256-site stages (128 / 64 where three of the larger ones do not fit): every site counts for n_ij, so its K is the
-        // long one and the per-stage hand-overs — TMA wait, proxy fence, MMA issue, commit — are what paces the kernel:
-        // 0.70 (64) -> 0.55 (128) -> 0.50 ms (256 sites per stage) on the C2 shape, bit-identical sums.  PG_K2T_CH = 1 | 2 | 4.
-        int ch_n = wide_n ? 4 : 1;
-        if (const char* e = getenv("PG_K2T_CH")) {
-            const int v = atoi(e);
-            ch_n = (v == 4 && wide_n) ? 4 : ((v == 2 && wide_n) ? 2 : 1);
-        }
-        size_t smem = geometry(1, nbmax_n, asep_n, gp.nstages, gp.nraw, gp.xg, ch_n);
-        while (ch_n > 1 && gp.nstages < 3) {
+        // every site counts for n_ij, so its K is the long one: the widest stage (up to 256 sites) whose two operand slots
+        // leave room for at least two raw slots.  PG_K2T_CH = 1 | 2 | 4 caps it.
+        int ch_n = 4;
+        if (const char* e = getenv("PG_K2T_CH")) ch_n = std::min(ch_n, std::max(1, atoi(e)));
+        size_t smem = geometry(1, brows_n, asep_n, ch_n, gp.nstages, gp.nraw);
+        while (ch_n > 1 && (smem > (size_t)budget || gp.nraw < 2)) {
             ch_n /= 2;
-            smem = geometry(1, nbmax_n, asep_n, gp.nstages, gp.nraw, gp.xg, ch_n);
+            smem = geometry(1, brows_n, asep_n, ch_n, gp.nstages, gp.nraw);
         }
+        PG_CHECK(smem <= (size_t)budget, "pairwise path: %d mask rows do not fit the Gram kernel's shared memory", Rn);
         gp.plane = ps.vpair ? ps.vpair : ps.vplane;
         gp.nchunks = ps.nchunk_v;
         gp.cps = nullptr;
         gp.out = d_n;
         const unsigned grid = (unsigned)std::min<int64_t>((int64_t)nb * gp.ngroups, ctx->sm_count);
         const int ti = pg_time_begin(ctx, "k2t_gram_n");
-        if (ch_n == 4) k2t_gram<1, 8, 4, 4><<<grid, gram_threads(8, 4), smem, ctx->stream>>>(gp);
-        else if (ch_n == 2) k2t_gram<1, 8, 4, 2><<<grid, gram_threads(8, 4), smem, ctx->stream>>>(gp);
-        else if (wide_n) k2t_gram<1, 8, 4><<<grid, gram_threads(8, 4), smem, ctx->stream>>>(gp);
-        else k2t_gram<1, 4, 8><<<grid, gram_threads(4, 8), smem, ctx->stream>>>(gp);
+        if (ch_n == 4) k2t_gram<1, 4><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
+        else if (ch_n == 2) k2t_gram<1, 2><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
+        else k2t_gram<1, 1><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
         pg_time_end(ctx, ti);
         PG_CUDA(cudaGetLastError());
     }
@@ -1157,18 +1075,17 @@ int pg_k2t_pairs(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const in
         gp.Hk = ps.Hk;
         gp.groups = d_gd;
         gp.ngroups = (int)gd.size();
-        gp.nbmax = nbmax_d;
+        gp.brows = brows_d;
         gp.a_sep = asep_d;
-        // (128-pseudo-site stages do not fit here: two planes per stage, 3 x 102 KB for 400 rows)
-        const size_t smem = geometry(2, nbmax_d, asep_d, gp.nstages, gp.nraw, gp.xg);
+        const size_t smem = geometry(2, brows_d, asep_d, 1, gp.nstages, gp.nraw);
+        PG_CHECK(smem <= (size_t)budget, "pairwise path: %d haplotype rows do not fit the Gram kernel's shared memory", ps.R);
         gp.plane = ps.pq;
         gp.nchunks = (ps.npseudo + 63) / 64;
         gp.cps = ps.cps;
         gp.out = d_diff;
         const unsigned grid = (unsigned)std::min<int64_t>((int64_t)nb * gp.ngroups, ctx->sm_count);
         const int ti = pg_time_begin(ctx, "k2t_gram_diff");
-        if (wide_d) k2t_gram<2, 8, 4><<<grid, gram_threads(8, 4), smem, ctx->stream>>>(gp);
-        else k2t_gram<2, 4, 8><<<grid, gram_threads(4, 8), smem, ctx->stream>>>(gp);
+        k2t_gram<2, 1><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
         pg_time_end(ctx, ti);
         PG_CUDA(cudaGetLastError());
     }

@@ -76,7 +76,7 @@ int pg_pitch_for(int H);
 
 struct pg_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;
     // genotype matrix
     int8_t* d_geno = nullptr;

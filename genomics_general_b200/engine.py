@@ -1,6 +1,6 @@
 """Thin object wrapper over the C-ABI: one ``Engine`` = one ``pg_ctx`` = one GPU.
 
-All numerics run in libpgwin.so (hand-written CUDA, sm_100a).  numpy is used only for host
+All numerics run in libpgwin.so (hand-written CUDA, sm_90a).  numpy is used only for host
 buffers.  Nothing here computes statistics on the CPU.
 """
 from __future__ import annotations

@@ -1,6 +1,6 @@
-"""``genomics``-compatible host API backed by libpgwin.so (the B200 engine).
+"""``genomics``-compatible host API backed by libpgwin.so (the H100 engine).
 
-This mirrors the slice of /root/reference/genomics.py that the four hot scripts use (SURVEY.md §8b):
+This mirrors the slice of genomics_general/genomics.py that the four hot scripts use (SURVEY.md §8b):
 ``SampleData`` (1264-1290), ``GenoWindow`` (1721-1797), the window generators (1971-2171),
 ``parseGenoFile`` (1949-1967), ``genoToAlignment`` (1101-1127), ``Alignment`` with
 ``distMatrix / pairNonNan / groupDistStats / indPairDists / siteFreqs / siteNonNan / seqNonNan / subset``

@@ -1,11 +1,11 @@
 /*
- * pgwin.h — C-ABI of libpgwin.so: the B200 (sm_100a) engine for the per-window / per-site numerics of
+ * pgwin.h — C-ABI of libpgwin.so: the H100 (sm_90a) engine for the per-window / per-site numerics of
  * simonhmartin/genomics_general (popgenWindows.py / ABBABABAwindows.py / fourPopWindows.py / freq.py / sfs.py /
  * distMat.py) and for the .geno text parsing in front of them.
  *
  * The reference has no FFI: its seam is the Python API of genomics.py as used by the four scripts
  * (SURVEY.md §8b).  Each entry point below names the reference code it replaces
- * (/root/reference/<file>:<line>).  The binding a maintainer would add is a ctypes stub —
+ * (genomics_general/<file>:<line>).  The binding a maintainer would add is a ctypes stub —
  * see INTEGRATION.md and genomics_general_b200/_lib.py.
  *
  * Conventions

@@ -6,7 +6,7 @@ reference`` legs may import it; the product (``genomics_general_b200``) never
 does and fails loudly when its CUDA library is missing.
 
 It restates, over dense int8 arrays, the algorithms of the reference's per-window
-numerics (all citations are /root/reference/<file>:<line>):
+numerics (all citations are genomics_general/<file>:<line>):
 
   pair counts / p-distance .... genomics.py:903-916, 1042-1047, 1219-1221
   nanmean_min ................. genomics.py:88-90
@@ -24,7 +24,7 @@ numerics (all citations are /root/reference/<file>:<line>):
 
 PINNING: the reference has no tests or golden vectors (SURVEY.md §4), so this
 oracle is pinned against outputs of the *reference itself* executed in the
-build container: ``oracle/make_golden.py`` imports /root/reference/genomics.py,
+build container: ``oracle/make_golden.py`` imports genomics_general/genomics.py,
 runs it on small seeded inputs and commits inputs + outputs under
 ``tests/golden/`` (``oracle/make_golden2.py`` adds the second batch); ``tests/test_oracle_golden.py`` and
 ``tests/test_oracle_golden2.py`` check every function here against those fixtures.

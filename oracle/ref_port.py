@@ -9,7 +9,7 @@ box, where /root/reference does not exist.  It is validated against the referenc
 through tests/golden (tests/test_oracle_golden.py) and its throughput against the
 survey's measurements of the unmodified scripts (BASELINE.md §2).
 
-Citations are /root/reference/<file>:<line>.
+Citations are genomics_general/<file>:<line>.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
-"""The tensor-core pairwise path (csrc/k2t.cu: tcgen05.mma kind::i8 Gram kernels over bit-packed planes) against plain numpy
+"""The tensor-core pairwise path (csrc/k2t.cu: wgmma u8 Gram kernels over bit-packed planes) against plain numpy
 and against the round-1 POPC kernels, through the C-ABI: integer pair matrices bit-exact on every tile geometry (one group,
-several 128-row tiles, a separate A region beyond 512 haplotypes, 1600 haplotypes), multi-allelic sites, window edges inside a
+several 128-row tiles, a separate A region beyond 256 haplotypes, 1600 haplotypes), multi-allelic sites, window edges inside a
 64-site chunk, per-sample and per-haplotype missingness, many windows per persistent CTA, and the smallest ring configurations
 (PG_K2T_NRAW / PG_K2T_NSTAGES) that stress the mbarrier hand-overs."""
 import os
@@ -83,7 +83,7 @@ def test_allele_level_missingness_uses_one_mask_row_per_haplotype(eng):
                                  {"PG_K2T_NO_PAIRS": "1"}, {"PG_K2T_CH": "2"}, {"PG_K2T_CH": "2", "PG_K2T_NRAW": "1"},
                                  {"PG_K2T_CH": "1"}], ids=lambda e: "_".join("%s%s" % (k[7:], v) for k, v in e.items()) or "default")
 def test_many_windows_per_cta_equal_the_popc_kernels(eng, env, monkeypatch):
-    """600 windows over 148 persistent CTAs, every ring geometry: statistics identical to the POPC path, run after run"""
+    """600 windows over one persistent CTA per SM, every ring geometry: statistics identical to the POPC path, run after run"""
     S = 3_000_000
     spec = synth.SynthSpec(4, 50, miss=0.02, seed=20260925)
     eng.synth_fill(spec, S)

@@ -132,7 +132,7 @@ def test_mid_pos_matches_python_round():
 def test_geno_window_mutators_follow_the_reference_container():
     """GenoWindow.addSite / addBlock / slide / trim (genomics.py:1745-1788) on the dense-backed mirror: positions, token
     rows and the int8 matrix stay aligned; the expected states are the reference container's (the same calls on
-    /root/reference/genomics.GenoWindow give these lists — the `[:-0]` slice of trim included; the reference's own
+    genomics_general/genomics.GenoWindow give these lists — the `[:-0]` slice of trim included; the reference's own
     addBlock cannot run: its chained comparison of a list / array of positions raises, genomics.py:1749)."""
     from genomics_general_b200 import genomics as G
     w = G.GenoWindow(scaffold="chr1", limits=[1, 100], names=["a", "b"], ploidy=[2, 2])

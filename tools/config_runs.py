@@ -1,5 +1,5 @@
 """Device-side timing of the BASELINE.json configs (C1..C5 shapes) on one GPU. Not the bench contract — a probe
-whose output is kept under profiles/ for DESIGN.md's tables."""
+whose output feeds DESIGN.md's tables."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

@@ -1,4 +1,4 @@
-"""One 2%-missing popgen pass on the C2 row shape (for ncu captures of the pairwise kernels)."""
+"""One 2%-missing popgen pass on the C2 row shape (for profiler captures of the pairwise kernels)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
