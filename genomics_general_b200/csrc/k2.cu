@@ -1123,10 +1123,11 @@ int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, int32_t 
         PG_TRY(ctx->misc5.ensure(nb * (size_t)nblk * 16 + 64));
         ep.blk_s = (double*)ctx->misc5.p;
         ep.blk_c = (long long*)(ep.blk_s + nb * (size_t)nblk);
-        const int ti = pg_time_begin(ctx, "k2_popgen_epi");
         // sample-pair walk: mask ids are r >> 1 (the tensor path's per-sample n rows) and populations start on even rows
         bool by_pairs = ps.tensor && ps.Hm * 2 == ps.Hk && (size_t)nblk * 64 <= 48 * 1024;
         for (int X = 0; X <= P; ++X) by_pairs = by_pairs && (pop_start[X] % 2 == 0);
+        // the timing label names the stage-1 kernel, so that a caller can tell which epilogue ran
+        const int ti = pg_time_begin(ctx, by_pairs ? "k2_popgen_epi_pairs" : "k2_popgen_epi_blocks");
         // one CTA per window when there are many windows, else the blocks of a window over several CTAs (~8 CTAs per SM)
         const unsigned nsplit = (unsigned)std::max<int64_t>(1, std::min<int64_t>(nblk, (8 * (int64_t)ctx->sm_count + (int64_t)nb - 1) / (int64_t)nb));
         if (by_pairs) k2_popgen_epi_pairs<<<dim3((unsigned)nb, nsplit), 128, (size_t)nblk * 64, ctx->stream>>>(ep);

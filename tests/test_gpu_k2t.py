@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from genomics_general_b200 import synth
+from helpers import ref_counts
 
 pytestmark = pytest.mark.gpu
 
@@ -19,17 +20,6 @@ def eng():
     e = Engine(0)
     yield e
     e.close()
-
-
-def ref_counts(g):
-    """g int8 [L, H] -> diff, n int64 [H, H]  (genomics.py:903-916, 1042-1047)"""
-    v = (g >= 0).astype(np.float32)
-    n = (v.T @ v).astype(np.int64)
-    same = np.zeros_like(n)
-    for a in range(4):
-        x = (g == a).astype(np.float32)
-        same += (x.T @ x).astype(np.int64)
-    return n - same, n
 
 
 SHAPES = [  # (pops, samples per pop, sites, missing, p_third, windows)
