@@ -286,6 +286,10 @@ K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw, 
     // warps per tile: the largest team (dividing the consumer-warp count) whose tile still fits the target
     const int wpt_max = (nw % 8 == 0) ? 8 : 4;
     while (wpt < wpt_max && (32 * (wpt * 2) / G) * p.pitch <= tile_target) wpt *= 2;
+    // a tile holds a multiple of 4 sites (the positions ride behind the rows in 16-byte pieces): with 16 or 32 lanes per
+    // site that takes a team of G / 8 warps, even when 4 rows exceed the tile target (pitches above 16 KiB, i.e. more
+    // than 16,368 haplotypes)
+    while (wpt < wpt_max && (32 * wpt / G) % 4 != 0) wpt *= 2;
     if (wpt == wpt_max && G == 1) {
         I = tile_target / (32 * wpt * p.pitch);
         if (I < 1) I = 1;
@@ -313,6 +317,14 @@ K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw, 
     return p;
 }
 
+// The geometry the site-pass kernels run: whole 16-byte position pieces per tile (T % 4 == 0), power-of-two G, teams that
+// divide the consumer warps, a ring of 2..8 stages inside the shared memory.
+int pg_k1_plan_ok(const K1Plan& p) {
+    const bool pow2G = p.G >= 1 && p.G <= 32 && (p.G & (p.G - 1)) == 0;
+    const bool okw = (p.wpt == 1 || p.wpt == 2 || p.wpt == 4 || p.wpt == 8) && p.nw > 0 && (p.nw % p.wpt) == 0;
+    return (p.T % 4) == 0 && pow2G && okw && p.I >= 1 && p.stages >= 2 && p.stages <= 8 && p.smem_bytes <= 227 * 1024;
+}
+
 extern "C" int pg_debug_k1_plan(int64_t S, int32_t H, int32_t* pitch, int32_t* lanes_per_site, int32_t* tile_sites,
                                 int32_t* stages, int32_t* smem_bytes) {
     PG_CHECK(S >= 0 && H > 0, "pg_debug_k1_plan: bad shape");
@@ -322,6 +334,15 @@ extern "C" int pg_debug_k1_plan(int64_t S, int32_t H, int32_t* pitch, int32_t* l
     if (tile_sites) *tile_sites = p.T;
     if (stages) *stages = p.stages;
     if (smem_bytes) *smem_bytes = p.smem_bytes;
+    return PG_OK;
+}
+
+extern "C" int pg_debug_k1_plan_ex(int64_t S, int32_t H, int32_t nw, int32_t force_G, int32_t table_bytes, int32_t* out) {
+    PG_CHECK(S >= 0 && H > 0 && (nw == 8 || nw == 12) && force_G >= 0 && table_bytes >= 0 && out,
+             "pg_debug_k1_plan_ex: bad arguments");
+    K1Plan p = pg_make_k1_plan(S, H, 132, table_bytes, nw, force_G);
+    const int vals[9] = {p.pitch, p.G, p.wpt, p.I, p.T, p.stages, p.smem_bytes, p.ctas, pg_k1_plan_ok(p)};
+    memcpy(out, vals, sizeof(vals));
     return PG_OK;
 }
 

@@ -1156,13 +1156,21 @@ void build_tables(const std::vector<int32_t>& hap_pop_local, int H, int chunks, 
     }
 }
 
+// shared memory of the mask tables (+ the per-population tables of the lane-per-population variant)
+int table_bytes_of(const PopTables& t) { return (int)t.ent_chunk.size() * 20 + 64 + 512; }
+
 int check_plan(const K1Plan& pl) {
-    const bool pow2G = pl.G >= 1 && pl.G <= 32 && (pl.G & (pl.G - 1)) == 0;
-    const bool okw = (pl.wpt == 1 || pl.wpt == 2 || pl.wpt == 4 || pl.wpt == 8) && (pl.nw % pl.wpt) == 0;
     PG_CHECK((pl.T % 4) == 0, "rows of %d bytes are too long for the site-pass kernel", pl.pitch);
-    PG_CHECK(pow2G && okw && pl.I >= 1 && pl.stages >= 2 && pl.stages <= 8 && pl.smem_bytes <= 227 * 1024,
-             "invalid site-pass geometry G=%d wpt=%d I=%d stages=%d smem=%d", pl.G, pl.wpt, pl.I, pl.stages, pl.smem_bytes);
+    PG_CHECK(pg_k1_plan_ok(pl), "invalid site-pass geometry G=%d wpt=%d I=%d stages=%d smem=%d", pl.G, pl.wpt, pl.I, pl.stages,
+             pl.smem_bytes);
     return PG_OK;
+}
+
+// Long rows of 4 or 8 populations prefer the lane-per-population kernel (G = P lanes per site), but its plan stops
+// fitting earlier than the general one (T = 8 sites at G = 4): take it only where it runs.
+bool lanepop_fits(int64_t S, int H, int sm_count, int table_bytes, int nw, int P) {
+    const K1Plan p = pg_make_k1_plan(S, H, sm_count, table_bytes, nw, P);
+    return pg_k1_plan_ok(p) != 0;
 }
 
 struct K1Launch {
@@ -1228,7 +1236,7 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
     PG_TRY(pg_build_segments(ctx));
     build_tables(hap_pop_local, ctx->H, ctx->pitch / 16, Ppad, pt);
     const int n_ent = (int)pt.ent_chunk.size();
-    const int table_bytes = n_ent * 20 + 64 + 512;        // + the per-population tables of the lane-per-population variant
+    const int table_bytes = table_bytes_of(pt);
     PG_CHECK(table_bytes <= 48 * 1024, "population layout needs %d bytes of mask tables (limit 48 KiB)", table_bytes);
     L.plan = pg_make_k1_plan(ctx->S, ctx->H, ctx->sm_count, table_bytes, nw, force_G);
     PG_CHECK(L.plan.stages >= 2, "rows of %d haplotypes are too long for the site-pass kernel (pitch %d bytes)", ctx->H,
@@ -1500,8 +1508,13 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
             maxN = std::max(maxN, N);
         }
         bool lp = !many && (Pp == 4 || Pp == 8) && Pp == P && maxN <= 255 && ctx->pitch >= 1024 && !getenv("PG_K1_NO_BYTES");
-        if (const char* e = getenv("PG_K1_LANEPOP"))
+        if (const char* e = getenv("PG_K1_LANEPOP")) {
             lp = atoi(e) != 0 && !many && (Pp == 4 || Pp == 8) && maxN <= 255 && !getenv("PG_K1_NO_BYTES");
+        } else if (lp) {
+            PopTables pt;
+            build_tables(pop_map, ctx->H, ctx->pitch / 16, Pp, pt);
+            lp = lanepop_fits(ctx->S, ctx->H, ctx->sm_count, table_bytes_of(pt), k1_env_nw12(), Pp);
+        }
         c.lanepop = lp;
         const int nw = lp ? k1_env_nw12() : k1_nw_for(ctx->pitch);
         PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, lp ? Pp : 0));
@@ -1910,12 +1923,13 @@ int site_counts_slab(pg_ctx* ctx, int64_t first, int64_t cnt) {
         PopTables pt;
         build_tables(local, ctx->H, ctx->pitch / 16, Pp, pt);
         const int n_ent = (int)pt.ent_chunk.size();
-        const int table_bytes = n_ent * 20 + 64 + 512;
+        const int table_bytes = table_bytes_of(pt);
         PG_CHECK(table_bytes <= 48 * 1024, "population layout needs too many mask entries");
         K1Launch L;
         // long rows, a full group of 4 or 8 populations: one lane per population (counts fit 16 bits in any case)
         bool lp = (Pp == 4 || Pp == 8) && Pp == pc && ctx->pitch >= 1024;
         if (const char* e = getenv("PG_K1_LANEPOP")) lp = atoi(e) != 0 && (Pp == 4 || Pp == 8);
+        else if (lp) lp = lanepop_fits(cnt, ctx->H, ctx->sm_count, table_bytes, k1_env_nw12(), Pp);
         const int nw = lp ? k1_env_nw12() : k1_nw_for(ctx->pitch);
         L.plan = pg_make_k1_plan(cnt, ctx->H, ctx->sm_count, table_bytes, nw, lp ? Pp : 0);
         PG_CHECK(L.plan.stages >= 2, "rows of %d haplotypes are too long for the site-pass kernel", ctx->H);

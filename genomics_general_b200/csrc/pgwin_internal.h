@@ -72,6 +72,7 @@ struct K1Plan {
     int ctas;         // persistent CTAs, each owning a contiguous tile range
 };
 K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw = 8, int force_G = 0);
+int pg_k1_plan_ok(const K1Plan& p);   // 1 if the site-pass kernels can run this plan
 int pg_pitch_for(int H);
 
 struct pg_ctx {

@@ -460,10 +460,12 @@ class Engine:
         return int(n.value)
 
 
-def k1_plan(S: int, H: int):
-    """Host-only: the site-pass launch geometry for a shape (works without a GPU)."""
-    L = _lib.lib()
-    v = [C.c_int32(0) for _ in range(5)]
-    check(L.pg_debug_k1_plan(int(S), int(H), *[C.byref(x) for x in v]), "pg_debug_k1_plan")
-    return dict(pitch=v[0].value, lanes_per_site=v[1].value, tile_sites=v[2].value, stages=v[3].value,
-                smem_bytes=v[4].value)
+def k1_plan(S: int, H: int, nw: int = 8, lanes: int = 0, table_bytes: int = 4096):
+    """Host-only: the site-pass launch geometry for a shape (works without a GPU).  `nw` consumer warps per CTA (8, or 12
+    for rows under 1 KiB by default), `lanes` > 0 forces the lanes per site (the lane-per-population variant uses one lane
+    per population), `table_bytes` of mask tables share the shared memory.  The PG_K1_* geometry overrides apply, as they
+    do to the launches.  `ok` is False for rows the site pass refuses."""
+    v = (C.c_int32 * 9)()
+    check(_lib.lib().pg_debug_k1_plan_ex(int(S), int(H), int(nw), int(lanes), int(table_bytes), v), "pg_debug_k1_plan_ex")
+    return dict(pitch=v[0], lanes_per_site=v[1], warps_per_tile=v[2], sites_per_lane=v[3], tile_sites=v[4], stages=v[5],
+                smem_bytes=v[6], ctas=v[7], ok=bool(v[8]))

@@ -263,6 +263,11 @@ int pg_launch_count(pg_ctx* ctx, int64_t* n);
 /* Host-only planning self-test hook (no device needed): returns the K1 launch plan for a shape. */
 int pg_debug_k1_plan(int64_t S, int32_t H, int32_t* pitch, int32_t* lanes_per_site, int32_t* tile_sites,
                      int32_t* stages, int32_t* smem_bytes);
+/* The same for a given consumer-warp count (8 or 12), lanes per site forced to force_G (the lane-per-population variant;
+ * 0 = chosen by row length) and table_bytes of mask tables in shared memory.  Reads the PG_K1_* geometry overrides like the
+ * launches do.  out[9] = pitch, G, wpt, I, T (sites per tile), stages, smem_bytes, CTAs on 132 SMs, 1 if the site-pass
+ * kernels accept the plan (0: such rows are refused). */
+int pg_debug_k1_plan_ex(int64_t S, int32_t H, int32_t nw, int32_t force_G, int32_t table_bytes, int32_t* out);
 
 #ifdef __cplusplus
 }

@@ -43,10 +43,15 @@ def test_no_cpu_fallback_without_device():
 
 
 def test_k1_plan_geometry():
-    for S, H in ((10 ** 5, 40), (10 ** 7, 400), (2 * 10 ** 6, 1000), (10 ** 8, 1600), (100, 1), (1000, 3000)):
+    for S, H in ((10 ** 5, 40), (10 ** 7, 400), (2 * 10 ** 6, 1000), (10 ** 8, 1600), (100, 1), (1000, 3000), (10 ** 6, 16368),
+                 (10 ** 6, 16369), (10 ** 6, 20000), (10 ** 6, 28272)):
         p = engine.k1_plan(S, H)
+        assert p["ok"], (S, H, p)
         assert p["pitch"] % 16 == 0 and (p["pitch"] // 16) % 2 == 1 and p["pitch"] >= H      # odd 16-byte chunk count
         assert p["lanes_per_site"] in (1, 2, 4, 8, 16, 32)
+        assert p["tile_sites"] % 4 == 0                          # positions ride behind the rows in 16-byte pieces
+        assert p["tile_sites"] == 32 * p["warps_per_tile"] // p["lanes_per_site"] * p["sites_per_lane"]
+        assert 8 % p["warps_per_tile"] == 0 and 1 <= p["ctas"] <= 132
         assert 2 <= p["stages"] <= 8
         assert p["tile_sites"] * p["pitch"] * p["stages"] <= p["smem_bytes"] <= 227 * 1024
 
