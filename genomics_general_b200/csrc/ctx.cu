@@ -73,6 +73,7 @@ extern "C" int pg_ctx_destroy(pg_ctx* ctx) {
     pg_k1_cache_free(ctx);
     pg_nccl_finalize(ctx);
     ctx->gather.release();
+    ctx->gather_flag.release();
     if (ctx->d_geno) cudaFree(ctx->d_geno);
     if (ctx->d_pos) cudaFree(ctx->d_pos);
     PgBuf* bufs[] = {&ctx->tables, &ctx->part, &ctx->segmeta, &ctx->winmeta, &ctx->out_d, &ctx->out_i,
@@ -415,6 +416,7 @@ extern "C" int pg_alloc_sites(pg_ctx* ctx, int64_t S, int32_t H) {
     ctx->H = H;
     ctx->pitch = pitch;
     if (!same_shape) ctx->epoch += 1;          // same shape: cached launch plans stay valid
+    ctx->data_gen += 1;                        // (synth_fill and the text ingest come through here too)
     PG_CUDA(cudaMemsetAsync(ctx->d_pos, 0, pneed, ctx->stream));
     // every byte starts as "missing" (0x00): row padding and the slack rows never count
     PG_CUDA(cudaMemsetAsync(ctx->d_geno, 0, need, ctx->stream));
@@ -455,6 +457,7 @@ extern "C" int pg_append_sites(pg_ctx* ctx, int64_t n, const int8_t* geno, const
     }
     ctx->S = S1;
     ctx->epoch += 1;
+    ctx->data_gen += 1;
     ctx->brk.clear();
     ctx->ingest_sites = -1;
     return pg_upload_range(ctx, S0, n, geno, pos);
@@ -491,6 +494,7 @@ extern "C" int pg_upload_range(pg_ctx* ctx, int64_t site0, int64_t n, const int8
              (long long)site0, (long long)n, (long long)ctx->S);
     PG_CUDA(cudaSetDevice(ctx->device));
     if (n == 0) return PG_OK;
+    ctx->data_gen += 1;
     if (!ctx->copy_stream) {
         PG_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
         for (int k = 0; k < 2; ++k) {
@@ -660,6 +664,7 @@ extern "C" int pg_set_pops(pg_ctx* ctx, int32_t P, const int32_t* hap_pop) {
         PG_CHECK(hap_pop[h] >= -1 && hap_pop[h] < P, "pg_set_pops: hap_pop[%d]=%d outside [-1,%d)", h, hap_pop[h], P);
     ctx->P = P;
     ctx->epoch += 1;
+    ctx->data_gen += 1;
     return PG_OK;
 }
 

@@ -1480,7 +1480,9 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
             h[w * RC + 2] = (0 < min_sites) ? 0 : 1;
             for (int k = 3; k < RC; ++k) h[w * RC + k] = nanbits;
         }
-        PG_CUDA(cudaMemcpy(d_rec, h.data(), h.size() * 8, cudaMemcpyHostToDevice));
+        // on the ctx stream, so that work queued behind it (the pipelined gather's read-back) sees the records
+        PG_CUDA(cudaMemcpyAsync(d_rec, h.data(), h.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+        PG_CUDA(cudaStreamSynchronize(ctx->stream));
         return PG_OK;
     }
     const int Pp = many ? 2 : pad_pops(P);
@@ -1585,7 +1587,7 @@ int pg_popgen_resolve(pg_ctx* ctx, int32_t min_sites, double min_data, void* d_r
     k2_windows.reserve((size_t)nk2);
     for (int64_t w = 0; w < W; ++w)
         if (h_path[w] == 2) k2_windows.push_back(w);
-    return pg_k2_popgen_windows(ctx, k2_windows, min_sites, min_data, d_rec, RC);
+    return pg_k2_popgen_windows(ctx, k2_windows, ctx->win_lo.data(), ctx->win_hi.data(), min_sites, min_data, d_rec, RC);
 }
 
 // Device-record variant: d_rec is a DEVICE buffer of W * (4 + 5P + 2*npairs) 8-byte words.

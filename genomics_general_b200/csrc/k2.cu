@@ -1070,9 +1070,10 @@ int run_pair_batch(pg_ctx* ctx, const PlaneSet& ps, const std::vector<int64_t>& 
 }  // namespace
 
 // pi / dxy / Fst for the listed windows through the pairwise path, written straight into the device
-// record table at the windows' own rows.
-int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, int32_t min_sites, double min_data, void* d_rec,
-                         int RC) {
+// record table at the windows' own rows.  The bounds come from the caller: the pipelined gather resolves a batch whose
+// windows the ctx may no longer hold.
+int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, const int64_t* win_lo, const int64_t* win_hi,
+                         int32_t min_sites, double min_data, void* d_rec, int RC) {
     const int P = ctx->P;
     // plane rows: haplotypes that belong to a population, sorted by population (stable)
     std::vector<int32_t> order;
@@ -1086,8 +1087,8 @@ int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, int32_t 
     // empty windows cannot be "ragged"; every window here has at least one site
     int64_t lo = ctx->S, hi = 0;
     for (int64_t w : wins) {
-        lo = std::min(lo, ctx->win_lo[w]);
-        hi = std::max(hi, ctx->win_hi[w]);
+        lo = std::min(lo, win_lo[w]);
+        hi = std::max(hi, win_hi[w]);
     }
     PlaneSet ps;
     PG_TRY(build_planes(ctx, order, lo, hi, ps));
@@ -1100,8 +1101,8 @@ int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, int32_t 
         const size_t nb = std::min(per_batch, wins.size() - b0);
         std::vector<int64_t> blo(nb), bhi(nb);
         for (size_t k = 0; k < nb; ++k) {
-            blo[k] = ctx->win_lo[wins[b0 + k]];
-            bhi[k] = ctx->win_hi[wins[b0 + k]];
+            blo[k] = win_lo[wins[b0 + k]];
+            bhi[k] = win_hi[wins[b0 + k]];
         }
         int32_t *d_diff = nullptr, *d_n = nullptr;
         PG_TRY(run_pair_batch(ctx, ps, blo, bhi, &d_diff, &d_n));

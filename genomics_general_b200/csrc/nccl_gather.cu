@@ -136,13 +136,12 @@ extern "C" int pg_popgen_allgather(pg_ctx* ctx, int32_t min_sites, double min_da
     const int RC = 4 + 5 * P + 2 * (P * (P - 1) / 2);
     const size_t slot_words = (size_t)w_max * RC;
     const size_t total_words = slot_words * (size_t)ctx->nccl_ranks;
-    if (ctx->gather.cap < total_words * 8 || ctx->gather_words != total_words) {
-        PG_TRY(ctx->gather.ensure(total_words * 8));
-        PG_CUDA(cudaMemsetAsync(ctx->gather.p, 0, total_words * 8, ctx->stream));
-        ctx->gather_words = total_words;
-    }
+    PG_TRY(ctx->gather.ensure(total_words * 8));
     unsigned long long* base = (unsigned long long*)ctx->gather.p;
     unsigned long long* mine = base + slot_words * (size_t)ctx->nccl_rank;
+    // the finalize writes every word of rows < W and the all-gather every other rank's part; rows W..w_max-1 may hold an
+    // earlier call's records (more windows, or another record layout of the same buffer)
+    PG_CUDA(cudaMemsetAsync(mine + (size_t)ctx->W * RC, 0, (size_t)(w_max - ctx->W) * RC * 8, ctx->stream));
     // enqueue: site pass -> finalize -> all-gather -> D2H of the table; ONE host synchronisation
     int* h_cnt = nullptr;
     PG_TRY(pg_popgen_enqueue(ctx, min_sites, min_data, force_path, mine, &h_cnt));
@@ -204,8 +203,16 @@ extern "C" int pg_popgen_gather_begin(pg_ctx* ctx, int32_t min_sites, double min
     ctx->gslot_wmax[slot] = w_max;
     ctx->gslot_min_sites[slot] = min_sites;
     ctx->gslot_min_data[slot] = min_data;
+    // `end` may run after the windows, the matrix or the populations have changed for the next batch
+    ctx->gslot_W[slot] = ctx->W;
+    ctx->gslot_RC[slot] = RC;
+    ctx->gslot_lo[slot] = ctx->win_lo;
+    ctx->gslot_hi[slot] = ctx->win_hi;
+    ctx->gslot_gen[slot] = ctx->data_gen;
     unsigned long long* base = (unsigned long long*)ctx->gslot[slot].p;
     unsigned long long* mine = base + slot_words * (size_t)rank;
+    // the finalize writes rows < W only: rows of an earlier batch with more windows must not reach the table
+    PG_CUDA(cudaMemsetAsync(mine + (size_t)ctx->W * RC, 0, (size_t)(w_max - ctx->W) * RC * 8, ctx->stream));
     int* h_cnt = nullptr;
     PG_TRY(pg_popgen_enqueue(ctx, min_sites, min_data, 0, mine, &h_cnt));
     PG_CUDA(cudaEventRecord(ctx->g_rec[slot], ctx->stream));
@@ -225,25 +232,43 @@ extern "C" int pg_popgen_gather_end(pg_ctx* ctx, int32_t slot, const void** h_ta
     PG_CUDA(cudaSetDevice(ctx->device));
     PG_CUDA(cudaEventSynchronize(ctx->g_done[slot]));
     const int ranks = ctx->nccl_comm ? ctx->nccl_ranks : 1, rank = ctx->nccl_comm ? ctx->nccl_rank : 0;
-    const int P = ctx->P;
-    const int RC = 4 + 5 * P + 2 * (P * (P - 1) / 2);
-    const int64_t w_max = ctx->gslot_wmax[slot];
+    // the batch as it was at `begin`: the ctx may already hold the next batch's windows, populations or data
+    const int RC = ctx->gslot_RC[slot];
+    const int64_t w_max = ctx->gslot_wmax[slot], W = ctx->gslot_W[slot];
     const size_t slot_words = (size_t)w_max * RC, total_words = slot_words * (size_t)ranks;
     const unsigned long long* tab = (const unsigned long long*)ctx->gslot_host[slot];
-    // windows routed to the pairwise path: a collective decision read off the gathered path column
+    // windows routed to the pairwise path: a collective decision read off the gathered path column (rows past a rank's
+    // window count are zero); this rank's own windows are read off its rows of the slot's table
     bool any = false;
-    int64_t mine_k2 = 0;
+    std::vector<int64_t> k2_windows;
     for (size_t r = 0; r < (size_t)ranks * (size_t)w_max; ++r) {
         const bool k2 = tab[r * RC + 2] == 2ull;
         any = any || k2;
-        if (k2 && r / (size_t)w_max == (size_t)rank) ++mine_k2;
+        if (k2 && r / (size_t)w_max == (size_t)rank && (int64_t)(r % (size_t)w_max) < W)
+            k2_windows.push_back((int64_t)(r % (size_t)w_max));
     }
-    if (n_pairwise) *n_pairwise = mine_k2;
+    if (n_pairwise) *n_pairwise = (int64_t)k2_windows.size();
     if (any) {
+        const long long refuse = (!k2_windows.empty() && ctx->gslot_gen[slot] != ctx->data_gen) ? 1 : 0;
+        long long refusals = refuse;
+        if (ctx->nccl_comm) {      // collective: a rank refusing alone would leave the others waiting in the second gather
+            PG_TRY(ctx->gather_flag.ensure(8));
+            PG_CUDA(cudaMemcpyAsync(ctx->gather_flag.p, &refuse, 8, cudaMemcpyHostToDevice, ctx->stream));
+            PG_TRY(pg_nccl_allreduce_i64(ctx, ctx->gather_flag.p, 1));
+            PG_CUDA(cudaMemcpyAsync(&refusals, ctx->gather_flag.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+            PG_CUDA(cudaStreamSynchronize(ctx->stream));
+        }
+        PG_CHECK(!refuse, "pg_popgen_gather_end: the genotype matrix or the populations changed after this slot's "
+                 "pg_popgen_gather_begin; its %lld pairwise windows cannot be computed from the batch's data "
+                 "(call end before changing them)", (long long)k2_windows.size());
+        PG_CHECK(refusals == 0, "pg_popgen_gather_end: %lld other rank(s) refused this slot: their genotype matrix or "
+                 "populations changed after pg_popgen_gather_begin", refusals);
         unsigned long long* base = (unsigned long long*)ctx->gslot[slot].p;
         unsigned long long* mine = base + slot_words * (size_t)rank;
         PG_CUDA(cudaStreamSynchronize(ctx->gather_stream));
-        PG_TRY(pg_popgen_resolve(ctx, ctx->gslot_min_sites[slot], ctx->gslot_min_data[slot], mine, (int)mine_k2));
+        if (!k2_windows.empty())
+            PG_TRY(pg_k2_popgen_windows(ctx, k2_windows, ctx->gslot_lo[slot].data(), ctx->gslot_hi[slot].data(),
+                                        ctx->gslot_min_sites[slot], ctx->gslot_min_data[slot], mine, RC));
         if (ranks > 1) {
             PG_NCCL(g_nccl.all_gather(mine, base, slot_words, NCCL_UINT64, (NcclComm)ctx->nccl_comm, ctx->stream));
             ctx->launches += 1;
@@ -270,7 +295,6 @@ int gather_fixed_records(pg_ctx* ctx, int rc, int64_t w_max, void* h_table, cons
     unsigned long long* base = (unsigned long long*)ctx->gather.p;
     unsigned long long* mine = base + slot_words * (size_t)ctx->nccl_rank;
     PG_CUDA(cudaMemsetAsync(mine, 0, slot_words * 8, ctx->stream));
-    ctx->gather_words = 0;                                   // the popgen gather re-zeroes its layout next time
     PG_TRY(enqueue(mine));
     PG_NCCL(g_nccl.all_gather(mine, base, slot_words, NCCL_UINT64, (NcclComm)ctx->nccl_comm, ctx->stream));
     ctx->launches += 1;

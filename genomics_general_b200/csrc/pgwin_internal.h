@@ -111,13 +111,15 @@ struct pg_ctx {
     cudaEvent_t stage_full[2] = {nullptr, nullptr}, stage_free[2] = {nullptr, nullptr};
     bool want_freq = false;                   // carry the popFreq counters in the popgen site pass
     uint64_t epoch = 1;                       // bumped by every change of data shape / populations / windows
+    uint64_t data_gen = 1;                    // bumped by every write of the resident matrix or the population map (also
+                                              // an upload of the same shape, which keeps `epoch`)
     void* k1_cache[3] = {nullptr, nullptr, nullptr};   // cached launch state (popgen, abba, fourpop) — owned by k1.cu
     std::vector<unsigned long long> h_rec;    // host copy of the per-window records
     // native NCCL gather (nccl_gather.cu)
     void* nccl_comm = nullptr;
     int nccl_ranks = 1, nccl_rank = 0;
     PgBuf gather;
-    size_t gather_words = 0;
+    PgBuf gather_flag;                        // one int64 all-reduced by the pipelined gather's collective refusal
     // pipelined gather (pg_popgen_gather_begin / _end): two record tables, exchange + read-back on a side stream
     cudaStream_t gather_stream = nullptr;
     cudaEvent_t g_rec[2] = {nullptr, nullptr}, g_done[2] = {nullptr, nullptr};
@@ -127,6 +129,11 @@ struct pg_ctx {
     int64_t gslot_wmax[2] = {0, 0};
     int32_t gslot_min_sites[2] = {0, 0};
     double gslot_min_data[2] = {0, 0};
+    // what `end` needs of the batch as it was at `begin`: window count, record width (from P), bounds, data generation
+    int64_t gslot_W[2] = {0, 0};
+    int32_t gslot_RC[2] = {0, 0};
+    std::vector<int64_t> gslot_lo[2], gslot_hi[2];
+    uint64_t gslot_gen[2] = {0, 0};
     void* h_pinned = nullptr;                 // small pinned staging for result read-back
     size_t h_pinned_cap = 0;
 };
@@ -164,9 +171,10 @@ int pg_k2t_het(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const int6
                int n_ind, int min_sites, double* d_out);
 
 // implemented in k1.cu / k2.cu
-// pairwise statistics for the listed windows, written into the DEVICE record table (stride RC words)
-int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, int32_t min_sites, double min_data,
-                         void* d_rec, int RC);
+// pairwise statistics for the listed windows, written into the DEVICE record table (stride RC words); window w spans sites
+// [win_lo[w], win_hi[w]) of the resident matrix
+int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, const int64_t* win_lo, const int64_t* win_hi,
+                         int32_t min_sites, double min_data, void* d_rec, int RC);
 void pg_k1_cache_free(pg_ctx* ctx);
 int pg_nccl_allreduce_i64(pg_ctx* ctx, void* d_buf, size_t count);   // nccl_gather.cu
 int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t force_path, void* d_rec, int** h_count);

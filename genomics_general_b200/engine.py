@@ -66,6 +66,7 @@ class Engine:
         self.H = 0
         self.P = 0
         self.W = 0
+        self._gslot_shape = {}     # table shape of each pipelined-gather slot, recorded at its begin
 
     # ---- lifetime ----
     def close(self):
@@ -207,16 +208,21 @@ class Engine:
         """Pipelined popgen_allgather: enqueue one batch (statistics on the main stream, all-gather + D2H on a side stream)."""
         check(self._lib.pg_popgen_gather_begin(self._ctx, int(min_sites) if min_sites else 0, float(min_data), int(w_max),
                                                int(slot)), "pg_popgen_gather_begin")
+        world = getattr(self, "_world", 1) or 1
+        self._gslot_shape[int(slot)] = (world * int(w_max), self.popgen_record_width())   # P may change before `end`
 
-    def popgen_gather_end(self, w_max: int, slot: int) -> np.ndarray:
-        """-> float64 [world * w_max, popgen_record_width()] view of the slot's pinned table (valid until its next begin)."""
+    def popgen_gather_end(self, w_max: int, slot: int, with_pairwise: bool = False):
+        """-> float64 [world * w_max, record width at the slot's begin] view of the slot's pinned table (valid until its next
+        begin); with_pairwise=True: (table, number of this rank's windows that took the pairwise path)."""
         p = C.c_void_p()
         n = C.c_int64(0)
         check(self._lib.pg_popgen_gather_end(self._ctx, int(slot), C.byref(p), C.byref(n)), "pg_popgen_gather_end")
+        shape = self._gslot_shape[int(slot)]
         world = getattr(self, "_world", 1) or 1
-        shape = (world * int(w_max), self.popgen_record_width())
+        assert shape[0] == world * int(w_max), (shape, w_max)
         buf = (C.c_double * (shape[0] * shape[1])).from_address(p.value)
-        return np.frombuffer(buf, dtype=np.float64).reshape(shape)
+        table = np.frombuffer(buf, dtype=np.float64).reshape(shape)
+        return (table, int(n.value)) if with_pairwise else table
 
     def abbababa_allgather(self, p1: int, p2: int, p3: int, o: int, min_data: float, w_max: int, table: np.ndarray):
         """ABBA-BABA statistics of this rank's windows + ONE ncclAllGather: `table` float64 [world * w_max, 8] receives

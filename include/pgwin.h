@@ -189,7 +189,15 @@ int pg_popgen_allgather(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t
  * table on a side stream; `end` waits for that batch and returns the slot's pinned table (nranks * w_max records, valid until
  * the slot's next `begin`).  begin(0); begin(1); end(0); begin(0); end(1); ... hides the all-gather and the D2H of one batch
  * under the site pass of the next (the reference's sorter + writer run concurrently with its workers,
- * popgenWindows.py:108-160).  Works without a communicator too (one rank). */
+ * popgenWindows.py:108-160).  Works without a communicator too (one rank).
+ * `begin` records the batch: its windows and their bounds, the record width (P) and a generation of the resident matrix and
+ * population map; this rank's rows W..w_max-1 of the slot are zeroed.  So between begin(k) and end(k) the caller may set the
+ * next batch's windows or populations and call begin(k+1): `end` resolves the slot's pairwise windows (read off its own path
+ * column, *n_pairwise = their number) with the recorded bounds.  When the matrix or the populations changed meanwhile
+ * (upload, synth fill, ingest, append, pg_set_pops) and the slot has pairwise windows, `end` fails with PG_ERR rather
+ * than compute them from the other batch's data; a slot without pairwise windows is complete at `begin` and is returned.
+ * With a communicator the refusal is collective (one all-reduce of a flag, only when some rank has pairwise windows): every
+ * rank returns PG_ERR, so none is left waiting in the second all-gather. */
 int pg_popgen_gather_begin(pg_ctx* ctx, int32_t min_sites, double min_data, int64_t w_max, int32_t slot);
 int pg_popgen_gather_end(pg_ctx* ctx, int32_t slot, const void** h_table, int64_t* n_pairwise);
 /* The same for the ABBA-BABA statistics (ABBABABAwindows.py window-sharded over the GPUs): h_table receives
