@@ -70,6 +70,12 @@ _SIGS = {
                          C.c_void_p, C.POINTER(C.c_int64)]),
     "pg_sfs_tables": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
                                 C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
+    "pg_sfs_sparse": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.POINTER(C.c_int64)]),
+    "pg_sfs_tables_sparse": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32,
+                                       C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.POINTER(C.c_int64)]),
+    "pg_sfs_sparse_fetch": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_pairdist": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                               C.c_void_p]),
     "pg_pairdist_cat": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64)]),

@@ -4,6 +4,10 @@ the joint spectra of pairs / trios / quartets, computed on the GPU — from geno
 counts -> target allele -> dense histograms, `pg_sfs`) or from tables of counts (`baseCounts`: the rows freq.py writes;
 `targetCounts`, the script's default: e.g. freq.py --target derived --asCounts; `pg_sfs_tables`) — and written in the
 reference's sparse format and order.
+A request whose spectra add up to more cells than the dense histograms allow (engine.SFS_MAX_CELLS: e.g. 4-D spectra
+of 129+ haplotypes per population, --doQuartets on many populations, count tables with large counts) takes the sparse
+path instead (`pg_sfs_sparse` / `pg_sfs_tables_sparse`: only the non-empty cells, with their counts and first sites);
+the choice is made once per request, and every other request keeps the dense path.
 
 `--regions` / `--regionsFile` (sfs.py:266-276, 430-435): one count column per interval — the spectra of the intervals
 are computed one after the other on the device (the interval is a site mask) and merged into the reference's rows.
@@ -27,7 +31,7 @@ import sys
 import numpy as np
 
 from .. import genomics, mgpu
-from ..engine import Engine
+from ..engine import SFS_MAX_CELLS, Engine, sfs_shapes, sfs_table_dims
 from . import _common as C
 
 
@@ -68,11 +72,10 @@ def build_parser():
     return p
 
 
-def ordered_chains(hist, first):
-    """Dense spectrum + first-site array -> rows [k1, .., kd, count] in the order the reference writes its nested
-    SparseFS dictionaries (sfs.py:117-125): at every nesting level, keys in order of first appearance.  `hist` / `first`
-    may be lists (one spectrum per --regions interval): a row then carries one count per interval, and a key appears
-    when its first site in ANY interval does (sfs.py:492-494 adds the whole boolean vector at once)."""
+def dense_entries(hist, first):
+    """Dense spectrum + first-site array -> its non-empty cells: (coords int64 [nnz, d], [count [nnz]], first [nnz]).
+    `hist` / `first` may be lists (one spectrum per --regions interval): a cell is then non-empty in ANY interval, there is
+    one count array per interval, and `first` is the cell's first site over the intervals that hold it."""
     hs = list(hist) if isinstance(hist, (list, tuple)) else [hist]
     fs = list(first) if isinstance(first, (list, tuple)) else [first]
     big = np.iinfo(np.int64).max
@@ -82,30 +85,83 @@ def ordered_chains(hist, first):
         tot = tot + h
         fmin = np.minimum(fmin, np.where(h > 0, f1, big))
     nz = np.argwhere(tot > 0)
-    if len(nz) == 0:
+    return nz, [h[tuple(nz.T)] for h in hs], fmin[tuple(nz.T)]
+
+
+def order_entries(coords, counts, first):
+    """Non-empty cells (coords [nnz, d], one count array per interval, first site [nnz]; any order) -> rows
+    [k1, .., kd, count, ..] in the order the reference writes its nested SparseFS dictionaries (sfs.py:116-122): at every
+    nesting level, keys in order of first appearance.  A site hits one cell of a spectrum, so the first sites are
+    distinct and the order is total."""
+    if len(coords) == 0:
         return []
-    f = fmin[tuple(nz.T)]
+    big = np.iinfo(np.int64).max
+    f = np.asarray(first, dtype=np.int64)
     keys = []
-    for lev in range(nz.shape[1]):
-        _, inv = np.unique(nz[:, :lev + 1], axis=0, return_inverse=True)
+    for lev in range(coords.shape[1]):
+        _, inv = np.unique(coords[:, :lev + 1], axis=0, return_inverse=True)
         inv = np.asarray(inv).reshape(-1)
         m = np.full(inv.max() + 1, big, dtype=np.int64)
         np.minimum.at(m, inv, f)
         keys.append(m[inv])
     order = np.lexsort(tuple(reversed(keys)))
-    cnts = [h[tuple(nz.T)] for h in hs]
-    return [list(map(int, nz[i])) + [int(c[i]) for c in cnts] for i in order]
+    return [list(map(int, coords[i])) + [int(c[i]) for c in counts] for i in order]
 
 
-def write_spectra(args, FSpops, hists, firsts):
+def ordered_chains(hist, first):
+    """Dense spectrum + first-site array (or one of each per --regions interval) -> rows in the reference's order: a row
+    carries one count per interval, and a key appears when its first site in ANY interval does (sfs.py:492-494 adds the
+    whole boolean vector at once)."""
+    return order_entries(*dense_entries(hist, first))
+
+
+def merge_sparse(parts):
+    """[(coords, count, first)] of one spectrum (one per interval or per rank) -> the union of their cells: (coords,
+    [count per part, 0 where the part lacks the cell], first site over the parts that hold it)"""
+    big = np.iinfo(np.int64).max
+    d = parts[0][0].shape[1]
+    allc = np.concatenate([np.asarray(p[0], dtype=np.int64).reshape(-1, d) for p in parts])
+    if len(allc) == 0:
+        return allc, [np.zeros(0, dtype=np.int64) for _ in parts], np.zeros(0, dtype=np.int64)
+    coords, inv = np.unique(allc, axis=0, return_inverse=True)
+    inv = np.asarray(inv).reshape(-1)
+    counts, fmin, o = [], np.full(len(coords), big, dtype=np.int64), 0
+    for c, n, f in parts:
+        k = inv[o:o + len(c)]
+        cnt = np.zeros(len(coords), dtype=np.int64)
+        cnt[k] = n
+        counts.append(cnt)
+        np.minimum.at(fmin, k, np.asarray(f, dtype=np.int64))
+        o += len(c)
+    return coords, counts, fmin
+
+
+def sparse_rows(per, n_spectra):
+    """[(per spectrum (coords, count, first), n) per interval] -> the rows of every spectrum (cells merged over the
+    intervals as merge_intervals + ordered_chains do for dense spectra)"""
+    return [order_entries(*merge_sparse([p[0][k] for p in per])) for k in range(n_spectra)]
+
+
+def write_rows(args, FSpops, rows):
     """one file per spectrum (<pref><pops joined by _><suff>, sfs.py:495-497) or everything to stdout (--pipe, 491-493)"""
     for i, grp in enumerate(FSpops):
-        text = "\n".join("\t".join(str(x) for x in row) for row in ordered_chains(hists[i], firsts[i])) + "\n"
+        text = "\n".join("\t".join(str(x) for x in row) for row in rows[i]) + "\n"
         if args.pipe:
             sys.stdout.write(text)
         else:
             with open(args.pref + "_".join(grp) + args.suff, "w") as out:
                 out.write(text)
+
+
+def write_spectra(args, FSpops, hists, firsts):
+    """dense spectra (one per FSpops entry, or one list per entry over the --regions intervals) -> write_rows"""
+    write_rows(args, FSpops, [ordered_chains(hists[i], firsts[i]) for i in range(len(FSpops))])
+
+
+def use_sparse(groups, dims):
+    """the sparse path exactly where the dense spectra would exceed their limit (engine.SFS_MAX_CELLS in all); decided once
+    per request, so every interval and every rank takes the same path"""
+    return sum(sfs_shapes(groups, dims)[1]) > SFS_MAX_CELLS
 
 
 def parse_region_text(text):
@@ -277,9 +333,12 @@ def main_tables(args, include, exclude):
         table = df[order].to_numpy(dtype=np.int64) if len(df) else np.zeros((0, len(order)), dtype=np.int64)
         kind = "target"
     groups = [tuple(inPopNames.index(pn) for pn in grp) for grp in FSpops]
+    og = len(inPopNames) if outgroup else -1
     with Engine(args.device) as eng:
-        per = [eng.sfs_tables(kind, table, len(inPopNames), groups, outgroup=len(inPopNames) if outgroup else -1, site_mask=m)
-               for m in masks]
+        if use_sparse(groups, sfs_table_dims(kind, table)[1]):
+            per = [eng.sfs_tables_sparse(kind, table, len(inPopNames), groups, outgroup=og, site_mask=m) for m in masks]
+            return write_rows(args, FSpops, sparse_rows(per, len(FSpops)))
+        per = [eng.sfs_tables(kind, table, len(inPopNames), groups, outgroup=og, site_mask=m) for m in masks]
     write_spectra(args, FSpops, *merge_intervals(per, len(FSpops)))
 
 
@@ -378,7 +437,9 @@ def main(argv=None):
         og = len(inPopNames) if outgroup else -1
         sub = subsample_sizes(args, inPopNames)
         if sub is None:
-            per = [eng.sfs(len(inPopNames), groups, sizes, outgroup=og, site_mask=m) for m in masks]
+            sparse = use_sparse(groups, [n + 1 for n in sizes])
+            per = [(eng.sfs_sparse if sparse else eng.sfs)(len(inPopNames), groups, sizes, outgroup=og, site_mask=m)
+                   for m in masks]
         else:
             for pn, n in zip(inPopNames, sub):                            # sfs.py:391-392
                 have = sizes[enginePops.index(pn)]
@@ -388,9 +449,33 @@ def main(argv=None):
             counts = eng.site_counts()
             table, went = downsample_counts(counts, sub, args.seed, considered_sites(masks, len(counts)))
             assert table.max(initial=0) <= 65535
-            per = [eng.sfs_tables("base", table, len(inPopNames), groups, outgroup=og,
-                                  site_mask=went if m is None else (m & went)) for m in masks]
-    if rdv is not None:
+            sparse = use_sparse(groups, sfs_table_dims("base", table)[1])
+            per = [(eng.sfs_tables_sparse if sparse else eng.sfs_tables)("base", table, len(inPopNames), groups, outgroup=og,
+                                                                          site_mask=went if m is None else (m & went))
+                   for m in masks]
+    if rdv is not None and sparse:
+        # the ranks' non-empty cells, first sites made file-wide; rank 0 takes the union (counts summed, first site the
+        # smallest)
+        n_before = int(sum(int(x) for x in rdv.allgather("sfs_sites", np.array(gd.n_sites, dtype=np.int64))[:rdv.rank]))
+        for i, (entries, _) in enumerate(per):
+            for k, (coords, count, first) in enumerate(entries):
+                rdv.put("sfs_c_%d_%d" % (i, k), coords)
+                rdv.put("sfs_n_%d_%d" % (i, k), count)
+                rdv.put("sfs_f_%d_%d" % (i, k), first + n_before)
+        if rdv.rank != 0:
+            rdv.finish()
+            return
+        merged = []
+        for i in range(len(per)):
+            entries = []
+            for k in range(len(FSpops)):
+                parts = [tuple(rdv.get("sfs_%s_%d_%d" % (x, i, k), q) for x in "cnf") for q in range(rdv.world)]
+                coords, counts, first = merge_sparse(parts)
+                entries.append((coords, np.sum(counts, axis=0), first))
+            merged.append((entries, 0))
+        per = merged
+        rdv.finish()
+    elif rdv is not None:
         n_before = int(sum(int(x) for x in rdv.allgather("sfs_sites", np.array(gd.n_sites, dtype=np.int64))[:rdv.rank]))
         for i, (hists, firsts, _) in enumerate(per):
             for k in range(len(FSpops)):
@@ -411,7 +496,10 @@ def main(argv=None):
             merged.append((H, F, 0))
         per = merged
         rdv.finish()
-    write_spectra(args, FSpops, *merge_intervals(per, len(FSpops)))
+    if sparse:
+        write_rows(args, FSpops, sparse_rows(per, len(FSpops)))
+    else:
+        write_spectra(args, FSpops, *merge_intervals(per, len(FSpops)))
 
 
 if __name__ == "__main__":

@@ -77,7 +77,9 @@ extern "C" int pg_ctx_destroy(pg_ctx* ctx) {
     if (ctx->d_geno) cudaFree(ctx->d_geno);
     if (ctx->d_pos) cudaFree(ctx->d_pos);
     PgBuf* bufs[] = {&ctx->tables, &ctx->part, &ctx->segmeta, &ctx->winmeta, &ctx->out_d, &ctx->out_i,
-                     &ctx->planes, &ctx->planes2, &ctx->pairs, &ctx->misc, &ctx->misc2, &ctx->misc3, &ctx->misc4, &ctx->misc5, &ctx->text, &ctx->starts, &ctx->meta};
+                     &ctx->planes, &ctx->planes2, &ctx->pairs, &ctx->misc, &ctx->misc2, &ctx->misc3, &ctx->misc4, &ctx->misc5, &ctx->text, &ctx->starts, &ctx->meta,
+                     &ctx->sfs_acc_k[0], &ctx->sfs_acc_k[1], &ctx->sfs_acc_r[0], &ctx->sfs_acc_r[1], &ctx->sfs_slab,
+                     &ctx->sfs_merge, &ctx->sfs_cub};
     for (PgBuf* b : bufs) b->release();
     for (cudaEvent_t ev : ctx->event_pool) cudaEventDestroy(ev);
     ctx->stage[0].release();

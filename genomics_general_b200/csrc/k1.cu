@@ -15,7 +15,9 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
+#include <cub/cub.cuh>
 
 #include "pgwin_internal.h"
 
@@ -2095,6 +2097,11 @@ extern "C" int pg_site_target_freqs(pg_ctx* ctx, int64_t site0, int64_t n, int32
 // pg_sfs — sfs.py's per-site loop for --inputType genotypes (sfs.py:430-470, getTargetCounts 68-92, SparseFS 94-125)
 // ================================================================================================
 namespace {
+// One non-empty cell of a sparse spectrum (or one site before the reduction): its count and the first site that hit it.
+struct SfsRun {
+    long long count, first;
+};
+
 struct SfsParams {
     const uint16_t* counts;     // [n x P x 4] of this slab
     int64_t n, site0;           // sites of the slab, absolute index of its first site
@@ -2111,35 +2118,29 @@ struct SfsParams {
     unsigned long long* hist;
     long long* first;           // first site (absolute) that hit the cell
     unsigned long long* n_counted;
+    // sparse path (k1_sfs_keys): the slab's counted sites are packed; entry j of spectrum g is at g * key_stride + j
+    unsigned long long* keys;   // dense flat index of the cell
+    SfsRun* runs;               // {1, absolute site}
+    int64_t key_stride;
 };
 
-__global__ void __launch_bounds__(256) k1_sfs(const __grid_constant__ SfsParams sp) {
-    const int64_t s = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    if (s >= sp.n) return;
+// sfs.py's per-site test (430-474), shared by the dense and the sparse path: is site s of the slab counted, and which
+// allele is its target.  target = -1: a targetCounts row (sfs.py:472-474), whose table already holds the counts.
+__device__ __forceinline__ bool sfs_site_target(const SfsParams& sp, int64_t s, int& target) {
     const int64_t site = sp.site0 + s;
-    if (sp.mask && !sp.mask[site]) return;
-    if (sp.targets) {                                                // sfs.py:472-474: the table already holds the counts
-        const int32_t* t = sp.targets + s * sp.P;
-        atomicAdd(sp.n_counted, 1ull);
-        for (int g = 0; g < sp.n_groups; ++g) {
-            long long idx = 0;
-            for (int k = sp.group_off[g]; k < sp.group_off[g + 1]; ++k) idx = idx * sp.dims[sp.group_pops[k]] + t[sp.group_pops[k]];
-            atomicAdd(sp.hist + sp.hist_off[g] + idx, 1ull);
-            atomicMin(sp.first + sp.hist_off[g] + idx, (long long)site);
-        }
-        return;
-    }
+    if (sp.mask && !sp.mask[site]) return false;
+    target = -1;
+    if (sp.targets) return true;
     const ushort4* c = reinterpret_cast<const ushort4*>(sp.counts) + s * sp.P;
     unsigned tot[4] = {0, 0, 0, 0};
     for (int X = 0; X < sp.n_in; ++X) {
         const ushort4 v = c[X];
-        if (sp.require_complete && (int)v.x + v.y + v.z + v.w != sp.popN[X]) return;   // every in-group haplotype called (449)
+        if (sp.require_complete && (int)v.x + v.y + v.z + v.w != sp.popN[X]) return false;   // every in-group haplotype called (449)
         tot[0] += v.x;
         tot[1] += v.y;
         tot[2] += v.z;
         tot[3] += v.w;
     }
-    int target;
     if (sp.outgroup >= 0) {
         const ushort4 o = c[sp.outgroup];
         const unsigned oc[4] = {o.x, o.y, o.z, o.w};
@@ -2148,43 +2149,99 @@ __global__ void __launch_bounds__(256) k1_sfs(const __grid_constant__ SfsParams 
             n_all += (tot[a] > 0 || oc[a] > 0) ? 1 : 0;
             n_out += oc[a] > 0 ? 1 : 0;
         }
-        if (n_all < 1 || n_all > 2) return;                          // 79
+        if (n_all < 1 || n_all > 2) return false;                    // 79
         // `outgroupMono & nOutAlleles != 1` is (outgroupMono & nOutAlleles) != 1: the count must be odd, i.e. 1 (84)
-        if (n_out == 0 || (n_out & 1) != 1) return;
-        target = -1;
+        if (n_out == 0 || (n_out & 1) != 1) return false;
         for (int a = 3; a >= 0; --a)
             if (tot[a] > 0 && oc[a] == 0) target = a;               // first in-group allele the outgroup lacks (86)
         if (target < 0)
             for (int a = 3; a >= 0; --a)
                 if (tot[a] == 0) target = a;                         // invariant: first absent allele (87), count 0
-        if (target < 0) return;
-    } else {
-        int n_all = 0;
-        for (int a = 0; a < 4; ++a) n_all += tot[a] > 0 ? 1 : 0;
-        if (n_all < 1 || n_all > 2) return;
-        // totalBaseCounts.argsort()[-2] (90): second in a stable ascending order = with two alleles the rarer one, the
-        // lower allele on an exact tie; with one allele an absent allele (count 0 everywhere)
-        int best = -1, second = -1;                                  // positions [-1] and [-2] of the stable argsort
-        for (int a = 0; a < 4; ++a) {
-            if (best < 0 || tot[a] >= tot[best]) {
-                second = best;
-                best = a;
-            } else if (second < 0 || tot[a] >= tot[second]) second = a;
-        }
-        target = second;
+        return target >= 0;
     }
+    int n_all = 0;
+    for (int a = 0; a < 4; ++a) n_all += tot[a] > 0 ? 1 : 0;
+    if (n_all < 1 || n_all > 2) return false;
+    // totalBaseCounts.argsort()[-2] (90): second in a stable ascending order = with two alleles the rarer one, the
+    // lower allele on an exact tie; with one allele an absent allele (count 0 everywhere)
+    int best = -1, second = -1;                                      // positions [-1] and [-2] of the stable argsort
+    for (int a = 0; a < 4; ++a) {
+        if (best < 0 || tot[a] >= tot[best]) {
+            second = best;
+            best = a;
+        } else if (second < 0 || tot[a] >= tot[second]) second = a;
+    }
+    target = second;
+    return true;
+}
+
+// Row-major mixed-radix index of the site's cell in spectrum g: the dense histogram's flat index, and the sparse key.
+__device__ __forceinline__ long long sfs_cell(const SfsParams& sp, int64_t s, int target, int g) {
+    long long idx = 0;
+    if (target < 0) {
+        const int32_t* t = sp.targets + s * sp.P;
+        for (int k = sp.group_off[g]; k < sp.group_off[g + 1]; ++k) idx = idx * sp.dims[sp.group_pops[k]] + t[sp.group_pops[k]];
+        return idx;
+    }
+    const ushort4* c = reinterpret_cast<const ushort4*>(sp.counts) + s * sp.P;
+    for (int k = sp.group_off[g]; k < sp.group_off[g + 1]; ++k) {
+        const int X = sp.group_pops[k];
+        const ushort4 v = c[X];
+        const unsigned t = target == 0 ? v.x : (target == 1 ? v.y : (target == 2 ? v.z : v.w));
+        idx = idx * sp.dims[X] + t;
+    }
+    return idx;
+}
+
+__global__ void __launch_bounds__(256) k1_sfs(const __grid_constant__ SfsParams sp) {
+    const int64_t s = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (s >= sp.n) return;
+    int target;
+    if (!sfs_site_target(sp, s, target)) return;
+    const int64_t site = sp.site0 + s;
     atomicAdd(sp.n_counted, 1ull);
     for (int g = 0; g < sp.n_groups; ++g) {
-        long long idx = 0;
-        for (int k = sp.group_off[g]; k < sp.group_off[g + 1]; ++k) {
-            const int X = sp.group_pops[k];
-            const ushort4 v = c[X];
-            const unsigned t = target == 0 ? v.x : (target == 1 ? v.y : (target == 2 ? v.z : v.w));
-            idx = idx * sp.dims[X] + t;
-        }
+        const long long idx = sfs_cell(sp, s, target, g);
         atomicAdd(sp.hist + sp.hist_off[g] + idx, 1ull);
         atomicMin(sp.first + sp.hist_off[g] + idx, (long long)site);
     }
+}
+
+// Sparse path: every counted site of the slab writes its cell of every spectrum as a (key, {1, site}) entry.  The
+// entries are packed by a warp-aggregated counter (n_counted, zeroed per slab), so their order within the slab is that of
+// the atomics; the reduction that follows sums counts and takes the minimum site, which no order changes.
+__global__ void __launch_bounds__(256) k1_sfs_keys(const __grid_constant__ SfsParams sp) {
+    const int64_t s = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    int target = -1;
+    const bool ok = s < sp.n && sfs_site_target(sp, s, target);
+    const unsigned m = __ballot_sync(0xffffffffu, ok);
+    if (m == 0) return;
+    const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
+    unsigned long long base = 0;
+    if (lane == leader) base = atomicAdd(sp.n_counted, (unsigned long long)__popc(m));
+    base = __shfl_sync(0xffffffffu, base, leader);
+    if (!ok) return;
+    const int64_t j = (int64_t)base + __popc(m & ((1u << lane) - 1u));
+    const long long site = sp.site0 + s;
+    for (int g = 0; g < sp.n_groups; ++g) {
+        sp.keys[g * sp.key_stride + j] = (unsigned long long)sfs_cell(sp, s, target, g);
+        sp.runs[g * sp.key_stride + j] = SfsRun{1, site};
+    }
+}
+
+struct SfsRunMerge {
+    __device__ __forceinline__ SfsRun operator()(const SfsRun& a, const SfsRun& b) const {
+        return SfsRun{a.count + b.count, a.first < b.first ? a.first : b.first};
+    }
+};
+
+__global__ void sfs_runs_split(const SfsRun* __restrict__ runs, int64_t n, long long* __restrict__ count,
+                               long long* __restrict__ first) {
+    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    const SfsRun r = runs[i];
+    count[i] = r.count;
+    first[i] = r.first;
 }
 }  // namespace
 
@@ -2381,5 +2438,258 @@ extern "C" int pg_sfs_tables(pg_ctx* ctx, int32_t kind, const void* table, int64
     for (long long k = 0; k < cells; ++k)
         if (hist[k] == 0) first[k] = -1;
     if (n_counted) *n_counted = (int64_t)h_cnt;
+    return PG_OK;
+}
+
+// ================================================================================================
+// Sparse spectra — sfs.py's SparseFS (94-125) without a dense histogram: pg_sfs_sparse / pg_sfs_tables_sparse / _fetch
+// ================================================================================================
+// Per slab, k1_sfs_keys packs one (cell, {1, site}) entry per counted site and spectrum.  Each spectrum's entries are
+// appended to the runs it has so far, radix-sorted on the bits its cell count needs and reduced by cell (counts summed,
+// the smallest site kept), so after every slab a spectrum holds at most one run per non-empty cell, cells ascending.
+namespace {
+// bits of the largest cell index of a spectrum of `cells` cells: the radix sort's end_bit
+int sfs_key_bits(long long cells) {
+    int b = 1;
+    while (b < 63 && (1ll << b) < cells) ++b;
+    return b;
+}
+
+// Π dims of every spectrum, refused when one does not fit in 63 bits (the cell index is an int64)
+int sfs_sparse_cells(const char* who, int32_t n_groups, const int32_t* group_off, const int32_t* group_pops, int32_t n_in,
+                     const int32_t* dims, std::vector<long long>& cells) {
+    cells.assign(n_groups, 1);
+    for (int g = 0; g < n_groups; ++g) {
+        PG_CHECK(group_off[g + 1] > group_off[g], "%s: spectrum %d has no population", who, g);
+        long long sz = 1;
+        for (int k = group_off[g]; k < group_off[g + 1]; ++k) {
+            PG_CHECK(group_pops[k] >= 0 && group_pops[k] < n_in, "%s: spectrum %d uses a population outside the in-group", who, g);
+            const long long d = dims[group_pops[k]];
+            PG_CHECK(d >= 1, "%s: dims must be >= 1", who);
+            PG_CHECK(sz <= LLONG_MAX / d, "%s: spectrum %d has more than 2^63 - 1 cells (the product of its populations' "
+                     "largest counts + 1); its cell index does not fit in 64 bits", who, g);
+            sz *= d;
+        }
+        cells[g] = sz;
+    }
+    return PG_OK;
+}
+
+// Sites per slab: the dense path's slab, cut so that the entries of all spectra stay at most 2^25 (24 bytes each, about
+// 0.8 GB); PG_SFS_SPARSE_SLAB caps it further (tests put slab seams into small inputs with it).
+int64_t sfs_sparse_slab(int64_t dense_slab, int n_groups) {
+    int64_t slab = std::max<int64_t>(1, std::min<int64_t>(dense_slab, ((int64_t)1 << 25) / n_groups));
+    if (const char* e = getenv("PG_SFS_SPARSE_SLAB")) slab = std::max<int64_t>(1, std::min<int64_t>(slab, atoll(e)));
+    return slab;
+}
+
+// The pass shared by genotypes and tables.  `sp` carries everything but the slab fields; load(s0, cnt) puts the slab's
+// rows where sp.counts / sp.targets point.
+template <typename Load>
+int sfs_sparse_pass(pg_ctx* ctx, SfsParams sp, int64_t n_sites, int64_t slab, const std::vector<long long>& cells, Load load,
+                    int64_t* nnz, int64_t* n_counted) {
+    const int G = sp.n_groups;
+    std::vector<int64_t> len(G, 0), off(G, 0);                      // runs of each spectrum in sfs_acc_*[cur], group-major
+    int cur = 0;
+    int64_t total = 0, counted = 0;
+    const size_t slab_keys = align_up((size_t)slab * G * 8, 16);
+    PG_TRY(ctx->sfs_slab.ensure(slab_keys + (size_t)slab * G * sizeof(SfsRun) + 64));
+    unsigned long long* d_keys = (unsigned long long*)ctx->sfs_slab.p;
+    SfsRun* d_runs = (SfsRun*)((uint8_t*)ctx->sfs_slab.p + slab_keys);
+    PG_TRY(ctx->out_i.ensure(64));
+    unsigned long long* d_cnt = (unsigned long long*)ctx->out_i.p;
+    int* d_nruns = (int*)(d_cnt + 1);
+    for (int64_t s0 = 0; s0 < n_sites; s0 += slab) {
+        const int64_t cnt = std::min(slab, n_sites - s0);
+        PG_TRY(load(s0, cnt));
+        PG_CUDA(cudaMemsetAsync(d_cnt, 0, 8, ctx->stream));
+        sp.n = cnt;
+        sp.site0 = s0;
+        sp.keys = d_keys;
+        sp.runs = d_runs;
+        sp.key_stride = slab;
+        sp.n_counted = d_cnt;
+        const int ti = pg_time_begin(ctx, "k1_sfs_keys");
+        k1_sfs_keys<<<(unsigned)((cnt + 255) / 256), 256, 0, ctx->stream>>>(sp);
+        pg_time_end(ctx, ti);
+        PG_CUDA(cudaGetLastError());
+        unsigned long long h_m = 0;
+        PG_CUDA(cudaMemcpyAsync(&h_m, d_cnt, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        PG_CUDA(cudaStreamSynchronize(ctx->stream));                 // also frees the slab's rows for the next load
+        const int64_t m = (int64_t)h_m;
+        counted += m;
+        if (m == 0) continue;
+        const int nxt = cur ^ 1;
+        PG_TRY(ctx->sfs_acc_k[nxt].ensure((size_t)(total + m * G) * 8 + 64));
+        PG_TRY(ctx->sfs_acc_r[nxt].ensure((size_t)(total + m * G) * sizeof(SfsRun) + 64));
+        unsigned long long* out_k = (unsigned long long*)ctx->sfs_acc_k[nxt].p;
+        SfsRun* out_r = (SfsRun*)ctx->sfs_acc_r[nxt].p;
+        int64_t o = 0;
+        for (int g = 0; g < G; ++g) {
+            const int64_t n = len[g] + m;
+            PG_CHECK(n < INT_MAX, "pg_sfs_sparse: spectrum %d holds more than 2^31 entries in one merge", g);
+            const size_t part_k = align_up((size_t)n * 8, 16), part = part_k + (size_t)n * sizeof(SfsRun);
+            PG_TRY(ctx->sfs_merge.ensure(2 * part + 64));
+            uint8_t* mb = (uint8_t*)ctx->sfs_merge.p;
+            unsigned long long *a_k = (unsigned long long*)mb, *b_k = (unsigned long long*)(mb + part);
+            SfsRun *a_r = (SfsRun*)(mb + part_k), *b_r = (SfsRun*)(mb + part + part_k);
+            const unsigned long long* in_k = d_keys + (size_t)g * slab;
+            const SfsRun* in_r = d_runs + (size_t)g * slab;
+            if (len[g] > 0) {                                        // the runs so far, then this slab's entries
+                const unsigned long long* acc_k = (const unsigned long long*)ctx->sfs_acc_k[cur].p + off[g];
+                const SfsRun* acc_r = (const SfsRun*)ctx->sfs_acc_r[cur].p + off[g];
+                PG_CUDA(cudaMemcpyAsync(a_k, acc_k, (size_t)len[g] * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+                PG_CUDA(cudaMemcpyAsync(a_k + len[g], in_k, (size_t)m * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+                PG_CUDA(cudaMemcpyAsync(a_r, acc_r, (size_t)len[g] * sizeof(SfsRun), cudaMemcpyDeviceToDevice, ctx->stream));
+                PG_CUDA(cudaMemcpyAsync(a_r + len[g], in_r, (size_t)m * sizeof(SfsRun), cudaMemcpyDeviceToDevice, ctx->stream));
+                in_k = a_k;
+                in_r = a_r;
+            }
+            const int bits = sfs_key_bits(cells[g]);
+            size_t t_sort = 0, t_red = 0;
+            PG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, in_k, b_k, in_r, b_r, (int)n, 0, bits, ctx->stream));
+            PG_CUDA(cub::DeviceReduce::ReduceByKey(nullptr, t_red, b_k, out_k + o, b_r, out_r + o, d_nruns, SfsRunMerge(),
+                                                   (int)n, ctx->stream));
+            PG_TRY(ctx->sfs_cub.ensure(std::max(t_sort, t_red) + 64));
+            int ti2 = pg_time_begin(ctx, "sfs_sort");
+            PG_CUDA(cub::DeviceRadixSort::SortPairs(ctx->sfs_cub.p, t_sort, in_k, b_k, in_r, b_r, (int)n, 0, bits, ctx->stream));
+            pg_time_end(ctx, ti2);
+            ti2 = pg_time_begin(ctx, "sfs_reduce");
+            PG_CUDA(cub::DeviceReduce::ReduceByKey(ctx->sfs_cub.p, t_red, b_k, out_k + o, b_r, out_r + o, d_nruns, SfsRunMerge(),
+                                                   (int)n, ctx->stream));
+            pg_time_end(ctx, ti2);
+            int h_runs = 0;
+            PG_CUDA(cudaMemcpyAsync(&h_runs, d_nruns, 4, cudaMemcpyDeviceToHost, ctx->stream));
+            PG_CUDA(cudaStreamSynchronize(ctx->stream));             // scratch may be regrown for the next spectrum
+            off[g] = o;
+            len[g] = h_runs;
+            o += h_runs;
+        }
+        total = o;
+        cur = nxt;
+    }
+    for (int g = 0; g < G; ++g) nnz[g] = len[g];
+    if (n_counted) *n_counted = counted;
+    ctx->sfs_cur = cur;
+    ctx->sfs_total = total;
+    return PG_OK;
+}
+
+// group tables and site mask on the device, as pg_sfs / pg_sfs_tables put them
+int sfs_sparse_tables(pg_ctx* ctx, int32_t n_groups, const int32_t* group_off, const int32_t* group_pops,
+                      const uint8_t* site_mask, int64_t n_mask, SfsParams& sp) {
+    const int n_gp = group_off[n_groups];
+    PG_TRY(ctx->misc2.ensure((size_t)(n_groups + 1) * 4 + (size_t)n_gp * 4 + 128));
+    uint8_t* tb = (uint8_t*)ctx->misc2.p;
+    size_t o = 0;
+    int32_t* d_goff = nullptr;
+    int32_t* d_gpops = nullptr;
+    PG_TRY(push(ctx, tb, o, group_off, (size_t)n_groups + 1, &d_goff));
+    PG_TRY(push(ctx, tb, o, group_pops, (size_t)n_gp, &d_gpops));
+    sp.n_groups = n_groups;
+    sp.group_off = d_goff;
+    sp.group_pops = d_gpops;
+    sp.mask = nullptr;
+    if (site_mask && n_mask > 0) {
+        PG_TRY(ctx->misc3.ensure((size_t)n_mask + 64));
+        sp.mask = (uint8_t*)ctx->misc3.p;
+        PG_CUDA(cudaMemcpyAsync(ctx->misc3.p, site_mask, (size_t)n_mask, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));                     // host tables behind the async copies
+    return PG_OK;
+}
+}  // namespace
+
+extern "C" int pg_sfs_sparse(pg_ctx* ctx, int32_t n_in, int32_t outgroup, int32_t n_groups, const int32_t* group_off,
+                             const int32_t* group_pops, const uint8_t* site_mask, int64_t* nnz, int64_t* n_counted) {
+    PG_CHECK(ctx && group_off && group_pops && nnz, "pg_sfs_sparse: null argument");
+    ctx->sfs_total = -1;
+    PG_CHECK(ctx->P >= 1 && ctx->P <= PG_MAX_POPS, "pg_sfs_sparse: call pg_set_pops first (at most %d populations)", PG_MAX_POPS);
+    PG_CHECK(n_in >= 1 && n_in <= ctx->P, "pg_sfs_sparse: n_in out of range");
+    PG_CHECK(outgroup == -1 || (outgroup >= n_in && outgroup < ctx->P),
+             "pg_sfs_sparse: the outgroup must be a population after the in-group");
+    PG_CHECK(n_groups >= 1, "pg_sfs_sparse: no spectra requested");
+    const int P = ctx->P;
+    std::vector<int> popN(P, 0), dims(P, 0);
+    for (int h = 0; h < ctx->H; ++h)
+        if (ctx->hap_pop[h] >= 0) popN[ctx->hap_pop[h]] += 1;
+    for (int X = 0; X < P; ++X) dims[X] = popN[X] + 1;
+    std::vector<long long> cells;
+    PG_TRY(sfs_sparse_cells("pg_sfs_sparse", n_groups, group_off, group_pops, n_in, dims.data(), cells));
+    PG_CUDA(cudaSetDevice(ctx->device));
+    pg_timings_reset(ctx);
+    SfsParams sp;
+    memset(&sp, 0, sizeof(sp));
+    PG_TRY(sfs_sparse_tables(ctx, n_groups, group_off, group_pops, site_mask, ctx->S, sp));
+    sp.P = P;
+    sp.n_in = n_in;
+    sp.outgroup = outgroup;
+    for (int X = 0; X < P; ++X) {
+        sp.popN[X] = popN[X];
+        sp.dims[X] = dims[X];
+    }
+    sp.require_complete = 1;
+    const int64_t stride = (int64_t)P * 4;
+    const int64_t slab = sfs_sparse_slab((int64_t)(1ll << 28) / (stride * 2), n_groups);
+    PG_TRY(ctx->misc.ensure((size_t)std::min<int64_t>(slab, std::max<int64_t>(ctx->S, 1)) * stride * 2 + 64));
+    sp.counts = (const uint16_t*)ctx->misc.p;
+    return sfs_sparse_pass(ctx, sp, ctx->S, slab, cells, [&](int64_t s0, int64_t cnt) { return site_counts_slab(ctx, s0, cnt); },
+                           nnz, n_counted);
+}
+
+extern "C" int pg_sfs_tables_sparse(pg_ctx* ctx, int32_t kind, const void* table, int64_t n, int32_t P, const int32_t* dims,
+                                    int32_t n_in, int32_t outgroup, int32_t n_groups, const int32_t* group_off,
+                                    const int32_t* group_pops, const uint8_t* site_mask, int64_t* nnz, int64_t* n_counted) {
+    PG_CHECK(ctx && (table || n == 0) && dims && group_off && group_pops && nnz, "pg_sfs_tables_sparse: null argument");
+    ctx->sfs_total = -1;
+    PG_CHECK(kind == 0 || kind == 1, "pg_sfs_tables_sparse: kind must be 0 (base counts) or 1 (target counts)");
+    PG_CHECK(P >= 1 && P <= PG_MAX_POPS, "pg_sfs_tables_sparse: at most %d populations", PG_MAX_POPS);
+    PG_CHECK(n_in >= 1 && n_in <= P && n >= 0, "pg_sfs_tables_sparse: bad shape");
+    PG_CHECK(outgroup == -1 || (kind == 0 && outgroup >= n_in && outgroup < P), "pg_sfs_tables_sparse: bad outgroup");
+    PG_CHECK(n_groups >= 1, "pg_sfs_tables_sparse: no spectra requested");
+    std::vector<long long> cells;
+    PG_TRY(sfs_sparse_cells("pg_sfs_tables_sparse", n_groups, group_off, group_pops, n_in, dims, cells));
+    PG_CUDA(cudaSetDevice(ctx->device));
+    pg_timings_reset(ctx);
+    SfsParams sp;
+    memset(&sp, 0, sizeof(sp));
+    PG_TRY(sfs_sparse_tables(ctx, n_groups, group_off, group_pops, site_mask, n, sp));
+    const size_t row_bytes = kind == 0 ? (size_t)P * 8 : (size_t)P * 4;
+    const int64_t slab = sfs_sparse_slab((int64_t)(((size_t)256 << 20) / row_bytes), n_groups);
+    PG_TRY(ctx->misc.ensure((size_t)std::min<int64_t>(slab, std::max<int64_t>(n, 1)) * row_bytes + 64));
+    sp.counts = kind == 0 ? (const uint16_t*)ctx->misc.p : nullptr;
+    sp.targets = kind == 1 ? (const int32_t*)ctx->misc.p : nullptr;
+    sp.P = P;
+    sp.n_in = n_in;
+    sp.outgroup = outgroup;
+    for (int X = 0; X < P; ++X) sp.dims[X] = dims[X];
+    sp.require_complete = 0;
+    auto load = [&](int64_t s0, int64_t cnt) {
+        PG_CUDA(cudaMemcpyAsync(ctx->misc.p, (const uint8_t*)table + (size_t)s0 * row_bytes, (size_t)cnt * row_bytes,
+                                cudaMemcpyHostToDevice, ctx->stream));
+        return PG_OK;
+    };
+    return sfs_sparse_pass(ctx, sp, n, slab, cells, load, nnz, n_counted);
+}
+
+extern "C" int pg_sfs_sparse_fetch(pg_ctx* ctx, int64_t total, int64_t* cell, int64_t* count, int64_t* first) {
+    PG_CHECK(ctx, "pg_sfs_sparse_fetch: null argument");
+    PG_CHECK(ctx->sfs_total >= 0, "pg_sfs_sparse_fetch: no sparse spectra pending (already fetched, or the pass failed)");
+    PG_CHECK(total == ctx->sfs_total, "pg_sfs_sparse_fetch: %lld entries requested, the pending spectra hold %lld",
+             (long long)total, (long long)ctx->sfs_total);
+    PG_CHECK(total == 0 || (cell && count && first), "pg_sfs_sparse_fetch: null argument");
+    PG_CUDA(cudaSetDevice(ctx->device));
+    ctx->sfs_total = -1;                                             // fetched once
+    if (total == 0) return PG_OK;
+    const int cur = ctx->sfs_cur;
+    PG_TRY(ctx->sfs_merge.ensure((size_t)total * 16 + 64));
+    long long* d_count = (long long*)ctx->sfs_merge.p;
+    long long* d_first = d_count + total;
+    sfs_runs_split<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>((const SfsRun*)ctx->sfs_acc_r[cur].p, total,
+                                                                            d_count, d_first);
+    PG_CUDA(cudaGetLastError());
+    PG_TRY(pg_d2h_staged(ctx, cell, ctx->sfs_acc_k[cur].p, (size_t)total * 8));
+    PG_TRY(pg_d2h_staged(ctx, count, d_count, (size_t)total * 8));
+    PG_TRY(pg_d2h_staged(ctx, first, d_first, (size_t)total * 8));
     return PG_OK;
 }

@@ -136,6 +136,12 @@ struct pg_ctx {
     uint64_t gslot_gen[2] = {0, 0};
     void* h_pinned = nullptr;                 // small pinned staging for result read-back
     size_t h_pinned_cap = 0;
+    // sparse spectra (pg_sfs_sparse / pg_sfs_tables_sparse, k1.cu): the runs accumulated so far (keys + {count, first})
+    // and the next merge's output, the slab's entries, the merge and CUB scratch.  The result waits in
+    // sfs_acc_*[sfs_cur] until pg_sfs_sparse_fetch; sfs_total = its entries, -1 = none pending.
+    PgBuf sfs_acc_k[2], sfs_acc_r[2], sfs_slab, sfs_merge, sfs_cub;
+    int sfs_cur = 0;
+    int64_t sfs_total = -1;
 };
 
 // timing helpers: every kernel launch is bracketed by events on ctx->stream

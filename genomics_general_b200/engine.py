@@ -55,6 +55,45 @@ def _check_sfs_cells(cells):
                       "fewer joint spectra per run, or --subsample smaller populations)" % (sum(cells), SFS_MAX_CELLS))
 
 
+def sfs_shapes(groups, dims):
+    """spectrum shapes (dims of each group's populations) and their cell counts (Python ints: no overflow)"""
+    shapes = [tuple(int(dims[x]) for x in grp) for grp in groups]
+    return shapes, [int(np.prod([int(d) for d in sh], dtype=object)) for sh in shapes]
+
+
+def sfs_table_dims(kind, table):
+    """the table as the engine reads it (uint16 [n,P,4] base counts | int32 [n,P] target counts) and the radix of every
+    population: its largest count + 1"""
+    if kind == "base":
+        table = np.ascontiguousarray(table, dtype=np.uint16)
+        n, P = table.shape[0], table.shape[1]
+        dims = (table.sum(axis=2, dtype=np.int64).max(axis=0) + 1 if n else np.ones(P, np.int64)).astype(np.int32)
+    else:
+        table = np.ascontiguousarray(table, dtype=np.int32)
+        n, P = table.shape
+        dims = (table.max(axis=0) + 1 if n else np.ones(P, np.int64)).astype(np.int32)
+        assert n == 0 or table.min() >= 0
+    return table, dims
+
+
+def _sfs_group_tables(groups):
+    goff = np.zeros(len(groups) + 1, dtype=np.int32)
+    for k, grp in enumerate(groups):
+        goff[k + 1] = goff[k] + len(grp)
+    return goff, np.array([x for grp in groups for x in grp], dtype=np.int32)
+
+
+def sfs_unravel(cell, shape):
+    """row-major flat cell indices -> int64 coordinates [n, len(shape)]"""
+    cell = np.asarray(cell, dtype=np.int64)
+    coords = np.empty((len(cell), len(shape)), dtype=np.int64)
+    rest = cell.copy()
+    for j in range(len(shape) - 1, -1, -1):
+        coords[:, j] = rest % shape[j]
+        rest //= shape[j]
+    return coords
+
+
 class Engine:
     def __init__(self, device: int = 0):
         self._lib = _lib.lib()
@@ -393,6 +432,45 @@ class Engine:
         offs = np.concatenate([[0], np.cumsum(cells)])
         return ([hist[offs[k]:offs[k + 1]].reshape(shapes[k]) for k in range(len(groups))],
                 [first[offs[k]:offs[k + 1]].reshape(shapes[k]) for k in range(len(groups))], int(cnt.value))
+
+    def _sfs_sparse_fetch(self, nnz, shapes):
+        total = int(nnz.sum())
+        cell = np.empty(total, dtype=np.int64)
+        count = np.empty(total, dtype=np.int64)
+        first = np.empty(total, dtype=np.int64)
+        check(self._lib.pg_sfs_sparse_fetch(self._ctx, total, _ptr(cell), _ptr(count), _ptr(first)), "pg_sfs_sparse_fetch")
+        offs = np.concatenate([[0], np.cumsum(nnz)])
+        return [(sfs_unravel(cell[offs[k]:offs[k + 1]], shapes[k]), count[offs[k]:offs[k + 1]], first[offs[k]:offs[k + 1]])
+                for k in range(len(shapes))]
+
+    def sfs_sparse(self, n_in: int, groups, pop_sizes, outgroup: int = -1, site_mask=None):
+        """sfs() without dense histograms (any number of cells): returns (per spectrum (coords int64 [nnz, d], count int64
+        [nnz], first site int64 [nnz]) with cells in row-major order, sites counted)."""
+        goff, gp = _sfs_group_tables(groups)
+        shapes, _ = sfs_shapes(groups, [int(x) + 1 for x in pop_sizes])
+        mask = None if site_mask is None else np.ascontiguousarray(site_mask, dtype=np.uint8)
+        if mask is not None:
+            assert mask.shape == (self.S,)
+        nnz = np.zeros(len(groups), dtype=np.int64)
+        n = C.c_int64(0)
+        check(self._lib.pg_sfs_sparse(self._ctx, int(n_in), int(outgroup), len(groups), _ptr(goff), _ptr(gp), _ptr(mask),
+                                      _ptr(nnz), C.byref(n)), "pg_sfs_sparse")
+        return self._sfs_sparse_fetch(nnz, shapes), int(n.value)
+
+    def sfs_tables_sparse(self, kind: str, table, n_in: int, groups, outgroup: int = -1, site_mask=None):
+        """sfs_tables() without dense histograms: returns (per spectrum (coords, count, first) as sfs_sparse(), sites
+        counted)."""
+        table, dims = sfs_table_dims(kind, table)
+        n, P = table.shape[0], table.shape[1]
+        goff, gp = _sfs_group_tables(groups)
+        shapes, _ = sfs_shapes(groups, dims)
+        mask = None if site_mask is None else np.ascontiguousarray(site_mask, dtype=np.uint8)
+        nnz = np.zeros(len(groups), dtype=np.int64)
+        cnt = C.c_int64(0)
+        check(self._lib.pg_sfs_tables_sparse(self._ctx, 0 if kind == "base" else 1, _ptr(table), int(n), int(P), _ptr(dims),
+                                             int(n_in), int(outgroup), len(groups), _ptr(goff), _ptr(gp), _ptr(mask),
+                                             _ptr(nnz), C.byref(cnt)), "pg_sfs_tables_sparse")
+        return self._sfs_sparse_fetch(nnz, shapes), int(cnt.value)
 
     def pairdist(self, hap_ind, n_ind: int, include_same_with_same: bool = False, min_sites: int = 0, out=None):
         """-> dict(dist [W,n_ind,n_ind], sites [W], pos_sum [W]).  min_sites > 0 masks haplotype pairs with fewer

@@ -126,7 +126,8 @@ int pg_site_target_freqs(pg_ctx* ctx, int64_t site0, int64_t n, int32_t target, 
  * on numpy's sort, here the lower allele).  Spectrum g is over the populations group_pops[group_off[g] .. group_off[g+1]);
  * hist holds the spectra one after the other as dense row-major arrays of prod(N_k + 1) cells, first[cell] = index of
  * the first site that hit the cell (-1 = empty; gives the reference's first-appearance output order).
- * site_mask (may be NULL): only sites with mask 1 are counted (--include / --exclude). */
+ * site_mask (may be NULL): only sites with mask 1 are counted (--include / --exclude).
+ * The dense histograms are limited to 2^28 cells in total (PG_ERR above); pg_sfs_sparse has no such limit. */
 int pg_sfs(pg_ctx* ctx, int32_t n_in, int32_t outgroup, int32_t n_groups, const int32_t* group_off,
            const int32_t* group_pops, const uint8_t* site_mask, int64_t* hist, int64_t* first, int64_t* n_counted);
 
@@ -137,6 +138,21 @@ int pg_sfs(pg_ctx* ctx, int32_t n_in, int32_t outgroup, int32_t n_groups, const 
 int pg_sfs_tables(pg_ctx* ctx, int32_t kind, const void* table, int64_t n, int32_t P, const int32_t* dims, int32_t n_in,
                   int32_t outgroup, int32_t n_groups, const int32_t* group_off, const int32_t* group_pops,
                   const uint8_t* site_mask, int64_t* hist, int64_t* first, int64_t* n_counted);
+
+/* Sparse spectra: the same per-site logic as pg_sfs / pg_sfs_tables (same arguments), kept the way sfs.py's nested
+ * SparseFS dicts keep them (sfs.py:94-125, 484-487) — only the non-empty cells, so no limit on the cells of a spectrum
+ * other than that prod(dims) of each must fit in 63 bits (PG_ERR before any launch, naming the spectrum).  Device memory
+ * grows with the sites counted, not with the cells.  nnz[g] receives the non-empty cells of spectrum g; the cells
+ * themselves stay in a buffer of the context until pg_sfs_sparse_fetch copies them out: total = sum(nnz), group-major,
+ * cells ascending within a spectrum, cell = the dense row-major flat index pg_sfs would use, count = its sites,
+ * first = the first site that hit it (the reference's first-appearance order).  A result is fetched once; the next
+ * sparse call replaces a pending one, and fetch fails (PG_ERR) when total does not match or nothing is pending. */
+int pg_sfs_sparse(pg_ctx* ctx, int32_t n_in, int32_t outgroup, int32_t n_groups, const int32_t* group_off,
+                  const int32_t* group_pops, const uint8_t* site_mask, int64_t* nnz, int64_t* n_counted);
+int pg_sfs_tables_sparse(pg_ctx* ctx, int32_t kind, const void* table, int64_t n, int32_t P, const int32_t* dims,
+                         int32_t n_in, int32_t outgroup, int32_t n_groups, const int32_t* group_off,
+                         const int32_t* group_pops, const uint8_t* site_mask, int64_t* nnz, int64_t* n_counted);
+int pg_sfs_sparse_fetch(pg_ctx* ctx, int64_t total, int64_t* cell, int64_t* count, int64_t* first);
 
 /* Replaces Alignment.indPairDists (genomics.py:934-954) as used by distMat.py:42-45 and popgenWindows.py:54-57.
  * hap_ind[h] = individual index in [0,n_ind) or -1; dist [W x n_ind x n_ind]; n_sites/pos_sum [W] (may be NULL).
