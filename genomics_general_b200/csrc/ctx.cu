@@ -75,6 +75,7 @@ extern "C" int pg_ctx_destroy(pg_ctx* ctx) {
     ctx->gather.release();
     ctx->gather_flag.release();
     if (ctx->d_geno) cudaFree(ctx->d_geno);
+    if (ctx->d_packed) cudaFree(ctx->d_packed);
     if (ctx->d_pos) cudaFree(ctx->d_pos);
     PgBuf* bufs[] = {&ctx->tables, &ctx->part, &ctx->segmeta, &ctx->winmeta, &ctx->out_d, &ctx->out_i,
                      &ctx->planes, &ctx->planes2, &ctx->pairs, &ctx->misc, &ctx->misc2, &ctx->misc3, &ctx->misc4, &ctx->misc5, &ctx->text, &ctx->starts, &ctx->meta,
@@ -275,9 +276,13 @@ static int env_int(const char* name, int dflt) {
 // (T consecutive sites) at a time, so up to 8/wpt tiles are being consumed while `stages` tiles sit in the
 // TMA ring.  G lanes share one site row when a row is too long for one lane's tile share.
 K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw, int force_G) {
+    return pg_make_k1_plan_rows(S, pg_pitch_for(H), sm_count, table_bytes, nw, force_G);
+}
+
+K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G) {
     K1Plan p;
     memset(&p, 0, sizeof(p));
-    p.pitch = pg_pitch_for(H);
+    p.pitch = pitch;
     p.chunks = p.pitch / 16;
     const int smem_cap = 227 * 1024 - 2048 - table_bytes;   // per-CTA dynamic smem we allow ourselves
     const int tile_target = env_int("PG_K1_TILE_KB", 64) * 1024;
@@ -413,15 +418,29 @@ extern "C" int pg_alloc_sites(pg_ctx* ctx, int64_t S, int32_t H) {
         PG_CUDA(cudaMalloc((void**)&ctx->d_pos, pneed));
         ctx->pos_cap = pneed;
     }
+    const int ppitch = pg_packed_pitch_for(H);
+    const size_t kneed = (size_t)(S + 64) * ppitch + 4096;
+    if (kneed > ctx->packed_cap) {
+        if (ctx->d_packed) cudaFree(ctx->d_packed);
+        ctx->d_packed = nullptr;
+        ctx->packed_cap = 0;
+        if (cudaMalloc((void**)&ctx->d_packed, kneed) == cudaSuccess) ctx->packed_cap = kneed;
+        else {                                 // no companion: the popgen site pass reads the one-hot bytes
+            ctx->d_packed = nullptr;
+            cudaGetLastError();
+        }
+    }
     const bool same_shape = (ctx->S == S && ctx->H == H && ctx->pitch == pitch);
     ctx->S = S;
     ctx->H = H;
     ctx->pitch = pitch;
+    ctx->packed_pitch = ppitch;
     if (!same_shape) ctx->epoch += 1;          // same shape: cached launch plans stay valid
     ctx->data_gen += 1;                        // (synth_fill and the text ingest come through here too)
     PG_CUDA(cudaMemsetAsync(ctx->d_pos, 0, pneed, ctx->stream));
     // every byte starts as "missing" (0x00): row padding and the slack rows never count
     PG_CUDA(cudaMemsetAsync(ctx->d_geno, 0, need, ctx->stream));
+    if (ctx->d_packed) PG_CUDA(cudaMemsetAsync(ctx->d_packed, 0, kneed, ctx->stream));
     // windows/pops stay; segments depend on S only
     if (!same_shape) ctx->brk.clear();
     return PG_OK;
@@ -457,6 +476,25 @@ extern "C" int pg_append_sites(pg_ctx* ctx, int64_t n, const int8_t* geno, const
         ctx->d_pos = fresh;
         ctx->pos_cap = pneed;
     }
+    const size_t kneed = (size_t)(S1 + 64) * ctx->packed_pitch + 4096;
+    if (ctx->d_packed && kneed > ctx->packed_cap) {   // the companion grows with the matrix, or is dropped
+        uint32_t* fresh = nullptr;
+        if (cudaMalloc((void**)&fresh, kneed) == cudaSuccess) {
+            PG_CUDA(cudaMemsetAsync(fresh, 0, kneed, ctx->stream));
+            PG_CUDA(cudaMemcpyAsync(fresh, ctx->d_packed, (size_t)S0 * ctx->packed_pitch, cudaMemcpyDeviceToDevice,
+                                    ctx->stream));
+            PG_CUDA(cudaStreamSynchronize(ctx->stream));
+            cudaFree(ctx->d_packed);
+            ctx->d_packed = fresh;
+            ctx->packed_cap = kneed;
+        } else {
+            cudaGetLastError();
+            PG_CUDA(cudaStreamSynchronize(ctx->stream));
+            cudaFree(ctx->d_packed);
+            ctx->d_packed = nullptr;
+            ctx->packed_cap = 0;
+        }
+    }
     ctx->S = S1;
     ctx->epoch += 1;
     ctx->data_gen += 1;
@@ -488,6 +526,87 @@ __global__ void k_ingest(const uint8_t* __restrict__ stage, uint8_t* __restrict_
         }
         reinterpret_cast<uint32_t*>(geno + (row0 + r) * pitch)[wi] = encode4(w);   // padding bytes encode to 0x00
     }
+}
+
+// Packed companion: a row is three planes of wd = ceil(H / 32) words — valid bits, then the low and the high bit of the
+// allele code (A 0, C 1, G 2, T 3) — haplotype h at bit h % 32 of word h / 32, padded to 16 bytes.  A site is one contiguous
+// row, so the site pass streams it like the one-hot rows, at 3/8 of their bytes.
+int pg_packed_pitch_for(int H) {
+    const int wd = (H + 31) / 32;
+    return (3 * wd * 4 + 15) / 16 * 16;
+}
+
+// One warp per row, 32 words (1024 haplotypes) at a time: lane j loads bytes 4j..4j+3 of each 128-haplotype group (coalesced,
+// the groups' loads in flight together), each 32-haplotype word is three ballots, and lane w % 32 keeps word w of the three
+// planes for coalesced stores.  The resident bytes of the H haplotypes are one-hot or 0 by construction (encode4 / k_ingest,
+// k_synth, k_parse_lines), so "valid" is byte != 0 and the code bits are "C or T" (0x44) and "G or T" (0x50).  Bytes past H
+// are ignored: an append inside the capacity of an earlier, wider matrix leaves them as that matrix wrote them.
+__global__ void __launch_bounds__(256) k_pack_rows(const uint8_t* __restrict__ geno, uint32_t* __restrict__ packed, int64_t row0,
+                                                   int64_t n, int pitch, int H, int ppw, int wd) {
+    const unsigned full = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = row0 + (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5); r < row0 + n; r += nwarps) {
+        const uint8_t* src = geno + r * pitch;
+        uint32_t* dst = packed + r * ppw;
+        for (int w0 = 0; w0 < wd; w0 += 32) {
+            const int ng = min(8, (wd - w0 + 3) / 4);       // 128-haplotype groups in this stretch (warp-uniform)
+            uint32_t v[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int off = w0 * 32 + j * 128 + lane * 4;
+                v[j] = (j < ng && off < pitch) ? *reinterpret_cast<const uint32_t*>(src + off) : 0u;
+            }
+            uint32_t V = 0u, B0 = 0u, B1 = 0u;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                if (j >= ng) break;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    // haplotype 32 (w0 + 4 j + k) + lane is byte (lane & 3) of the word lane 8 k + lane / 4 loaded
+                    const uint32_t byte = (__shfl_sync(full, v[j], k * 8 + (lane >> 2)) >> (8 * (lane & 3))) & 0xffu;
+                    const uint32_t b = 32 * (w0 + 4 * j + k) + lane < H ? byte : 0u;
+                    const uint32_t bv = __ballot_sync(full, b != 0u);
+                    const uint32_t b0 = __ballot_sync(full, (b & 0x44u) != 0u);
+                    const uint32_t b1 = __ballot_sync(full, (b & 0x50u) != 0u);
+                    if (lane == 4 * j + k) {
+                        V = bv;
+                        B0 = b0;
+                        B1 = b1;
+                    }
+                }
+            }
+            const int w = w0 + lane;
+            if (w < wd) {
+                dst[w] = V;
+                dst[wd + w] = B0;
+                dst[2 * wd + w] = B1;
+            }
+        }
+    }
+}
+
+int pg_pack_rows(pg_ctx* ctx, int64_t s0, int64_t n) {
+    if (!ctx->d_packed || n <= 0) return PG_OK;
+    const int wd = (ctx->H + 31) / 32;
+    const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((n + 7) / 8, (int64_t)ctx->sm_count * 16));
+    k_pack_rows<<<blocks, 256, 0, ctx->stream>>>((const uint8_t*)ctx->d_geno, ctx->d_packed, s0, n, ctx->pitch, ctx->H,
+                                                 ctx->packed_pitch / 4, wd);
+    PG_CUDA(cudaGetLastError());
+    ctx->launches += 1;
+    return PG_OK;
+}
+
+extern "C" int pg_debug_packed(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* row_words, uint32_t* out) {
+    PG_CHECK(ctx && row_words, "pg_debug_packed: null argument");
+    PG_CHECK(site0 >= 0 && n >= 0 && site0 + n <= ctx->S, "pg_debug_packed: range outside S");
+    *row_words = ctx->d_packed ? ctx->packed_pitch / 4 : 0;
+    if (!ctx->d_packed || !out || n == 0) return PG_OK;
+    PG_CUDA(cudaSetDevice(ctx->device));
+    PG_CUDA(cudaMemcpyAsync(out, (const uint8_t*)ctx->d_packed + site0 * ctx->packed_pitch, (size_t)n * ctx->packed_pitch,
+                            cudaMemcpyDeviceToHost, ctx->stream));
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    return PG_OK;
 }
 
 extern "C" int pg_upload_range(pg_ctx* ctx, int64_t site0, int64_t n, const int8_t* geno, const int32_t* pos) {
@@ -525,6 +644,7 @@ extern "C" int pg_upload_range(pg_ctx* ctx, int64_t site0, int64_t n, const int8
         PG_CUDA(cudaGetLastError());
         ctx->launches += 1;
         PG_CUDA(cudaEventRecord(ctx->stage_free[b], ctx->stream));
+        PG_TRY(pg_pack_rows(ctx, site0 + s, cnt));      // under the next slab's H2D copy
     }
     if (pos) {
         PG_CUDA(cudaMemcpyAsync(ctx->d_pos + site0, pos, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice,
@@ -648,6 +768,7 @@ extern "C" int pg_synth_fill(pg_ctx* ctx, int64_t S, int32_t n_pops, int32_t sam
     int blocks = (int)std::min<int64_t>(S, (int64_t)ctx->sm_count * 16);
     k_synth<<<blocks, 128, 0, ctx->stream>>>(ctx->d_geno, ctx->d_pos, sp);
     PG_CUDA(cudaGetLastError());
+    PG_TRY(pg_pack_rows(ctx, 0, S));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
     return PG_OK;
 }

@@ -515,6 +515,7 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
         PG_CUDA(cudaGetLastError());
         ctx->launches += 1;
     }
+    PG_TRY(pg_pack_rows(ctx, 0, S));
     unsigned long long h_err[3] = {0, 0, 0};
     PG_CUDA(cudaMemcpyAsync(h_err, d_err, 24, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));

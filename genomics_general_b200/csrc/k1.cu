@@ -42,6 +42,9 @@ struct K1Params {
     int n_ent;
     int ent_lo[PG_MAX_K1_POPS], ent_hi[PG_MAX_K1_POPS], full_lo[PG_MAX_K1_POPS], full_hi[PG_MAX_K1_POPS];
     int popN[PG_MAX_K1_POPS];
+    // packed popgen pass: (word, mask) entries of the populations (ent_lo / ent_hi index them), words per plane
+    const uint2* word_ent;
+    int wd;
     // segments / slots
     const int64_t* brk;
     int nseg;
@@ -897,6 +900,181 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
     if (MODE != MODE_COUNTS) warp_flush_lp<3, QU>(ai, au, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW, Q, spw, X, s_q);
 }
 
+// ---- bit-sliced popgen pass on the packed companion (ctx.cu pg_pack_rows) ------------------------------------------
+// A site row is three planes of wd words: valid bits V, low code bits B0, high code bits B1 (A 0, C 1, G 2, T 3).  Population
+// X is the (word, mask) entries [ent_lo[X], ent_hi[X]) of prm.word_ent; one entry adds
+//   n = popc(M), c1 = popc(M & B0), c2 = popc(M & B1), c3 = popc(M & B0 & B1)      with M = V & mask
+// and the allele counts are T = c3, C = c1 - c3, G = c2 - c3, A = n - c1 - c2 + c3.  The per-site sums and the slot layout
+// are k1_site_pass's (MODE_POPGEN / MODE_POPGEN_FREQ), so k1_finalize folds the same integers into bit-identical records.
+// Tiles and the ring are k1_site_pass's too, over rows of prm.pitch = packed bytes.  Rows start on 16-byte boundaries, so
+// the 32 lanes of a warp reading the same word of their own rows meet in at most 8 banks: each lane starts its walk over a
+// population's entries at an offset taken from its site index, which spreads the reads over the banks.
+template <int MODE, int P, int NW>
+__global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __grid_constant__ K1Params prm) {
+    static_assert(MODE == MODE_POPGEN || MODE == MODE_POPGEN_FREQ, "packed site pass: popgen modes");
+    constexpr int K1_THREADS = (NW + 1) * 32;
+    constexpr int QI = ModeTraits<MODE, P>::QI, QU = ModeTraits<MODE, P>::QU;
+    extern __shared__ __align__(128) uint8_t smem[];
+    uint8_t* tiles = smem;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)prm.stages * prm.tile_bytes);   // [stages]
+    uint64_t* empty = full + 8;                                                                  // [stages]
+    volatile int* s_issued = reinterpret_cast<volatile int*>(empty + 8);
+    uint2* s_ent = reinterpret_cast<uint2*>(smem + (size_t)prm.stages * prm.tile_bytes + 256);
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int b = blockIdx.x, B = gridDim.x;
+    const int64_t t0 = (int64_t)b * prm.num_tiles / B, t1 = (int64_t)(b + 1) * prm.num_tiles / B;
+    const int ntiles = (int)(t1 - t0);
+
+    for (int e = tid; e < prm.n_ent; e += K1_THREADS) s_ent[e] = prm.word_ent[e];
+    if (tid == 0) {
+        for (int s = 0; s < prm.stages; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], (uint32_t)prm.wpt);
+        }
+        *s_issued = 0;
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp == NW) {
+        if (lane == 0) k1_producer<MODE>(prm, tiles, full, empty, s_issued, ntiles, t0);
+        return;
+    }
+
+    const int G = prm.G;
+    const int spw = 32 / G;
+    const int gsub = lane / spw;
+    const int sl = lane % spw;
+    const int nteams = NW / prm.wpt;
+    const int team = warp / prm.wpt, lw = warp % prm.wpt;
+    const int sites_per_iter = prm.wpt * spw;
+    const int wd = prm.wd;
+
+    // this lane's entries of population X: the first one, then steps of G (wrapping inside the population), as many as
+    // walk[X] >> 16 (first | count << 16: the table holds < 6144 entries).  The G lanes of a site share the start offset, so
+    // that together they visit every entry once.
+    uint32_t walk[P];
+#pragma unroll
+    for (int X = 0; X < P; ++X) {
+        const int n = prm.ent_hi[X] - prm.ent_lo[X];
+        const int cnt = gsub < n ? (n - gsub + G - 1) / G : 0;
+        const int first = prm.ent_lo[X] + (n > 0 ? (((sl >> 2) & 7) + gsub) % n : 0);
+        walk[X] = (uint32_t)first | ((uint32_t)cnt << 16);
+    }
+
+    Acc<QI, QU, 0> acc;
+#pragma unroll
+    for (int q = 0; q < QI; ++q) acc.i[q] = 0;
+#pragma unroll
+    for (int q = 0; q < QU; ++q) acc.u[q] = 0u;
+    int since_flush = 0;
+    int cur_seg = -1;
+    int64_t seg_end = -1;
+    const int seg_first = prm.cta_seg_first[b];
+    const int64_t slot_base = prm.cta_slot_off[b];
+
+    for (int it = team; it < ntiles; it += nteams) {
+        const int stage = it % prm.stages;
+        if (lane == 0)
+            while (atomicAdd(const_cast<int*>(s_issued), 0) <= it) __nanosleep(20);
+        __syncwarp();
+        mbar_wait(&full[stage], (uint32_t)((it / prm.stages) & 1));
+        const uint8_t* tile = tiles + (size_t)stage * prm.tile_bytes;
+        const int64_t tile_site0 = prm.site_begin + (t0 + it) * prm.T;
+
+        for (int i = 0; i < prm.I; ++i) {
+            const int slot = i * sites_per_iter + lw * spw + sl;
+            const int64_t site = tile_site0 + slot;
+            const bool valid = site < prm.site_end;
+            const bool owner = valid && (gsub == 0);
+            const uint32_t* row = reinterpret_cast<const uint32_t*>(tile + (size_t)(valid ? slot : 0) * prm.pitch);
+            const int posv = owner ? reinterpret_cast<const int32_t*>(tile + (size_t)prm.T * prm.pitch)[slot] : 0;
+
+            uint32_t n[P], c[P][4];
+#pragma unroll
+            for (int X = 0; X < P; ++X) {
+                uint32_t a = 0u, a1 = 0u, a2 = 0u, a3 = 0u;
+                const int lo = prm.ent_lo[X], span = prm.ent_hi[X] - lo;
+                int e = (int)(walk[X] & 0xffffu);
+                const int cnt = (int)(walk[X] >> 16);
+                for (int k = 0; k < cnt; ++k) {
+                    const uint2 em = s_ent[e];
+                    const uint32_t m = row[em.x] & em.y;
+                    const uint32_t b0 = row[wd + em.x], b1 = row[2 * wd + em.x];
+                    a += __popc(m);
+                    a1 += __popc(m & b0);
+                    a2 += __popc(m & b1);
+                    a3 += __popc(m & b0 & b1);
+                    e += G;
+                    if (e >= lo + span) e -= span;
+                }
+                // combine the G lanes of this site (16-bit fields: counts < 65536)
+                uint32_t p0 = a | (a1 << 16), p1 = a2 | (a3 << 16);
+                for (int d = spw; d < 32; d <<= 1) {
+                    p0 += __shfl_xor_sync(0xffffffffu, p0, d);
+                    p1 += __shfl_xor_sync(0xffffffffu, p1, d);
+                }
+                const uint32_t nn = p0 & 0xffffu, n1 = p0 >> 16, n2 = p1 & 0xffffu, n3 = p1 >> 16;
+                n[X] = nn;
+                c[X][0] = nn - n1 - n2 + n3;
+                c[X][1] = n1 - n3;
+                c[X][2] = n2 - n3;
+                c[X][3] = n3;
+            }
+
+            // ---- segment bookkeeping (warp-uniform control flow), as in k1_site_pass ----
+            int sg = cur_seg;
+            if (owner && site >= seg_end) sg = find_seg(prm.brk, prm.nseg, cur_seg + 1, site);
+            if (__any_sync(0xffffffffu, sg != cur_seg)) {
+                warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+                since_flush = 0;
+                if (sg != cur_seg) {
+                    cur_seg = sg;
+                    seg_end = __ldg(prm.brk + sg + 1);
+                }
+            }
+
+            bool allpres = true, allmiss = true;
+#pragma unroll
+            for (int X = 0; X < P; ++X) {
+                allpres = allpres && (n[X] == (uint32_t)prm.popN[X]);
+                allmiss = allmiss && (n[X] == 0u);
+            }
+            const bool pres = owner && allpres;
+            const bool ragged = owner && !allpres && !allmiss;
+            if (++since_flush > prm.acc_limit) {      // the 32-bit sums must not overflow
+                warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+                since_flush = 1;
+            }
+            acc.i[0] += pres ? 1 : 0;
+            acc.i[1] += ragged ? 1 : 0;
+            acc.i[2] += (long long)posv;
+            const uint32_t f = pres ? 1u : 0u;
+#pragma unroll
+            for (int X = 0; X < P; ++X) {
+                const uint32_t sq = c[X][0] * c[X][0] + c[X][1] * c[X][1] + c[X][2] * c[X][2] + c[X][3] * c[X][3];
+                acc.u[X] += sq * f;
+                if (MODE == MODE_POPGEN_FREQ) acc.u[P + P * (P - 1) / 2 + X] += (pres && sq != n[X] * n[X]) ? 1u : 0u;
+            }
+            int k = 0;
+#pragma unroll
+            for (int X = 0; X < P; ++X)
+#pragma unroll
+                for (int Y = X + 1; Y < P; ++Y) {
+                    const uint32_t cr = c[X][0] * c[Y][0] + c[X][1] * c[Y][1] + c[X][2] * c[Y][2] + c[X][3] * c[Y][3];
+                    acc.u[P + k] += cr * f;
+                    ++k;
+                }
+        }
+
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[stage]);
+    }
+    warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+}
+
 // ---- finalize: slots -> segments -> windows -> statistics ------------------------------------------
 struct FinParams {
     const unsigned long long* part;
@@ -1109,9 +1287,35 @@ __global__ void __launch_bounds__(64) k1_finalize(const __grid_constant__ FinPar
 struct PopTables {
     std::vector<int32_t> ent_chunk;
     std::vector<uint32_t> ent_mask;   // 4 words per entry
+    std::vector<uint32_t> word_ent;   // packed pass: (word, mask) per entry, instead of ent_chunk / ent_mask
     int ent_lo[PG_MAX_K1_POPS], ent_hi[PG_MAX_K1_POPS], full_lo[PG_MAX_K1_POPS], full_hi[PG_MAX_K1_POPS];
     int popN[PG_MAX_K1_POPS];
 };
+
+// The packed pass's form of the tables: population X is entries [ent_lo[X], ent_hi[X]) of word_ent, one per 32-haplotype
+// word it has a member in, with the mask of its members.
+void build_word_tables(const std::vector<int32_t>& hap_pop_local, int H, int Ppad, PopTables& t) {
+    t.ent_chunk.clear();
+    t.ent_mask.clear();
+    t.word_ent.clear();
+    for (int X = 0; X < PG_MAX_K1_POPS; ++X) t.ent_lo[X] = t.ent_hi[X] = t.full_lo[X] = t.full_hi[X] = t.popN[X] = 0;
+    const int wd = (H + 31) / 32;
+    for (int X = 0; X < Ppad; ++X) {
+        std::vector<uint32_t> m(wd, 0u);
+        for (int h = 0; h < H; ++h)
+            if (hap_pop_local[h] == X) {
+                m[h / 32] |= 1u << (h % 32);
+                ++t.popN[X];
+            }
+        t.ent_lo[X] = (int)t.word_ent.size() / 2;
+        for (int w = 0; w < wd; ++w)
+            if (m[w]) {
+                t.word_ent.push_back((uint32_t)w);
+                t.word_ent.push_back(m[w]);
+            }
+        t.ent_hi[X] = (int)t.word_ent.size() / 2;
+    }
+}
 
 // hap_pop_local[h] in [0, Ppad) or -1
 void build_tables(const std::vector<int32_t>& hap_pop_local, int H, int chunks, int Ppad, PopTables& t) {
@@ -1159,7 +1363,7 @@ void build_tables(const std::vector<int32_t>& hap_pop_local, int H, int chunks, 
 }
 
 // shared memory of the mask tables (+ the per-population tables of the lane-per-population variant)
-int table_bytes_of(const PopTables& t) { return (int)t.ent_chunk.size() * 20 + 64 + 512; }
+int table_bytes_of(const PopTables& t) { return (int)t.ent_chunk.size() * 20 + (int)t.word_ent.size() * 4 + 64 + 512; }
 
 int check_plan(const K1Plan& pl) {
     PG_CHECK((pl.T % 4) == 0, "rows of %d bytes are too long for the site-pass kernel", pl.pitch);
@@ -1189,11 +1393,12 @@ int seg_of(const std::vector<int64_t>& brk, int64_t site) {
 }
 
 // device layout of the uploaded tables inside ctx->tables:
-//   [ent_mask (16B each)] [ent_chunk] [brk] [cta_seg_first] [cta_slot_off] [seg_cta_lo] [seg_cta_hi]
+//   [ent_mask (16B each)] [ent_chunk] [word_ent (8B each)] [brk] [cta_seg_first] [cta_slot_off] [seg_cta_lo] [seg_cta_hi]
 //   [win_seg_lo] [win_seg_hi] [win_lo] [win_hi]
 struct DevTables {
     uint4* ent_mask;
     int32_t* ent_chunk;
+    uint2* word_ent;
     int64_t* brk;
     int32_t* cta_seg_first;
     int64_t* cta_slot_off;
@@ -1221,6 +1426,7 @@ int push(pg_ctx* ctx, uint8_t* base, size_t& off, const T* src, size_t n, T** ou
 struct K1Cache {
     bool valid = false;
     bool lanepop = false;
+    bool packed = false;      // the launch reads the packed companion (k1_site_pass_packed)
     uint64_t epoch = 0;
     int mode = -1;
     int sel[4] = {-1, -1, -1, -1};
@@ -1230,20 +1436,37 @@ struct K1Cache {
     PgBuf tables;
 };
 
+// The one-hot rows' launch plan for this population map, or the error that refuses such rows.
+int byte_plan(pg_ctx* ctx, const std::vector<int32_t>& hap_pop_local, int Ppad, int nw, int force_G, PopTables& pt,
+              K1Plan& plan) {
+    build_tables(hap_pop_local, ctx->H, ctx->pitch / 16, Ppad, pt);
+    const int table_bytes = table_bytes_of(pt);
+    PG_CHECK(table_bytes <= 48 * 1024, "population layout needs %d bytes of mask tables (limit 48 KiB)", table_bytes);
+    plan = pg_make_k1_plan(ctx->S, ctx->H, ctx->sm_count, table_bytes, nw, force_G);
+    PG_CHECK(plan.stages >= 2, "rows of %d haplotypes are too long for the site-pass kernel (pitch %d bytes)", ctx->H,
+             plan.pitch);
+    return check_plan(plan);
+}
+
+// packed: plan and tables for the packed companion's rows (k1_site_pass_packed) instead of the one-hot rows
 int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_pop_local, int Ppad, int Q, int nw,
-                     int force_G = 0) {
+                     int force_G = 0, bool packed = false) {
     K1Launch& L = c.L;
     DevTables& dt = c.dt;
     PopTables& pt = c.pt;
     PG_TRY(pg_build_segments(ctx));
-    build_tables(hap_pop_local, ctx->H, ctx->pitch / 16, Ppad, pt);
-    const int n_ent = (int)pt.ent_chunk.size();
-    const int table_bytes = table_bytes_of(pt);
-    PG_CHECK(table_bytes <= 48 * 1024, "population layout needs %d bytes of mask tables (limit 48 KiB)", table_bytes);
-    L.plan = pg_make_k1_plan(ctx->S, ctx->H, ctx->sm_count, table_bytes, nw, force_G);
-    PG_CHECK(L.plan.stages >= 2, "rows of %d haplotypes are too long for the site-pass kernel (pitch %d bytes)", ctx->H,
-             L.plan.pitch);
-    PG_TRY(check_plan(L.plan));
+    if (packed) {
+        build_word_tables(hap_pop_local, ctx->H, Ppad, pt);
+        const int table_bytes = table_bytes_of(pt);
+        PG_CHECK(table_bytes <= 48 * 1024, "population layout needs %d bytes of mask tables (limit 48 KiB)", table_bytes);
+        L.plan = pg_make_k1_plan_rows(ctx->S, ctx->packed_pitch, ctx->sm_count, table_bytes, nw, force_G);
+        PG_CHECK(L.plan.stages >= 2, "rows of %d haplotypes are too long for the packed site pass (%d bytes)", ctx->H,
+                 L.plan.pitch);
+        PG_TRY(check_plan(L.plan));
+    } else {
+        PG_TRY(byte_plan(ctx, hap_pop_local, Ppad, nw, force_G, pt, L.plan));
+    }
+    const int n_ent = packed ? (int)pt.word_ent.size() / 2 : (int)pt.ent_chunk.size();
     for (int X = 0; X < Ppad; ++X) PG_CHECK(pt.popN[X] <= 65535, "a population has more than 65535 haplotypes");
     const K1Plan& pl = L.plan;
     const int B = pl.ctas;
@@ -1276,8 +1499,8 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
             L.seg_cta_hi[g] = std::max(L.seg_cta_hi[g], b);
         }
     }
-    size_t bytes = 4096 + pt.ent_mask.size() * 4 + pt.ent_chunk.size() * 4 + ctx->brk.size() * 8 + (size_t)B * 12 +
-                   (size_t)std::max(nseg, 1) * 8 + (size_t)ctx->W * 24 + 16 * 16;
+    size_t bytes = 4096 + pt.ent_mask.size() * 4 + pt.ent_chunk.size() * 4 + pt.word_ent.size() * 4 + ctx->brk.size() * 8 +
+                   (size_t)B * 12 + (size_t)std::max(nseg, 1) * 8 + (size_t)ctx->W * 24 + 17 * 16;
     PG_TRY(c.tables.ensure(bytes));
     uint8_t* base = (uint8_t*)c.tables.p;
     size_t o = 0;
@@ -1285,6 +1508,9 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
     PG_TRY(push(ctx, base, o, pt.ent_mask.data(), pt.ent_mask.size(), &d_mask_words));
     dt.ent_mask = reinterpret_cast<uint4*>(d_mask_words);
     PG_TRY(push(ctx, base, o, pt.ent_chunk.data(), pt.ent_chunk.size(), &dt.ent_chunk));
+    uint32_t* d_word_ent = nullptr;
+    PG_TRY(push(ctx, base, o, pt.word_ent.data(), pt.word_ent.size(), &d_word_ent));
+    dt.word_ent = reinterpret_cast<uint2*>(d_word_ent);
     PG_TRY(push(ctx, base, o, ctx->brk.data(), ctx->brk.size(), &dt.brk));
     PG_TRY(push(ctx, base, o, L.cta_seg_first.data(), L.cta_seg_first.size(), &dt.cta_seg_first));
     PG_TRY(push(ctx, base, o, L.cta_slot_off.data(), L.cta_slot_off.size(), &dt.cta_slot_off));
@@ -1300,7 +1526,9 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
 
     K1Params& p = L.prm;
     memset(&p, 0, sizeof(p));
-    p.geno = (const uint8_t*)ctx->d_geno;
+    p.geno = packed ? (const uint8_t*)ctx->d_packed : (const uint8_t*)ctx->d_geno;
+    p.word_ent = dt.word_ent;
+    p.wd = (ctx->H + 31) / 32;
     p.pos = ctx->d_pos;
     p.site_begin = 0;
     p.site_end = ctx->S;
@@ -1336,7 +1564,7 @@ int arm_slots(pg_ctx* ctx, K1Cache& c) {
     PG_TRY(ctx->part.ensure(bytes));
     PG_CUDA(cudaMemsetAsync(ctx->part.p, 0, bytes, ctx->stream));
     c.L.prm.part = (unsigned long long*)ctx->part.p;
-    c.L.prm.geno = (const uint8_t*)ctx->d_geno;
+    c.L.prm.geno = c.packed ? (const uint8_t*)ctx->d_packed : (const uint8_t*)ctx->d_geno;
     c.L.prm.pos = ctx->d_pos;
     return PG_OK;
 }
@@ -1401,6 +1629,27 @@ int launch_site_pass(pg_ctx* ctx, const K1Launch& L, const char* name) {
     }
     if (L.prm.nw == 12) return launch_site_pass_nw<MODE, P, 12, false>(ctx, L, name);
     return launch_site_pass_nw<MODE, P, 8, false>(ctx, L, name);
+}
+
+template <int MODE, int P, int NW>
+int launch_site_pass_packed_nw(pg_ctx* ctx, const K1Launch& L, const char* name) {
+    auto kern = k1_site_pass_packed<MODE, P, NW>;
+    static bool attr_set[64] = {};
+    if (!attr_set[ctx->device & 63]) {
+        PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        attr_set[ctx->device & 63] = true;
+    }
+    const int ti = pg_time_begin(ctx, name);
+    kern<<<L.plan.ctas, (NW + 1) * 32, L.plan.smem_bytes, ctx->stream>>>(L.prm);
+    pg_time_end(ctx, ti);
+    PG_CUDA(cudaGetLastError());
+    return PG_OK;
+}
+
+template <int MODE, int P>
+int launch_site_pass_packed(pg_ctx* ctx, const K1Launch& L, const char* name) {
+    if (L.prm.nw == 12) return launch_site_pass_packed_nw<MODE, P, 12>(ctx, L, name);
+    return launch_site_pass_packed_nw<MODE, P, 8>(ctx, L, name);
 }
 
 int pad_pops(int P) { return P <= 2 ? 2 : (P <= 4 ? 4 : 8); }
@@ -1490,8 +1739,11 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     const int Pp = many ? 2 : pad_pops(P);
     const bool wf = ctx->want_freq && !many;
     const int Q = 3 + Pp + Pp * (Pp - 1) / 2 + (wf ? Pp : 0);
+    // The bit-sliced pass over the packed companion moves 3/8 of the one-hot bytes and is the faster one at every shape;
+    // the byte pass runs when the context has no companion, and PG_K1_BYTE_PASS selects it for the tests that compare the two.
+    const bool packed = ctx->d_packed != nullptr && !getenv("PG_K1_BYTE_PASS");
     K1Cache& c = *cache_of(ctx, 0);
-    if (!c.valid || c.epoch != ctx->epoch) {
+    if (!c.valid || c.epoch != ctx->epoch || c.packed != packed) {
         c.valid = false;
         for (int x = 0; x < P; ++x) {
             int N = 0;
@@ -1504,24 +1756,35 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
             for (int32_t& v : collapsed) v = v >= 0 ? 0 : -1;
         }
         const std::vector<int32_t>& pop_map = many ? collapsed : ctx->hap_pop;
-        // long rows, 4 or 8 real populations of <= 255 haplotypes: one lane per population (k1_site_pass_lp)
-        int maxN = 0;
-        for (int x = 0; x < P && !many; ++x) {
-            int N = 0;
-            for (int h = 0; h < ctx->H; ++h) N += ctx->hap_pop[h] == x;
-            maxN = std::max(maxN, N);
-        }
-        bool lp = !many && (Pp == 4 || Pp == 8) && Pp == P && maxN <= 255 && ctx->pitch >= 1024 && !getenv("PG_K1_NO_BYTES");
-        if (const char* e = getenv("PG_K1_LANEPOP")) {
-            lp = atoi(e) != 0 && !many && (Pp == 4 || Pp == 8) && maxN <= 255 && !getenv("PG_K1_NO_BYTES");
-        } else if (lp) {
+        if (packed) {
+            // the rows the byte pass refuses are refused here too, so that whether a call runs never depends on the
+            // companion having found memory
             PopTables pt;
-            build_tables(pop_map, ctx->H, ctx->pitch / 16, Pp, pt);
-            lp = lanepop_fits(ctx->S, ctx->H, ctx->sm_count, table_bytes_of(pt), k1_env_nw12(), Pp);
+            K1Plan bp;
+            PG_TRY(byte_plan(ctx, pop_map, Pp, k1_nw_for(ctx->pitch), 0, pt, bp));
+            c.lanepop = false;
+            PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, k1_nw_for(ctx->packed_pitch), 0, true));
+        } else {
+            // long rows, 4 or 8 real populations of <= 255 haplotypes: one lane per population (k1_site_pass_lp)
+            int maxN = 0;
+            for (int x = 0; x < P && !many; ++x) {
+                int N = 0;
+                for (int h = 0; h < ctx->H; ++h) N += ctx->hap_pop[h] == x;
+                maxN = std::max(maxN, N);
+            }
+            bool lp = !many && (Pp == 4 || Pp == 8) && Pp == P && maxN <= 255 && ctx->pitch >= 1024 && !getenv("PG_K1_NO_BYTES");
+            if (const char* e = getenv("PG_K1_LANEPOP")) {
+                lp = atoi(e) != 0 && !many && (Pp == 4 || Pp == 8) && maxN <= 255 && !getenv("PG_K1_NO_BYTES");
+            } else if (lp) {
+                PopTables pt;
+                build_tables(pop_map, ctx->H, ctx->pitch / 16, Pp, pt);
+                lp = lanepop_fits(ctx->S, ctx->H, ctx->sm_count, table_bytes_of(pt), k1_env_nw12(), Pp);
+            }
+            c.lanepop = lp;
+            const int nw = lp ? k1_env_nw12() : k1_nw_for(ctx->pitch);
+            PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, lp ? Pp : 0));
         }
-        c.lanepop = lp;
-        const int nw = lp ? k1_env_nw12() : k1_nw_for(ctx->pitch);
-        PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, lp ? Pp : 0));
+        c.packed = packed;
         c.epoch = ctx->epoch;
         c.valid = true;
     }
@@ -1534,7 +1797,17 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
         c.L.prm.lanepop = c.lanepop ? 1 : 0;
     }
     PG_TRY(arm_slots(ctx, c));
-    if (!wf) {
+    if (c.packed) {
+        if (!wf) {
+            if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 2>(ctx, c.L, "k1_popgen")));
+            else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 4>(ctx, c.L, "k1_popgen")));
+            else PG_TRY((launch_site_pass_packed<MODE_POPGEN, 8>(ctx, c.L, "k1_popgen")));
+        } else {
+            if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 2>(ctx, c.L, "k1_popgen")));
+            else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 4>(ctx, c.L, "k1_popgen")));
+            else PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 8>(ctx, c.L, "k1_popgen")));
+        }
+    } else if (!wf) {
         if (Pp == 2) PG_TRY((launch_site_pass<MODE_POPGEN, 2>(ctx, c.L, "k1_popgen")));
         else if (Pp == 4) PG_TRY((launch_site_pass<MODE_POPGEN, 4>(ctx, c.L, "k1_popgen")));
         else PG_TRY((launch_site_pass<MODE_POPGEN, 8>(ctx, c.L, "k1_popgen")));

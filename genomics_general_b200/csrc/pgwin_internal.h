@@ -72,8 +72,10 @@ struct K1Plan {
     int ctas;         // persistent CTAs, each owning a contiguous tile range
 };
 K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw = 8, int force_G = 0);
+K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G);   // rows of `pitch` bytes
 int pg_k1_plan_ok(const K1Plan& p);   // 1 if the site-pass kernels can run this plan
 int pg_pitch_for(int H);
+int pg_packed_pitch_for(int H);       // bytes per row of the packed companion
 
 struct pg_ctx {
     int device = 0;
@@ -86,6 +88,12 @@ struct pg_ctx {
     int32_t H = 0;
     int32_t pitch = 0;
     size_t geno_cap = 0, pos_cap = 0;
+    // packed companion of the resident matrix (DESIGN.md "Packed companion"): per site three planes of ceil(H / 32) words
+    // (valid bits, low and high bit of the allele code), rows of packed_pitch bytes.  Every writer of d_geno rebuilds the
+    // rows it wrote (pg_pack_rows); nullptr when it could not be allocated, and the popgen site pass then reads the bytes.
+    uint32_t* d_packed = nullptr;
+    int32_t packed_pitch = 0;
+    size_t packed_cap = 0;
     // populations
     int32_t P = 0;
     std::vector<int32_t> hap_pop;
@@ -151,6 +159,7 @@ void pg_time_end(pg_ctx* ctx, int idx);
 int pg_pinned(pg_ctx* ctx, size_t bytes, void** out);
 int pg_d2h_staged(pg_ctx* ctx, void* dst, const void* src, size_t bytes);   // large device -> pageable host copy
 int pg_build_segments(pg_ctx* ctx);
+int pg_pack_rows(pg_ctx* ctx, int64_t s0, int64_t n);   // rows [s0, s0 + n) of the packed companion from d_geno (ctx stream)
 
 // tensor-core pairwise path (k2t.cu): bit-packed operand planes of one site span
 struct K2TPlanes {

@@ -543,6 +543,18 @@ class Engine:
         check(self._lib.pg_launch_count(self._ctx, C.byref(n)), "pg_launch_count")
         return int(n.value)
 
+    def packed_rows(self, site0: int, n: int):
+        """uint32 [n, 3, ceil(H / 32)] rows of the packed companion (valid bits, low and high allele-code bit; haplotype h at
+        bit h % 32 of word h / 32), or None when the context has no companion."""
+        words = C.c_int32(0)
+        check(self._lib.pg_debug_packed(self._ctx, int(site0), int(n), C.byref(words), None), "pg_debug_packed")
+        if words.value == 0:
+            return None
+        out = np.empty((n, words.value), dtype=np.uint32)
+        check(self._lib.pg_debug_packed(self._ctx, int(site0), int(n), C.byref(words), _ptr(out)), "pg_debug_packed")
+        wd = (self.H + 31) // 32
+        return out[:, :3 * wd].reshape(n, 3, wd)
+
 
 def k1_plan(S: int, H: int, nw: int = 8, lanes: int = 0, table_bytes: int = 4096):
     """Host-only: the site-pass launch geometry for a shape (works without a GPU).  `nw` consumer warps per CTA (8, or 12

@@ -292,6 +292,10 @@ int pg_debug_k1_plan(int64_t S, int32_t H, int32_t* pitch, int32_t* lanes_per_si
  * launches do.  out[9] = pitch, G, wpt, I, T (sites per tile), stages, smem_bytes, CTAs on 132 SMs, 1 if the site-pass
  * kernels accept the plan (0: such rows are refused). */
 int pg_debug_k1_plan_ex(int64_t S, int32_t H, int32_t nw, int32_t force_G, int32_t table_bytes, int32_t* out);
+/* The packed companion of the resident matrix (rows the popgen site pass reads): *row_words = 32-bit words per site row
+ * (three planes of ceil(H / 32) words — valid bits, low and high bit of the allele code A0 C1 G2 T3 — then padding), 0 when
+ * the context has no companion.  out (may be NULL) receives rows [site0, site0 + n). */
+int pg_debug_packed(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* row_words, uint32_t* out);
 
 #ifdef __cplusplus
 }
