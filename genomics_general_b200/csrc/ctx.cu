@@ -76,6 +76,7 @@ extern "C" int pg_ctx_destroy(pg_ctx* ctx) {
     ctx->gather_flag.release();
     if (ctx->d_geno) cudaFree(ctx->d_geno);
     if (ctx->d_packed) cudaFree(ctx->d_packed);
+    if (ctx->d_site_cls) cudaFree(ctx->d_site_cls);
     if (ctx->d_pos) cudaFree(ctx->d_pos);
     PgBuf* bufs[] = {&ctx->tables, &ctx->part, &ctx->segmeta, &ctx->winmeta, &ctx->out_d, &ctx->out_i,
                      &ctx->planes, &ctx->planes2, &ctx->pairs, &ctx->misc, &ctx->misc2, &ctx->misc3, &ctx->misc4, &ctx->misc5, &ctx->text, &ctx->starts, &ctx->meta,
@@ -279,7 +280,7 @@ K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw, 
     return pg_make_k1_plan_rows(S, pg_pitch_for(H), sm_count, table_bytes, nw, force_G);
 }
 
-K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G) {
+K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G, int code_bytes) {
     K1Plan p;
     memset(&p, 0, sizeof(p));
     p.pitch = pitch;
@@ -311,7 +312,8 @@ K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes,
     p.wpt = wpt;
     p.nw = nw;
     p.T = (32 * wpt / G) * I;
-    p.tile_bytes = ((p.T * p.pitch + p.T * 4 + 127) / 128) * 128;   // genotype rows + the tile's positions
+    // genotype rows + the tile's positions (+ its codes, in 16-byte pieces)
+    p.tile_bytes = ((p.T * p.pitch + p.T * 4 + (p.T * code_bytes + 15) / 16 * 16 + 127) / 128) * 128;
     int stages = smem_cap / p.tile_bytes;
     if (stages > 8) stages = 8;
     stages = std::min(stages, std::max(2, env_int("PG_K1_STAGES", stages)));
@@ -430,6 +432,19 @@ extern "C" int pg_alloc_sites(pg_ctx* ctx, int64_t S, int32_t H) {
             cudaGetLastError();
         }
     }
+    const size_t cneed = (size_t)(S + 64);
+    if (!ctx->d_packed || cneed > ctx->cls_cap) {
+        if (ctx->d_site_cls) cudaFree(ctx->d_site_cls);
+        ctx->d_site_cls = nullptr;
+        ctx->cls_cap = 0;
+        if (ctx->d_packed) {
+            if (cudaMalloc((void**)&ctx->d_site_cls, cneed) == cudaSuccess) ctx->cls_cap = cneed;
+            else {                             // no classes: the popgen pass streams every packed row
+                ctx->d_site_cls = nullptr;
+                cudaGetLastError();
+            }
+        }
+    }
     const bool same_shape = (ctx->S == S && ctx->H == H && ctx->pitch == pitch);
     ctx->S = S;
     ctx->H = H;
@@ -441,6 +456,7 @@ extern "C" int pg_alloc_sites(pg_ctx* ctx, int64_t S, int32_t H) {
     // every byte starts as "missing" (0x00): row padding and the slack rows never count
     PG_CUDA(cudaMemsetAsync(ctx->d_geno, 0, need, ctx->stream));
     if (ctx->d_packed) PG_CUDA(cudaMemsetAsync(ctx->d_packed, 0, kneed, ctx->stream));
+    if (ctx->d_site_cls) PG_CUDA(cudaMemsetAsync(ctx->d_site_cls, 0, cneed, ctx->stream));
     // windows/pops stay; segments depend on S only
     if (!same_shape) ctx->brk.clear();
     return PG_OK;
@@ -495,6 +511,24 @@ extern "C" int pg_append_sites(pg_ctx* ctx, int64_t n, const int8_t* geno, const
             ctx->packed_cap = 0;
         }
     }
+    const size_t cneed = (size_t)(S1 + 64);
+    if (ctx->d_site_cls && (!ctx->d_packed || cneed > ctx->cls_cap)) {   // the classes grow with the companion, or are dropped
+        uint8_t* fresh = nullptr;
+        if (ctx->d_packed && cudaMalloc((void**)&fresh, cneed) == cudaSuccess) {
+            PG_CUDA(cudaMemsetAsync(fresh, 0, cneed, ctx->stream));
+            PG_CUDA(cudaMemcpyAsync(fresh, ctx->d_site_cls, (size_t)S0, cudaMemcpyDeviceToDevice, ctx->stream));
+            PG_CUDA(cudaStreamSynchronize(ctx->stream));
+            cudaFree(ctx->d_site_cls);
+            ctx->d_site_cls = fresh;
+            ctx->cls_cap = cneed;
+        } else {
+            cudaGetLastError();
+            PG_CUDA(cudaStreamSynchronize(ctx->stream));
+            cudaFree(ctx->d_site_cls);
+            ctx->d_site_cls = nullptr;
+            ctx->cls_cap = 0;
+        }
+    }
     ctx->S = S1;
     ctx->epoch += 1;
     ctx->data_gen += 1;
@@ -541,14 +575,19 @@ int pg_packed_pitch_for(int H) {
 // planes for coalesced stores.  The resident bytes of the H haplotypes are one-hot or 0 by construction (encode4 / k_ingest,
 // k_synth, k_parse_lines), so "valid" is byte != 0 and the code bits are "C or T" (0x44) and "G or T" (0x50).  Bytes past H
 // are ignored: an append inside the capacity of an earlier, wider matrix leaves them as that matrix wrote them.
-__global__ void __launch_bounds__(256) k_pack_rows(const uint8_t* __restrict__ geno, uint32_t* __restrict__ packed, int64_t row0,
-                                                   int64_t n, int pitch, int H, int ppw, int wd) {
+// With cls, the warp also writes the row's class (PG_CLS_*) from the same ballots: a word is uniform when its valid bits and
+// each code plane are all clear or all set over the word's haplotypes below H.
+__global__ void __launch_bounds__(256) k_pack_rows(const uint8_t* __restrict__ geno, uint32_t* __restrict__ packed,
+                                                   uint8_t* __restrict__ cls, int64_t row0, int64_t n, int pitch, int H, int ppw,
+                                                   int wd) {
     const unsigned full = 0xffffffffu;
     const int lane = threadIdx.x & 31;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t r = row0 + (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5); r < row0 + n; r += nwarps) {
         const uint8_t* src = geno + r * pitch;
         uint32_t* dst = packed + r * ppw;
+        // warp-uniform: some haplotype valid / missing, some valid code bit 0 (1) set / clear
+        bool any_v = false, any_m = false, any_b0 = false, any_nb0 = false, any_b1 = false, any_nb1 = false;
         for (int w0 = 0; w0 < wd; w0 += 32) {
             const int ng = min(8, (wd - w0 + 3) / 4);       // 128-haplotype groups in this stretch (warp-uniform)
             uint32_t v[8];
@@ -569,6 +608,14 @@ __global__ void __launch_bounds__(256) k_pack_rows(const uint8_t* __restrict__ g
                     const uint32_t bv = __ballot_sync(full, b != 0u);
                     const uint32_t b0 = __ballot_sync(full, (b & 0x44u) != 0u);
                     const uint32_t b1 = __ballot_sync(full, (b & 0x50u) != 0u);
+                    const int nh = min(32, max(0, H - 32 * (w0 + 4 * j + k)));     // haplotypes of this word below H
+                    const uint32_t in = nh == 32 ? full : (1u << nh) - 1u;
+                    any_v |= bv != 0u;
+                    any_m |= bv != in;
+                    any_b0 |= b0 != 0u;
+                    any_nb0 |= (bv & ~b0) != 0u;
+                    any_b1 |= b1 != 0u;
+                    any_nb1 |= (bv & ~b1) != 0u;
                     if (lane == 4 * j + k) {
                         V = bv;
                         B0 = b0;
@@ -583,6 +630,13 @@ __global__ void __launch_bounds__(256) k_pack_rows(const uint8_t* __restrict__ g
                 dst[2 * wd + w] = B1;
             }
         }
+        if (cls && lane == 0) {
+            uint8_t c = PG_CLS_VARIED;
+            if (!any_v) c = PG_CLS_MISSING;
+            else if (!any_m && !(any_b0 && any_nb0) && !(any_b1 && any_nb1))
+                c = (uint8_t)(PG_CLS_A + (any_b0 ? 1 : 0) + (any_b1 ? 2 : 0));
+            cls[r] = c;
+        }
     }
 }
 
@@ -590,8 +644,8 @@ int pg_pack_rows(pg_ctx* ctx, int64_t s0, int64_t n) {
     if (!ctx->d_packed || n <= 0) return PG_OK;
     const int wd = (ctx->H + 31) / 32;
     const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((n + 7) / 8, (int64_t)ctx->sm_count * 16));
-    k_pack_rows<<<blocks, 256, 0, ctx->stream>>>((const uint8_t*)ctx->d_geno, ctx->d_packed, s0, n, ctx->pitch, ctx->H,
-                                                 ctx->packed_pitch / 4, wd);
+    k_pack_rows<<<blocks, 256, 0, ctx->stream>>>((const uint8_t*)ctx->d_geno, ctx->d_packed, ctx->d_site_cls, s0, n,
+                                                 ctx->pitch, ctx->H, ctx->packed_pitch / 4, wd);
     PG_CUDA(cudaGetLastError());
     ctx->launches += 1;
     return PG_OK;

@@ -45,6 +45,11 @@ struct K1Params {
     // packed popgen pass: (word, mask) entries of the populations (ent_lo / ent_hi index them), words per plane
     const uint2* word_ent;
     int wd;
+    // packed pass with uniform sites elided (UniformStream): geno holds only the varied rows, tile t's being rows
+    // [row0[t], row0[t + 1]); codes holds a 16-bit code per site, tile t's at t * code_pitch
+    const int64_t* row0;
+    const uint16_t* codes;
+    int code_pitch;
     // segments / slots
     const int64_t* brk;
     int nseg;
@@ -322,6 +327,48 @@ __device__ __forceinline__ void k1_producer(const K1Params& prm, uint8_t* tiles,
         // been armed, or try_wait.parity would alias it with the previous (already complete) phase
         __threadfence_block();
         atomicExch(const_cast<int*>(s_issued), it + 1);      // an atomic, so that racecheck sees the flag as synchronisation
+    }
+}
+
+// Producer of the packed pass over the varied rows only (the whole producer warp): a tile is its varied rows
+// [row0[t], row0[t + 1]), then its T positions, then its T codes.  A tile is about a microsecond of HBM time, as long as a
+// dependent load of row0, so the 32 lanes load the offsets of the next 32 tiles while the current 32 are issued.
+__device__ __forceinline__ void k1_producer_uniform(const K1Params& prm, uint8_t* tiles, uint64_t* full, uint64_t* empty,
+                                                    volatile int* s_issued, int ntiles, int64_t t0, int lane) {
+    auto ld_row0 = [&](int64_t t) { return t <= prm.num_tiles ? __ldg(prm.row0 + t) : (int64_t)0; };
+    int64_t cur = ld_row0(t0 + lane);            // lane l: row0 of tile t0 + g + l
+    for (int g = 0; g < ntiles; g += 32) {
+        const int64_t nxt = ld_row0(t0 + g + 32 + lane);
+        const int kn = min(32, ntiles - g);
+        for (int k = 0; k < kn; ++k) {
+            const int64_t r0 = __shfl_sync(0xffffffffu, cur, k);
+            const int64_t r1 = k < 31 ? __shfl_sync(0xffffffffu, cur, k + 1) : __shfl_sync(0xffffffffu, nxt, 0);
+            if (lane == 0) {
+                const int it = g + k;
+                const int stage = it % prm.stages;
+                if (it >= prm.stages) mbar_wait(&empty[stage], (uint32_t)(((it / prm.stages) - 1) & 1));
+                const int64_t tile = t0 + it;
+                const int64_t s_lo = prm.site_begin + tile * prm.T;
+                int64_t rows = prm.site_end - s_lo;
+                if (rows > prm.T) rows = prm.T;
+                const uint32_t bytes = (uint32_t)((r1 - r0) * prm.pitch);
+                const uint32_t pbytes = (uint32_t)(((rows * 4 + 15) / 16) * 16);
+                const uint32_t cbytes = (uint32_t)(((rows * 2 + 15) / 16) * 16);
+                mbar_expect_tx(&full[stage], bytes + pbytes + cbytes);
+                const uint8_t* src = prm.geno + r0 * prm.pitch;
+                uint8_t* dst = tiles + (size_t)stage * prm.tile_bytes;
+                for (uint32_t off = 0; off < bytes; off += 32768u) {
+                    const uint32_t n = (bytes - off) < 32768u ? (bytes - off) : 32768u;
+                    bulk_g2s(dst + off, src + off, n, &full[stage]);
+                }
+                bulk_g2s(dst + (size_t)prm.T * prm.pitch, prm.pos + s_lo, pbytes, &full[stage]);
+                bulk_g2s(dst + (size_t)prm.T * (prm.pitch + 4), prm.codes + tile * prm.code_pitch, cbytes, &full[stage]);
+                __threadfence_block();
+                atomicExch(const_cast<int*>(s_issued), it + 1);
+            }
+            __syncwarp();
+        }
+        cur = nxt;
     }
 }
 
@@ -909,7 +956,13 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
 // Tiles and the ring are k1_site_pass's too, over rows of prm.pitch = packed bytes.  Rows start on 16-byte boundaries, so
 // the 32 lanes of a warp reading the same word of their own rows meet in at most 8 banks: each lane starts its walk over a
 // population's entries at an offset taken from its site index, which spreads the reads over the banks.
-template <int MODE, int P, int NW>
+// UNI: the tiles hold only the varied rows (k1_producer_uniform) and a code per site: its rank among the tile's varied sites
+// (its row in the tile; T <= 2048), or UNI_CODE | PG_CLS_* for a site whose H haplotypes all carry one allele or are all
+// missing.  Such a site walks nothing: its counts follow from the population sizes (n_X = c_Xa = popN[X], or n_X = 0), the
+// same integers the walk would add.
+constexpr uint32_t UNI_CODE = 0x8000u;
+
+template <int MODE, int P, int NW, bool UNI = false>
 __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __grid_constant__ K1Params prm) {
     static_assert(MODE == MODE_POPGEN || MODE == MODE_POPGEN_FREQ, "packed site pass: popgen modes");
     constexpr int K1_THREADS = (NW + 1) * 32;
@@ -939,7 +992,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     __syncthreads();
 
     if (warp == NW) {
-        if (lane == 0) k1_producer<MODE>(prm, tiles, full, empty, s_issued, ntiles, t0);
+        if (UNI) k1_producer_uniform(prm, tiles, full, empty, s_issued, ntiles, t0, lane);
+        else if (lane == 0) k1_producer<MODE>(prm, tiles, full, empty, s_issued, ntiles, t0);
         return;
     }
 
@@ -951,6 +1005,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     const int team = warp / prm.wpt, lw = warp % prm.wpt;
     const int sites_per_iter = prm.wpt * spw;
     const int wd = prm.wd;
+    const size_t codes_off = (size_t)prm.T * (prm.pitch + 4);
 
     // this lane's entries of population X: the first one, then steps of G (wrapping inside the population), as many as
     // walk[X] >> 16 (first | count << 16: the table holds < 6144 entries).  The G lanes of a site share the start offset, so
@@ -989,7 +1044,13 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             const int64_t site = tile_site0 + slot;
             const bool valid = site < prm.site_end;
             const bool owner = valid && (gsub == 0);
-            const uint32_t* row = reinterpret_cast<const uint32_t*>(tile + (size_t)(valid ? slot : 0) * prm.pitch);
+            // a slot past the data reads no code (the stage holds a previous tile's there) and walks nothing
+            const uint32_t code = UNI ? (valid ? (uint32_t)reinterpret_cast<const uint16_t*>(tile + codes_off)[slot]
+                                               : (UNI_CODE | PG_CLS_MISSING))
+                                      : 0u;
+            const bool uni = UNI && (code & UNI_CODE);
+            const int ri = UNI ? (uni ? 0 : (int)code) : (valid ? slot : 0);
+            const uint32_t* row = reinterpret_cast<const uint32_t*>(tile + (size_t)ri * prm.pitch);
             const int posv = owner ? reinterpret_cast<const int32_t*>(tile + (size_t)prm.T * prm.pitch)[slot] : 0;
 
             uint32_t n[P], c[P][4];
@@ -998,7 +1059,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
                 uint32_t a = 0u, a1 = 0u, a2 = 0u, a3 = 0u;
                 const int lo = prm.ent_lo[X], span = prm.ent_hi[X] - lo;
                 int e = (int)(walk[X] & 0xffffu);
-                const int cnt = (int)(walk[X] >> 16);
+                const int cnt = uni ? 0 : (int)(walk[X] >> 16);
                 for (int k = 0; k < cnt; ++k) {
                     const uint2 em = s_ent[e];
                     const uint32_t m = row[em.x] & em.y;
@@ -1022,6 +1083,12 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
                 c[X][1] = n1 - n3;
                 c[X][2] = n2 - n3;
                 c[X][3] = n3;
+                if (uni) {
+                    const uint32_t cls = code & 7u, N = (uint32_t)prm.popN[X];
+                    n[X] = cls == PG_CLS_MISSING ? 0u : N;
+#pragma unroll
+                    for (int al = 0; al < 4; ++al) c[X][al] = cls == (uint32_t)(PG_CLS_A + al) ? N : 0u;
+                }
             }
 
             // ---- segment bookkeeping (warp-uniform control flow), as in k1_site_pass ----
@@ -1421,6 +1488,71 @@ int push(pg_ctx* ctx, uint8_t* base, size_t& off, const T* src, size_t n, T** ou
     return PG_OK;
 }
 
+// ---- the packed rows of the varied sites only (DESIGN.md "Uniform sites") -------------------------------------------
+// Derived from the companion and its site classes (ctx->d_site_cls) for one data generation and tile size T: per tile the
+// index of its first varied row (row0, int64 [tiles + 1]), a 16-bit code per site (UNI_CODE | class, or the rank among the
+// tile's varied sites; tile t's T codes at t * code_pitch) and the varied rows, contiguous.
+struct UniformStream {
+    uint64_t gen = 0;         // ctx->data_gen it describes (0: none)
+    int T = 0;
+    bool forced = false;
+    bool in_use = false;      // false: too few uniform sites to pay off, or no memory; the packed pass streams every row
+    int64_t varied = 0;
+    int code_pitch = 0;
+    PgBuf cnt, row0, codes, src, rows, scan;
+    void release() {
+        for (PgBuf* b : {&cnt, &row0, &codes, &src, &rows, &scan}) b->release();
+        gen = 0;
+    }
+};
+
+// varied sites per tile
+__global__ void __launch_bounds__(256) k1_uni_count(const uint8_t* __restrict__ cls, int64_t S, int T, int64_t* __restrict__ cnt) {
+    __shared__ int s_n;
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    const int64_t s0 = (int64_t)blockIdx.x * T;
+    int n = 0;
+    for (int j = threadIdx.x; j < T; j += blockDim.x)
+        if (s0 + j < S && cls[s0 + j] == PG_CLS_VARIED) ++n;
+    n = __reduce_add_sync(0xffffffffu, n);
+    if ((threadIdx.x & 31) == 0) atomicAdd(&s_n, n);
+    __syncthreads();
+    if (threadIdx.x == 0) cnt[blockIdx.x] = s_n;
+}
+
+// codes of tile blockIdx.x, and the source site of each of its varied rows
+__global__ void __launch_bounds__(256) k1_uni_codes(const uint8_t* __restrict__ cls, int64_t S, int T, int code_pitch,
+                                                    const int64_t* __restrict__ row0, uint16_t* __restrict__ codes,
+                                                    int64_t* __restrict__ src) {
+    typedef cub::BlockScan<int, 256> Scan;
+    __shared__ typename Scan::TempStorage tmp;
+    const int64_t t = blockIdx.x, s0 = t * T, r0 = row0[t];
+    int base = 0;
+    for (int j0 = 0; j0 < code_pitch; j0 += 256) {
+        const int j = j0 + threadIdx.x;
+        const int64_t s = s0 + j;
+        const uint32_t k = (j < T && s < S) ? cls[s] : (uint32_t)PG_CLS_MISSING;
+        const int v = k == PG_CLS_VARIED ? 1 : 0;
+        int rank, total;
+        Scan(tmp).ExclusiveSum(v, rank, total);
+        __syncthreads();
+        if (j < code_pitch) codes[t * code_pitch + j] = (uint16_t)(v ? (uint32_t)(base + rank) : (UNI_CODE | k));
+        if (v) src[r0 + base + rank] = s;
+        base += total;
+    }
+}
+
+// varied row r <- companion row src[r], 16 bytes per thread
+__global__ void __launch_bounds__(256) k1_uni_gather(const uint4* __restrict__ packed, const int64_t* __restrict__ src,
+                                                     int64_t nrows, int chunks, uint4* __restrict__ rows) {
+    const int64_t total = nrows * chunks;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / chunks;
+        rows[i] = packed[src[r] * chunks + (i - r * chunks)];
+    }
+}
+
 // Everything a windowed launch needs, cached per configuration (data shape, populations, windows): a repeated
 // statistics call on the same configuration only clears the slots and launches two kernels.
 struct K1Cache {
@@ -1434,6 +1566,9 @@ struct K1Cache {
     DevTables dt;
     PopTables pt;
     PgBuf tables;
+    K1Plan uplan;             // packed: L.plan with room for the codes in each stage (same T, tiles and CTAs)
+    UniformStream us;         // packed: the varied rows (popgen cache only)
+    bool uni_last = false;    // the last popgen launch read us
 };
 
 // The one-hot rows' launch plan for this population map, or the error that refuses such rows.
@@ -1631,9 +1766,9 @@ int launch_site_pass(pg_ctx* ctx, const K1Launch& L, const char* name) {
     return launch_site_pass_nw<MODE, P, 8, false>(ctx, L, name);
 }
 
-template <int MODE, int P, int NW>
+template <int MODE, int P, int NW, bool UNI>
 int launch_site_pass_packed_nw(pg_ctx* ctx, const K1Launch& L, const char* name) {
-    auto kern = k1_site_pass_packed<MODE, P, NW>;
+    auto kern = k1_site_pass_packed<MODE, P, NW, UNI>;
     static bool attr_set[64] = {};
     if (!attr_set[ctx->device & 63]) {
         PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -1646,10 +1781,74 @@ int launch_site_pass_packed_nw(pg_ctx* ctx, const K1Launch& L, const char* name)
     return PG_OK;
 }
 
-template <int MODE, int P>
+template <int MODE, int P, bool UNI = false>
 int launch_site_pass_packed(pg_ctx* ctx, const K1Launch& L, const char* name) {
-    if (L.prm.nw == 12) return launch_site_pass_packed_nw<MODE, P, 12>(ctx, L, name);
-    return launch_site_pass_packed_nw<MODE, P, 8>(ctx, L, name);
+    if (L.prm.nw == 12) return launch_site_pass_packed_nw<MODE, P, 12, UNI>(ctx, L, name);
+    return launch_site_pass_packed_nw<MODE, P, 8, UNI>(ctx, L, name);
+}
+
+// Streaming only the varied rows costs 6 + (1 - u) * pitch bytes per site against 4 + pitch, for a uniform fraction u, plus a
+// rebuild whenever the data change.  tools/packed_site_pass.py --sweep times the two passes across u at the C2 shape (H100
+// SXM, 700 W): 0.48 against 0.54 ms at u = 20 %, 0.50 against 0.54 at 10 %, 0.52 against 0.54 at 5 %, 0.55 against 0.54 at
+// 1 %.  The stream is kept from u >= 1/8 on, where its gain is clear of the run-to-run spread.
+constexpr double UNI_MIN_FRACTION = 0.125;
+
+// (Re)builds c.us for the current data and plan when they changed: one host synchronisation per rebuild, nothing on a
+// call over unchanged data.  PG_K1_UNIFORM_FORCE keeps the stream whatever the uniform fraction (tests on missing data).
+int uniform_prepare(pg_ctx* ctx, K1Cache& c) {
+    UniformStream& us = c.us;
+    const bool forced = getenv("PG_K1_UNIFORM_FORCE") != nullptr;
+    const K1Plan& pl = c.uplan;
+    if (us.gen == ctx->data_gen && us.T == pl.T && us.forced == forced) return PG_OK;
+    us.gen = ctx->data_gen;
+    us.T = pl.T;
+    us.forced = forced;
+    us.in_use = false;
+    us.varied = ctx->S;
+    if (pl.stages < 2 || pl.T != c.L.plan.T || pl.num_tiles != c.L.plan.num_tiles) return PG_OK;
+    const int64_t nt = pl.num_tiles;
+    PG_TRY(us.cnt.ensure((size_t)(nt + 1) * 8));
+    PG_TRY(us.row0.ensure((size_t)(nt + 1) * 8));
+    int64_t* d_cnt = (int64_t*)us.cnt.p;
+    int64_t* d_row0 = (int64_t*)us.row0.p;
+    size_t scan_bytes = 0;
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_cnt, d_row0, nt + 1, ctx->stream));
+    PG_TRY(us.scan.ensure(scan_bytes));
+    int ti = pg_time_begin(ctx, "k1_uniform");
+    PG_CUDA(cudaMemsetAsync(d_cnt + nt, 0, 8, ctx->stream));
+    k1_uni_count<<<(unsigned)nt, 256, 0, ctx->stream>>>(ctx->d_site_cls, ctx->S, pl.T, d_cnt);
+    PG_CUDA(cudaGetLastError());
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, scan_bytes, d_cnt, d_row0, nt + 1, ctx->stream));
+    pg_time_end(ctx, ti);
+    int64_t varied = 0;
+    PG_CUDA(cudaMemcpyAsync(&varied, d_row0 + nt, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    us.varied = varied;
+    if (!forced && (double)(ctx->S - varied) < UNI_MIN_FRACTION * (double)ctx->S) return PG_OK;
+    us.code_pitch = (pl.T + 7) / 8 * 8;
+    const int chunks = ctx->packed_pitch / 16;
+    if (us.codes.ensure((size_t)nt * us.code_pitch * 2) != PG_OK || us.src.ensure((size_t)std::max<int64_t>(varied, 1) * 8) != PG_OK ||
+        us.rows.ensure((size_t)std::max<int64_t>(varied, 1) * ctx->packed_pitch) != PG_OK) {
+        cudaGetLastError();                   // no memory for the stream: the packed pass streams every row
+        us.rows.release();
+        us.src.release();
+        return PG_OK;
+    }
+    ti = pg_time_begin(ctx, "k1_uniform");
+    k1_uni_codes<<<(unsigned)nt, 256, 0, ctx->stream>>>(ctx->d_site_cls, ctx->S, pl.T, us.code_pitch, d_row0,
+                                                       (uint16_t*)us.codes.p, (int64_t*)us.src.p);
+    pg_time_end(ctx, ti);
+    PG_CUDA(cudaGetLastError());
+    if (varied > 0) {
+        const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((varied * chunks + 255) / 256, (int64_t)ctx->sm_count * 16));
+        ti = pg_time_begin(ctx, "k1_uniform");
+        k1_uni_gather<<<blocks, 256, 0, ctx->stream>>>((const uint4*)ctx->d_packed, (const int64_t*)us.src.p, varied, chunks,
+                                                       (uint4*)us.rows.p);
+        pg_time_end(ctx, ti);
+        PG_CUDA(cudaGetLastError());
+    }
+    us.in_use = true;
+    return PG_OK;
 }
 
 int pad_pops(int P) { return P <= 2 ? 2 : (P <= 4 ? 4 : 8); }
@@ -1693,6 +1892,7 @@ void pg_k1_cache_free(pg_ctx* ctx) {
         if (ctx->k1_cache[k]) {
             K1Cache* c = static_cast<K1Cache*>(ctx->k1_cache[k]);
             c->tables.release();
+            c->us.release();
             delete c;
             ctx->k1_cache[k] = nullptr;
         }
@@ -1763,7 +1963,10 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
             K1Plan bp;
             PG_TRY(byte_plan(ctx, pop_map, Pp, k1_nw_for(ctx->pitch), 0, pt, bp));
             c.lanepop = false;
-            PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, k1_nw_for(ctx->packed_pitch), 0, true));
+            const int nw = k1_nw_for(ctx->packed_pitch);
+            PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, 0, true));
+            c.uplan = pg_make_k1_plan_rows(ctx->S, ctx->packed_pitch, ctx->sm_count, table_bytes_of(c.pt), nw, 0, 2);
+            if (!pg_k1_plan_ok(c.uplan)) c.uplan.stages = 0;    // no room for the codes: every row is streamed
         } else {
             // long rows, 4 or 8 real populations of <= 255 haplotypes: one lane per population (k1_site_pass_lp)
             int maxN = 0;
@@ -1796,8 +1999,31 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
         c.L.prm.bytes = (maxN <= 255 && !getenv("PG_K1_NO_BYTES")) ? 1 : 0;
         c.L.prm.lanepop = c.lanepop ? 1 : 0;
     }
+    // The packed pass streams only the varied rows when enough sites are uniform (uniform_prepare); PG_K1_NO_UNIFORM keeps
+    // every row streamed, for the tests that compare the two.
+    const bool uni = c.packed && ctx->d_site_cls && !getenv("PG_K1_NO_UNIFORM");
+    if (uni) PG_TRY(uniform_prepare(ctx, c));
+    c.uni_last = uni && c.us.in_use;
     PG_TRY(arm_slots(ctx, c));
-    if (c.packed) {
+    if (c.uni_last) {
+        K1Launch UL = c.L;
+        UL.plan = c.uplan;
+        UL.prm.stages = c.uplan.stages;
+        UL.prm.tile_bytes = c.uplan.tile_bytes;
+        UL.prm.geno = (const uint8_t*)c.us.rows.p;
+        UL.prm.row0 = (const int64_t*)c.us.row0.p;
+        UL.prm.codes = (const uint16_t*)c.us.codes.p;
+        UL.prm.code_pitch = c.us.code_pitch;
+        if (!wf) {
+            if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 2, true>(ctx, UL, "k1_popgen")));
+            else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 4, true>(ctx, UL, "k1_popgen")));
+            else PG_TRY((launch_site_pass_packed<MODE_POPGEN, 8, true>(ctx, UL, "k1_popgen")));
+        } else {
+            if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 2, true>(ctx, UL, "k1_popgen")));
+            else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 4, true>(ctx, UL, "k1_popgen")));
+            else PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 8, true>(ctx, UL, "k1_popgen")));
+        }
+    } else if (c.packed) {
         if (!wf) {
             if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 2>(ctx, c.L, "k1_popgen")));
             else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 4>(ctx, c.L, "k1_popgen")));
@@ -1844,6 +2070,15 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     *h_cnt = 0;
     PG_CUDA(cudaMemcpyAsync(h_cnt, d_cnt, 4, cudaMemcpyDeviceToHost, ctx->stream));
     *h_count = h_cnt;
+    return PG_OK;
+}
+
+extern "C" int pg_debug_uniform(pg_ctx* ctx, int32_t* in_use, int64_t* varied_sites) {
+    PG_CHECK(ctx && in_use && varied_sites, "pg_debug_uniform: null argument");
+    const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
+    const bool read = c && c->uni_last;
+    *in_use = read ? 1 : 0;
+    *varied_sites = (c && c->us.gen == ctx->data_gen) ? c->us.varied : ctx->S;
     return PG_OK;
 }
 

@@ -72,10 +72,15 @@ struct K1Plan {
     int ctas;         // persistent CTAs, each owning a contiguous tile range
 };
 K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw = 8, int force_G = 0);
-K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G);   // rows of `pitch` bytes
+// rows of `pitch` bytes; code_bytes: bytes per site that a tile carries behind its positions (the uniform-site codes)
+K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G, int code_bytes = 0);
 int pg_k1_plan_ok(const K1Plan& p);   // 1 if the site-pass kernels can run this plan
 int pg_pitch_for(int H);
 int pg_packed_pitch_for(int H);       // bytes per row of the packed companion
+
+// Site class of a packed row over its H haplotypes: every haplotype carries allele A / C / G / T, every haplotype is missing,
+// or anything else.  Zeroed memory reads as "varied", which is always safe to walk.
+enum { PG_CLS_VARIED = 0, PG_CLS_A = 1, PG_CLS_C = 2, PG_CLS_G = 3, PG_CLS_T = 4, PG_CLS_MISSING = 5 };
 
 struct pg_ctx {
     int device = 0;
@@ -94,6 +99,10 @@ struct pg_ctx {
     uint32_t* d_packed = nullptr;
     int32_t packed_pitch = 0;
     size_t packed_cap = 0;
+    // one class byte per packed row (PG_CLS_*), written by pg_pack_rows with the row; allocated, grown and dropped with
+    // d_packed (nullptr: no classes, and the popgen pass streams every row)
+    uint8_t* d_site_cls = nullptr;
+    size_t cls_cap = 0;
     // populations
     int32_t P = 0;
     std::vector<int32_t> hap_pop;

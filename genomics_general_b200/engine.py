@@ -555,6 +555,13 @@ class Engine:
         wd = (self.H + 31) // 32
         return out[:, :3 * wd].reshape(n, 3, wd)
 
+    def uniform_stream(self):
+        """(in_use, varied_sites): whether the last popgen call's site pass streamed only the packed rows of the sites whose
+        haplotypes are not all the same, and how many such sites it counted (S when it did not count them)."""
+        in_use, varied = C.c_int32(0), C.c_int64(0)
+        check(self._lib.pg_debug_uniform(self._ctx, C.byref(in_use), C.byref(varied)), "pg_debug_uniform")
+        return bool(in_use.value), int(varied.value)
+
 
 def k1_plan(S: int, H: int, nw: int = 8, lanes: int = 0, table_bytes: int = 4096):
     """Host-only: the site-pass launch geometry for a shape (works without a GPU).  `nw` consumer warps per CTA (8, or 12

@@ -296,6 +296,10 @@ int pg_debug_k1_plan_ex(int64_t S, int32_t H, int32_t nw, int32_t force_G, int32
  * (three planes of ceil(H / 32) words — valid bits, low and high bit of the allele code A0 C1 G2 T3 — then padding), 0 when
  * the context has no companion.  out (may be NULL) receives rows [site0, site0 + n). */
 int pg_debug_packed(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* row_words, uint32_t* out);
+/* The popgen pass's stream of varied rows as the last popgen call left it: *in_use = 1 when that call streamed only the
+ * rows of sites whose haplotypes are not all the same (0: every packed row), *varied_sites = the varied sites it counted
+ * (S when it did not count them). */
+int pg_debug_uniform(pg_ctx* ctx, int32_t* in_use, int64_t* varied_sites);
 
 #ifdef __cplusplus
 }
