@@ -312,8 +312,9 @@ K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes,
     p.wpt = wpt;
     p.nw = nw;
     p.T = (32 * wpt / G) * I;
-    // genotype rows + the tile's positions (+ its codes, in 16-byte pieces)
-    p.tile_bytes = ((p.T * p.pitch + p.T * 4 + (p.T * code_bytes + 15) / 16 * 16 + 127) / 128) * 128;
+    // genotype rows + the tile's positions (+ code_bytes per site for its codes, in arrays of 2 bytes per site padded to
+    // 16-byte pieces)
+    p.tile_bytes = ((p.T * p.pitch + p.T * 4 + code_bytes * ((p.T + 7) / 8 * 8) + 127) / 128) * 128;
     int stages = smem_cap / p.tile_bytes;
     if (stages > 8) stages = 8;
     stages = std::min(stages, std::max(2, env_int("PG_K1_STAGES", stages)));

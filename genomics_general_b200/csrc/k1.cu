@@ -17,6 +17,7 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
+#include <type_traits>
 #include <cub/cub.cuh>
 
 #include "pgwin_internal.h"
@@ -46,10 +47,12 @@ struct K1Params {
     const uint2* word_ent;
     int wd;
     // packed pass with uniform sites elided (UniformStream): geno holds only the varied rows, tile t's being rows
-    // [row0[t], row0[t + 1]); codes holds a 16-bit code per site, tile t's at t * code_pitch
+    // [row0[t], row0[t + 1]); codes holds tile t's 16-bit codes, one per site, at t * 2 * code_pitch, and code_pitch further
+    // the site index in the tile (slot) of each of its varied rows; uni_gv > 0 forces the lanes per varied row (PG_K1_UNI_GV)
     const int64_t* row0;
     const uint16_t* codes;
     int code_pitch;
+    int uni_gv;
     // segments / slots
     const int64_t* brk;
     int nseg;
@@ -331,10 +334,13 @@ __device__ __forceinline__ void k1_producer(const K1Params& prm, uint8_t* tiles,
 }
 
 // Producer of the packed pass over the varied rows only (the whole producer warp): a tile is its varied rows
-// [row0[t], row0[t + 1]), then its T positions, then its T codes.  A tile is about a microsecond of HBM time, as long as a
-// dependent load of row0, so the 32 lanes load the offsets of the next 32 tiles while the current 32 are issued.
+// [row0[t], row0[t + 1]), then its T positions, then its codes (code_pitch of them) and the slots of its varied rows.  The
+// count of varied rows goes to s_nvar[stage] before the stage is armed, so the mbarrier's phase publishes it.  A tile is
+// about a microsecond of HBM time, as long as a dependent load of row0, so the 32 lanes load the offsets of the next 32 tiles
+// while the current 32 are issued.
 __device__ __forceinline__ void k1_producer_uniform(const K1Params& prm, uint8_t* tiles, uint64_t* full, uint64_t* empty,
-                                                    volatile int* s_issued, int ntiles, int64_t t0, int lane) {
+                                                    volatile int* s_issued, volatile int* s_nvar, int ntiles, int64_t t0,
+                                                    int lane) {
     auto ld_row0 = [&](int64_t t) { return t <= prm.num_tiles ? __ldg(prm.row0 + t) : (int64_t)0; };
     int64_t cur = ld_row0(t0 + lane);            // lane l: row0 of tile t0 + g + l
     for (int g = 0; g < ntiles; g += 32) {
@@ -351,9 +357,11 @@ __device__ __forceinline__ void k1_producer_uniform(const K1Params& prm, uint8_t
                 const int64_t s_lo = prm.site_begin + tile * prm.T;
                 int64_t rows = prm.site_end - s_lo;
                 if (rows > prm.T) rows = prm.T;
-                const uint32_t bytes = (uint32_t)((r1 - r0) * prm.pitch);
+                const int nvar = (int)(r1 - r0);
+                const uint32_t bytes = (uint32_t)(nvar * prm.pitch);
                 const uint32_t pbytes = (uint32_t)(((rows * 4 + 15) / 16) * 16);
-                const uint32_t cbytes = (uint32_t)(((rows * 2 + 15) / 16) * 16);
+                const uint32_t cbytes = (uint32_t)(prm.code_pitch * 2 + ((nvar * 2 + 15) / 16) * 16);
+                s_nvar[stage] = nvar;
                 mbar_expect_tx(&full[stage], bytes + pbytes + cbytes);
                 const uint8_t* src = prm.geno + r0 * prm.pitch;
                 uint8_t* dst = tiles + (size_t)stage * prm.tile_bytes;
@@ -362,7 +370,7 @@ __device__ __forceinline__ void k1_producer_uniform(const K1Params& prm, uint8_t
                     bulk_g2s(dst + off, src + off, n, &full[stage]);
                 }
                 bulk_g2s(dst + (size_t)prm.T * prm.pitch, prm.pos + s_lo, pbytes, &full[stage]);
-                bulk_g2s(dst + (size_t)prm.T * (prm.pitch + 4), prm.codes + tile * prm.code_pitch, cbytes, &full[stage]);
+                bulk_g2s(dst + (size_t)prm.T * (prm.pitch + 4), prm.codes + tile * 2 * prm.code_pitch, cbytes, &full[stage]);
                 __threadfence_block();
                 atomicExch(const_cast<int*>(s_issued), it + 1);
             }
@@ -956,11 +964,184 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
 // Tiles and the ring are k1_site_pass's too, over rows of prm.pitch = packed bytes.  Rows start on 16-byte boundaries, so
 // the 32 lanes of a warp reading the same word of their own rows meet in at most 8 banks: each lane starts its walk over a
 // population's entries at an offset taken from its site index, which spreads the reads over the banks.
-// UNI: the tiles hold only the varied rows (k1_producer_uniform) and a code per site: its rank among the tile's varied sites
-// (its row in the tile; T <= 2048), or UNI_CODE | PG_CLS_* for a site whose H haplotypes all carry one allele or are all
-// missing.  Such a site walks nothing: its counts follow from the population sizes (n_X = c_Xa = popN[X], or n_X = 0), the
-// same integers the walk would add.
+// UNI: the tiles hold only the varied rows (k1_producer_uniform), a code per site (UNI_CODE | PG_CLS_* for a site whose H
+// haplotypes all carry one allele or are all missing, else its rank among the tile's varied sites) and the slot of each varied
+// row (its site's index in the tile; T <= 2048).  A team then makes two passes over a tile.  Pass V packs the varied rows onto
+// the team's lanes, Gv lanes per row: the plan's lanes per site (1 at C2 and C5, where more measured slower; 2 for rows of
+// 1 KiB and more; PG_K1_UNI_GV forces 1 .. 32 for the tests), so that a warp walks only when it holds varied rows, and those
+// fill its lanes.  Pass U runs one lane per slot:
+// it adds every site's position, and counts the uniform sites that are not missing, whose sums follow from the population
+// sizes (n_X = c_Xa = N_X: N_X^2 and N_X N_Y per site) and are added at its flush (uniform_flush).  Either pass keeps its own
+// segment and flushes into the warp's slots, which add, so the slots end with the same integers.
 constexpr uint32_t UNI_CODE = 0x8000u;
+
+// this lane's entries of population X: the first one, then steps of G (wrapping inside the population), as many as
+// walk[X] >> 16 (first | count << 16: the table holds < 6144 entries).  The G lanes of a site (gsub = 0 .. G - 1) share the
+// start offset, so that together they visit every entry once; sl (the site's index in the warp) spreads the banks.
+template <int P>
+__device__ __forceinline__ void packed_walk(const K1Params& prm, int G, int gsub, int sl, uint32_t (&walk)[P]) {
+#pragma unroll
+    for (int X = 0; X < P; ++X) {
+        const int n = prm.ent_hi[X] - prm.ent_lo[X];
+        const int cnt = gsub < n ? (n - gsub + G - 1) / G : 0;
+        const int first = prm.ent_lo[X] + (n > 0 ? (((sl >> 2) & 7) + gsub) % n : 0);
+        walk[X] = (uint32_t)first | ((uint32_t)cnt << 16);
+    }
+}
+
+// this lane's walk[] of the varied-row pass, in shared memory ([X][lane]) or in registers (RegWalk)
+struct SmemWalk {
+    const uint32_t* p;     // the table + lane
+    __device__ __forceinline__ uint32_t operator[](int X) const { return p[X * 32]; }
+};
+template <int P>
+struct RegWalk {
+    uint32_t w[P];
+    __device__ __forceinline__ uint32_t operator[](int X) const { return w[X]; }
+};
+
+// the allele counts of one packed row, combined over the 32 / spw lanes that share it; walk[X] as packed_walk sets it
+// A row's counts per population: n(X) haplotypes present and c(X, a) of allele a.  ArrCounts holds the five numbers;
+// PkCounts holds the two 16-bit-field words they come from and derives them where they are used, which can keep 3 * P fewer
+// registers live between the walk and the sums.
+template <int P>
+struct ArrCounts {
+    uint32_t nn[P], cc[P][4];
+    __device__ __forceinline__ void set(int X, uint32_t p0, uint32_t p1) {
+        const uint32_t m = p0 & 0xffffu, n1 = p0 >> 16, n2 = p1 & 0xffffu, n3 = p1 >> 16;
+        nn[X] = m;
+        cc[X][0] = m - n1 - n2 + n3;
+        cc[X][1] = n1 - n3;
+        cc[X][2] = n2 - n3;
+        cc[X][3] = n3;
+    }
+    __device__ __forceinline__ uint32_t n(int X) const { return nn[X]; }
+    __device__ __forceinline__ uint32_t c(int X, int a) const { return cc[X][a]; }
+};
+template <int P>
+struct PkCounts {
+    uint32_t p0[P], p1[P];
+    __device__ __forceinline__ void set(int X, uint32_t a, uint32_t b) {
+        p0[X] = a;
+        p1[X] = b;
+    }
+    __device__ __forceinline__ uint32_t n(int X) const { return p0[X] & 0xffffu; }
+    __device__ __forceinline__ uint32_t c(int X, int a) const {
+        const uint32_t n1 = p0[X] >> 16, n2 = p1[X] & 0xffffu, n3 = p1[X] >> 16;
+        return a == 0 ? (p0[X] & 0xffffu) - n1 - n2 + n3 : (a == 1 ? n1 - n3 : (a == 2 ? n2 - n3 : n3));
+    }
+};
+
+template <int P, class W, class CT>
+__device__ __forceinline__ void packed_counts(const K1Params& prm, const uint2* s_ent, const uint32_t* row, const W& walk,
+                                              int G, int spw, CT& ct) {
+    const int wd = prm.wd;
+#pragma unroll
+    for (int X = 0; X < P; ++X) {
+        uint32_t a = 0u, a1 = 0u, a2 = 0u, a3 = 0u;
+        const int lo = prm.ent_lo[X], span = prm.ent_hi[X] - lo;
+        int e = (int)(walk[X] & 0xffffu);
+        const int cnt = (int)(walk[X] >> 16);
+        for (int k = 0; k < cnt; ++k) {
+            const uint2 em = s_ent[e];
+            const uint32_t m = row[em.x] & em.y;
+            const uint32_t b0 = row[wd + em.x], b1 = row[2 * wd + em.x];
+            a += __popc(m);
+            a1 += __popc(m & b0);
+            a2 += __popc(m & b1);
+            a3 += __popc(m & b0 & b1);
+            e += G;
+            if (e >= lo + span) e -= span;
+        }
+        // combine the G lanes of this site (16-bit fields: counts < 65536)
+        uint32_t p0 = a | (a1 << 16), p1 = a2 | (a3 << 16);
+        for (int d = spw; d < 32; d <<= 1) {
+            p0 += __shfl_xor_sync(0xffffffffu, p0, d);
+            p1 += __shfl_xor_sync(0xffffffffu, p1, d);
+        }
+        ct.set(X, p0, p1);
+    }
+}
+
+// whether the site (of the lane that owns it) has every haplotype of every population, or some but not all of them
+template <int P, class CT>
+__device__ __forceinline__ void packed_class(const K1Params& prm, bool owner, const CT& ct, bool& pres, bool& ragged) {
+    bool allpres = true, allmiss = true;
+#pragma unroll
+    for (int X = 0; X < P; ++X) {
+        allpres = allpres && (ct.n(X) == (uint32_t)prm.popN[X]);
+        allmiss = allmiss && (ct.n(X) == 0u);
+    }
+    pres = owner && allpres;
+    ragged = owner && !allpres && !allmiss;
+}
+
+// one site's sums but its position
+template <int MODE, int P, class ACC, class CT>
+__device__ __forceinline__ void packed_add(ACC& acc, bool pres, bool ragged, const CT& ct) {
+    acc.i[0] += pres ? 1 : 0;
+    acc.i[1] += ragged ? 1 : 0;
+    const uint32_t f = pres ? 1u : 0u;
+#pragma unroll
+    for (int X = 0; X < P; ++X) {
+        const uint32_t sq = ct.c(X, 0) * ct.c(X, 0) + ct.c(X, 1) * ct.c(X, 1) + ct.c(X, 2) * ct.c(X, 2) + ct.c(X, 3) * ct.c(X, 3);
+        acc.u[X] += sq * f;
+        if (MODE == MODE_POPGEN_FREQ) acc.u[P + P * (P - 1) / 2 + X] += (pres && sq != ct.n(X) * ct.n(X)) ? 1u : 0u;
+    }
+    int k = 0;
+#pragma unroll
+    for (int X = 0; X < P; ++X)
+#pragma unroll
+        for (int Y = X + 1; Y < P; ++Y) {
+            const uint32_t cr = ct.c(X, 0) * ct.c(Y, 0) + ct.c(X, 1) * ct.c(Y, 1) + ct.c(X, 2) * ct.c(Y, 2) + ct.c(X, 3) * ct.c(Y, 3);
+            acc.u[P + k] += cr * f;
+            ++k;
+        }
+}
+
+// Pass U's state, one per consumer warp in shared memory behind the entry table, so that it holds no register while pass V
+// walks: its segment (warp-uniform) and the segment's end, and the positions and the uniform non-missing sites it has added
+// since its last flush.  Behind the records: pass V's walk table (SmemWalk).
+struct UniRec {
+    long long pos;
+    long long seg_end;
+    int seg;
+    uint32_t npres;
+};
+constexpr int UNI_SMEM_BYTES = K1_MAX_WARPS * (int)sizeof(UniRec) + PG_MAX_K1_POPS * 32 * 4;
+
+// the exact sum of the 32 lanes' v, from 32-bit reductions of its 16-bit halves
+__device__ __forceinline__ long long warp_sum_i32(int v) {
+    const uint32_t u = (uint32_t)v;
+    const long long lo = __reduce_add_sync(0xffffffffu, u & 0xffffu), hi = __reduce_add_sync(0xffffffffu, u >> 16);
+    const int neg = __popc(__ballot_sync(0xffffffffu, v < 0));
+    return lo + (hi << 16) - ((long long)neg << 32);
+}
+
+// Pass U's flush (the whole warp, the same values in every lane): into this warp's slot of segment seg, the positions, the
+// uniform non-missing sites, and the sums those sites add (N_X^2 per population, N_X N_Y per pair), in 64 bits; lane q adds
+// word q, so the read-modify-writes go out together.
+template <int MODE, int P>
+__device__ __forceinline__ void uniform_flush(const K1Params& prm, int seg, long long np, long long pos, int64_t slot_base,
+                                              int seg_first, int warp, int lane, int nw) {
+    constexpr int QI = ModeTraits<MODE, P>::QI, Q = QI + ModeTraits<MODE, P>::QU, NQ = QI + P + P * (P - 1) / 2;
+    unsigned long long* dst = prm.part + slot_base + ((int64_t)(seg - seg_first) * nw + warp) * Q;
+#pragma unroll
+    for (int q0 = 0; q0 < NQ; q0 += 32) {
+        const int q = q0 + lane;
+        long long v = q == 0 ? np : (q == 2 ? pos : 0ll);
+        if (q >= QI && q < NQ) {       // population X = Y, then the pairs (X, Y > X) in order
+            int X = q - QI, Y = X;
+            if (X >= P) {
+                int k = X - P, left = P - 1;
+                for (X = 0; k >= left; ++X, --left) k -= left;
+                Y = X + 1 + k;
+            }
+            v = np * (long long)prm.popN[X] * (long long)prm.popN[Y];
+        }
+        if (q < NQ && q != 1) dst[q] += (unsigned long long)v;
+    }
+}
 
 template <int MODE, int P, int NW, bool UNI = false>
 __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __grid_constant__ K1Params prm) {
@@ -972,6 +1153,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)prm.stages * prm.tile_bytes);   // [stages]
     uint64_t* empty = full + 8;                                                                  // [stages]
     volatile int* s_issued = reinterpret_cast<volatile int*>(empty + 8);
+    volatile int* s_nvar = s_issued + 8;     // UNI: varied rows of the tile in each stage [stages]
     uint2* s_ent = reinterpret_cast<uint2*>(smem + (size_t)prm.stages * prm.tile_bytes + 256);
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -980,6 +1162,18 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     const int ntiles = (int)(t1 - t0);
 
     for (int e = tid; e < prm.n_ent; e += K1_THREADS) s_ent[e] = prm.word_ent[e];
+    UniRec* s_urec = reinterpret_cast<UniRec*>(s_ent + prm.n_ent);          // UNI: [NW] pass U records, then the walk table
+    uint32_t* s_walk = reinterpret_cast<uint32_t*>(s_urec + K1_MAX_WARPS);
+    const int Gv = prm.uni_gv > 0 ? prm.uni_gv : prm.G;                    // UNI: lanes per varied row, the plan's per site
+    if (UNI && warp < NW) {
+        if (warp == 0) {
+            uint32_t w[P];
+            packed_walk<P>(prm, Gv, lane / (32 / Gv), lane % (32 / Gv), w);
+#pragma unroll
+            for (int X = 0; X < P; ++X) s_walk[X * 32 + lane] = w[X];
+        }
+        if (lane == 0) s_urec[warp] = UniRec{0ll, -1ll, -1, 0u};
+    }
     if (tid == 0) {
         for (int s = 0; s < prm.stages; ++s) {
             mbar_init(&full[s], 1);
@@ -992,32 +1186,13 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     __syncthreads();
 
     if (warp == NW) {
-        if (UNI) k1_producer_uniform(prm, tiles, full, empty, s_issued, ntiles, t0, lane);
+        if (UNI) k1_producer_uniform(prm, tiles, full, empty, s_issued, s_nvar, ntiles, t0, lane);
         else if (lane == 0) k1_producer<MODE>(prm, tiles, full, empty, s_issued, ntiles, t0);
         return;
     }
 
-    const int G = prm.G;
-    const int spw = 32 / G;
-    const int gsub = lane / spw;
-    const int sl = lane % spw;
     const int nteams = NW / prm.wpt;
     const int team = warp / prm.wpt, lw = warp % prm.wpt;
-    const int sites_per_iter = prm.wpt * spw;
-    const int wd = prm.wd;
-    const size_t codes_off = (size_t)prm.T * (prm.pitch + 4);
-
-    // this lane's entries of population X: the first one, then steps of G (wrapping inside the population), as many as
-    // walk[X] >> 16 (first | count << 16: the table holds < 6144 entries).  The G lanes of a site share the start offset, so
-    // that together they visit every entry once.
-    uint32_t walk[P];
-#pragma unroll
-    for (int X = 0; X < P; ++X) {
-        const int n = prm.ent_hi[X] - prm.ent_lo[X];
-        const int cnt = gsub < n ? (n - gsub + G - 1) / G : 0;
-        const int first = prm.ent_lo[X] + (n > 0 ? (((sl >> 2) & 7) + gsub) % n : 0);
-        walk[X] = (uint32_t)first | ((uint32_t)cnt << 16);
-    }
 
     Acc<QI, QU, 0> acc;
 #pragma unroll
@@ -1030,114 +1205,161 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     const int seg_first = prm.cta_seg_first[b];
     const int64_t slot_base = prm.cta_slot_off[b];
 
-    for (int it = team; it < ntiles; it += nteams) {
-        const int stage = it % prm.stages;
-        if (lane == 0)
-            while (atomicAdd(const_cast<int*>(s_issued), 0) <= it) __nanosleep(20);
-        __syncwarp();
-        mbar_wait(&full[stage], (uint32_t)((it / prm.stages) & 1));
-        const uint8_t* tile = tiles + (size_t)stage * prm.tile_bytes;
-        const int64_t tile_site0 = prm.site_begin + (t0 + it) * prm.T;
+    if constexpr (!UNI) {
+        const int G = prm.G;
+        const int spw = 32 / G;
+        const int gsub = lane / spw;
+        const int sl = lane % spw;
+        const int sites_per_iter = prm.wpt * spw;
+        uint32_t walk[P];
+        packed_walk<P>(prm, G, gsub, sl, walk);
 
-        for (int i = 0; i < prm.I; ++i) {
-            const int slot = i * sites_per_iter + lw * spw + sl;
-            const int64_t site = tile_site0 + slot;
-            const bool valid = site < prm.site_end;
-            const bool owner = valid && (gsub == 0);
-            // a slot past the data reads no code (the stage holds a previous tile's there) and walks nothing
-            const uint32_t code = UNI ? (valid ? (uint32_t)reinterpret_cast<const uint16_t*>(tile + codes_off)[slot]
-                                               : (UNI_CODE | PG_CLS_MISSING))
-                                      : 0u;
-            const bool uni = UNI && (code & UNI_CODE);
-            const int ri = UNI ? (uni ? 0 : (int)code) : (valid ? slot : 0);
-            const uint32_t* row = reinterpret_cast<const uint32_t*>(tile + (size_t)ri * prm.pitch);
-            const int posv = owner ? reinterpret_cast<const int32_t*>(tile + (size_t)prm.T * prm.pitch)[slot] : 0;
+        for (int it = team; it < ntiles; it += nteams) {
+            const int stage = it % prm.stages;
+            if (lane == 0)
+                while (atomicAdd(const_cast<int*>(s_issued), 0) <= it) __nanosleep(20);
+            __syncwarp();
+            mbar_wait(&full[stage], (uint32_t)((it / prm.stages) & 1));
+            const uint8_t* tile = tiles + (size_t)stage * prm.tile_bytes;
+            const int64_t tile_site0 = prm.site_begin + (t0 + it) * prm.T;
 
-            uint32_t n[P], c[P][4];
-#pragma unroll
-            for (int X = 0; X < P; ++X) {
-                uint32_t a = 0u, a1 = 0u, a2 = 0u, a3 = 0u;
-                const int lo = prm.ent_lo[X], span = prm.ent_hi[X] - lo;
-                int e = (int)(walk[X] & 0xffffu);
-                const int cnt = uni ? 0 : (int)(walk[X] >> 16);
-                for (int k = 0; k < cnt; ++k) {
-                    const uint2 em = s_ent[e];
-                    const uint32_t m = row[em.x] & em.y;
-                    const uint32_t b0 = row[wd + em.x], b1 = row[2 * wd + em.x];
-                    a += __popc(m);
-                    a1 += __popc(m & b0);
-                    a2 += __popc(m & b1);
-                    a3 += __popc(m & b0 & b1);
-                    e += G;
-                    if (e >= lo + span) e -= span;
+            for (int i = 0; i < prm.I; ++i) {
+                const int slot = i * sites_per_iter + lw * spw + sl;
+                const int64_t site = tile_site0 + slot;
+                const bool valid = site < prm.site_end;
+                const bool owner = valid && (gsub == 0);
+                const uint32_t* row = reinterpret_cast<const uint32_t*>(tile + (size_t)(valid ? slot : 0) * prm.pitch);
+                const int posv = owner ? reinterpret_cast<const int32_t*>(tile + (size_t)prm.T * prm.pitch)[slot] : 0;
+
+                ArrCounts<P> ct;
+                packed_counts<P>(prm, s_ent, row, walk, G, spw, ct);
+
+                // ---- segment bookkeeping (warp-uniform control flow), as in k1_site_pass ----
+                int sg = cur_seg;
+                if (owner && site >= seg_end) sg = find_seg(prm.brk, prm.nseg, cur_seg + 1, site);
+                if (__any_sync(0xffffffffu, sg != cur_seg)) {
+                    warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+                    since_flush = 0;
+                    if (sg != cur_seg) {
+                        cur_seg = sg;
+                        seg_end = __ldg(prm.brk + sg + 1);
+                    }
                 }
-                // combine the G lanes of this site (16-bit fields: counts < 65536)
-                uint32_t p0 = a | (a1 << 16), p1 = a2 | (a3 << 16);
-                for (int d = spw; d < 32; d <<= 1) {
-                    p0 += __shfl_xor_sync(0xffffffffu, p0, d);
-                    p1 += __shfl_xor_sync(0xffffffffu, p1, d);
+                bool pres, ragged;
+                packed_class<P>(prm, owner, ct, pres, ragged);
+                if (++since_flush > prm.acc_limit) {      // the 32-bit sums must not overflow
+                    warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+                    since_flush = 1;
                 }
-                const uint32_t nn = p0 & 0xffffu, n1 = p0 >> 16, n2 = p1 & 0xffffu, n3 = p1 >> 16;
-                n[X] = nn;
-                c[X][0] = nn - n1 - n2 + n3;
-                c[X][1] = n1 - n3;
-                c[X][2] = n2 - n3;
-                c[X][3] = n3;
-                if (uni) {
-                    const uint32_t cls = code & 7u, N = (uint32_t)prm.popN[X];
-                    n[X] = cls == PG_CLS_MISSING ? 0u : N;
-#pragma unroll
-                    for (int al = 0; al < 4; ++al) c[X][al] = cls == (uint32_t)(PG_CLS_A + al) ? N : 0u;
-                }
+                acc.i[2] += (long long)posv;
+                packed_add<MODE, P>(acc, pres, ragged, ct);
             }
 
-            // ---- segment bookkeeping (warp-uniform control flow), as in k1_site_pass ----
-            int sg = cur_seg;
-            if (owner && site >= seg_end) sg = find_seg(prm.brk, prm.nseg, cur_seg + 1, site);
-            if (__any_sync(0xffffffffu, sg != cur_seg)) {
-                warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
-                since_flush = 0;
-                if (sg != cur_seg) {
-                    cur_seg = sg;
-                    seg_end = __ldg(prm.brk + sg + 1);
-                }
-            }
-
-            bool allpres = true, allmiss = true;
-#pragma unroll
-            for (int X = 0; X < P; ++X) {
-                allpres = allpres && (n[X] == (uint32_t)prm.popN[X]);
-                allmiss = allmiss && (n[X] == 0u);
-            }
-            const bool pres = owner && allpres;
-            const bool ragged = owner && !allpres && !allmiss;
-            if (++since_flush > prm.acc_limit) {      // the 32-bit sums must not overflow
-                warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
-                since_flush = 1;
-            }
-            acc.i[0] += pres ? 1 : 0;
-            acc.i[1] += ragged ? 1 : 0;
-            acc.i[2] += (long long)posv;
-            const uint32_t f = pres ? 1u : 0u;
-#pragma unroll
-            for (int X = 0; X < P; ++X) {
-                const uint32_t sq = c[X][0] * c[X][0] + c[X][1] * c[X][1] + c[X][2] * c[X][2] + c[X][3] * c[X][3];
-                acc.u[X] += sq * f;
-                if (MODE == MODE_POPGEN_FREQ) acc.u[P + P * (P - 1) / 2 + X] += (pres && sq != n[X] * n[X]) ? 1u : 0u;
-            }
-            int k = 0;
-#pragma unroll
-            for (int X = 0; X < P; ++X)
-#pragma unroll
-                for (int Y = X + 1; Y < P; ++Y) {
-                    const uint32_t cr = c[X][0] * c[Y][0] + c[X][1] * c[Y][1] + c[X][2] * c[Y][2] + c[X][3] * c[Y][3];
-                    acc.u[P + k] += cr * f;
-                    ++k;
-                }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[stage]);
         }
+    } else {
+        const size_t codes_off = (size_t)prm.T * (prm.pitch + 4);
+        const int spv = 32 / Gv, gsub = lane / spv, sl = lane % spv;
+        // Register budget: with 8 populations walk[] lives in shared memory and the counts are expanded once; with fewer, walk[]
+        // stays in registers and the counts stay two words per population (the choices with the fewest spills, ptxas sm_90a)
+        std::conditional_t<P == 8, SmemWalk, RegWalk<P>> walk;
+        if constexpr (P == 8) walk.p = s_walk + lane;
+        else packed_walk<P>(prm, Gv, gsub, sl, walk.w);
 
+        for (int it = team; it < ntiles; it += nteams) {
+            const int stage = it % prm.stages;
+            if (lane == 0)
+                while (atomicAdd(const_cast<int*>(s_issued), 0) <= it) __nanosleep(20);
+            __syncwarp();
+            mbar_wait(&full[stage], (uint32_t)((it / prm.stages) & 1));
+            const uint8_t* tile = tiles + (size_t)stage * prm.tile_bytes;
+            const int64_t tile_site0 = prm.site_begin + (t0 + it) * prm.T;
+            const int nvar = s_nvar[stage];
+            const uint16_t* s_slot = reinterpret_cast<const uint16_t*>(tile + codes_off) + prm.code_pitch;
+
+            // ---- pass V: blocks of spv varied rows, block k to warp k % wpt, so a lane's rows stay in site order ----
+            for (int r = lw * spv; r < nvar; r += prm.wpt * spv) {
+                const int rw = r + sl;
+                const bool valid = rw < nvar;
+                const bool owner = valid && (gsub == 0);
+                const uint32_t* row = reinterpret_cast<const uint32_t*>(tile + (size_t)(valid ? rw : r) * prm.pitch);
+                std::conditional_t<P == 8, ArrCounts<P>, PkCounts<P>> ct;
+                packed_counts<P>(prm, s_ent, row, walk, Gv, spv, ct);
+
+                const int64_t site = tile_site0 + (valid ? s_slot[rw] : 0);
+                int sg = cur_seg;
+                if (owner && site >= seg_end) sg = find_seg(prm.brk, prm.nseg, cur_seg + 1, site);
+                if (__any_sync(0xffffffffu, sg != cur_seg)) {
+                    warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+                    since_flush = 0;
+                    // A lane that owns no row here (a row's other lanes, lanes past the block) would keep an old segment
+                    // and flush the warp once more when it next owns one.  Its sums are zero now and none of its later
+                    // sites comes before the warp's sites here, so it takes the warp's last segment.
+                    const int last = __reduce_max_sync(0xffffffffu, sg);
+                    const int to = owner ? sg : last;
+                    if (to != cur_seg) {
+                        cur_seg = to;
+                        seg_end = __ldg(prm.brk + to + 1);
+                    }
+                }
+                bool pres, ragged;
+                packed_class<P>(prm, owner, ct, pres, ragged);
+                if (++since_flush > prm.acc_limit) {      // the 32-bit sums must not overflow
+                    warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+                    since_flush = 1;
+                }
+                packed_add<MODE, P>(acc, pres, ragged, ct);
+            }
+
+            // ---- pass U: every slot of the tile, 32 per iteration, one lane each, no walk.  The warps that walked no row take
+            // the iterations when they are at most two each, the whole team otherwise.  The lanes of an iteration hold
+            // increasing sites, so those before the warp's segment end are a prefix of them ----
+            const int vw = min(prm.wpt, (nvar + spv - 1) / spv), nit = (prm.T + 31) / 32;
+            const bool idle_only = vw < prm.wpt && nit <= 2 * (prm.wpt - vw);
+            const uint16_t* s_code = reinterpret_cast<const uint16_t*>(tile + codes_off);
+            const int uw = idle_only ? prm.wpt - vw : prm.wpt, ul = idle_only ? lw - vw : lw;
+            UniRec& ur = s_urec[warp];
+            int useg = ur.seg;
+            int64_t useg_end = ur.seg_end;
+            long long upos = ur.pos;
+            uint32_t upres = ur.npres;
+            for (int j0 = ul * 32; ul >= 0 && j0 < prm.T; j0 += uw * 32) {
+                const int j = j0 + lane;
+                const int64_t site = tile_site0 + j;
+                const bool valid = j < prm.T && site < prm.site_end;
+                uint32_t code = UNI_CODE | PG_CLS_MISSING;
+                int posv = 0;
+                if (valid) {
+                    code = s_code[j];
+                    posv = reinterpret_cast<const int32_t*>(tile + (size_t)prm.T * prm.pitch)[j];
+                }
+                const unsigned up = __ballot_sync(0xffffffffu, (code & UNI_CODE) && (code & 7u) != PG_CLS_MISSING);
+                unsigned left = __ballot_sync(0xffffffffu, valid);
+                while (true) {
+                    const unsigned in = __ballot_sync(0xffffffffu, site < useg_end) & left;
+                    upres += __popc(up & in);
+                    upos += warp_sum_i32((in >> lane) & 1u ? posv : 0);
+                    left &= ~in;
+                    if (!left) break;
+                    if (useg >= 0) {
+                        uniform_flush<MODE, P>(prm, useg, upres, upos, slot_base, seg_first, warp, lane, NW);
+                        upres = 0u;
+                        upos = 0ll;
+                    }
+                    useg = find_seg(prm.brk, prm.nseg, useg + 1, __shfl_sync(0xffffffffu, site, __ffs(left) - 1));
+                    useg_end = __ldg(prm.brk + useg + 1);
+                }
+            }
+            __syncwarp();
+            if (lane == 0) {
+                ur = UniRec{upos, useg_end, useg, upres};
+                mbar_arrive(&empty[stage]);
+            }
+        }
         __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[stage]);
+        const UniRec ur = s_urec[warp];
+        if (ur.seg >= 0) uniform_flush<MODE, P>(prm, ur.seg, ur.npres, ur.pos, slot_base, seg_first, warp, lane, NW);
     }
     warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
 }
@@ -1491,7 +1713,8 @@ int push(pg_ctx* ctx, uint8_t* base, size_t& off, const T* src, size_t n, T** ou
 // ---- the packed rows of the varied sites only (DESIGN.md "Uniform sites") -------------------------------------------
 // Derived from the companion and its site classes (ctx->d_site_cls) for one data generation and tile size T: per tile the
 // index of its first varied row (row0, int64 [tiles + 1]), a 16-bit code per site (UNI_CODE | class, or the rank among the
-// tile's varied sites; tile t's T codes at t * code_pitch) and the varied rows, contiguous.
+// tile's varied sites; tile t's T codes at t * 2 * code_pitch), the slot (index in the tile) of each of a tile's varied rows,
+// behind its codes, and the varied rows, contiguous.
 struct UniformStream {
     uint64_t gen = 0;         // ctx->data_gen it describes (0: none)
     int T = 0;
@@ -1521,7 +1744,7 @@ __global__ void __launch_bounds__(256) k1_uni_count(const uint8_t* __restrict__ 
     if (threadIdx.x == 0) cnt[blockIdx.x] = s_n;
 }
 
-// codes of tile blockIdx.x, and the source site of each of its varied rows
+// codes of tile blockIdx.x, and the slot and the source site of each of its varied rows
 __global__ void __launch_bounds__(256) k1_uni_codes(const uint8_t* __restrict__ cls, int64_t S, int T, int code_pitch,
                                                     const int64_t* __restrict__ row0, uint16_t* __restrict__ codes,
                                                     int64_t* __restrict__ src) {
@@ -1537,8 +1760,11 @@ __global__ void __launch_bounds__(256) k1_uni_codes(const uint8_t* __restrict__ 
         int rank, total;
         Scan(tmp).ExclusiveSum(v, rank, total);
         __syncthreads();
-        if (j < code_pitch) codes[t * code_pitch + j] = (uint16_t)(v ? (uint32_t)(base + rank) : (UNI_CODE | k));
-        if (v) src[r0 + base + rank] = s;
+        if (j < code_pitch) codes[t * 2 * code_pitch + j] = (uint16_t)(v ? (uint32_t)(base + rank) : (UNI_CODE | k));
+        if (v) {
+            codes[(t * 2 + 1) * code_pitch + base + rank] = (uint16_t)j;
+            src[r0 + base + rank] = s;
+        }
         base += total;
     }
 }
@@ -1787,10 +2013,11 @@ int launch_site_pass_packed(pg_ctx* ctx, const K1Launch& L, const char* name) {
     return launch_site_pass_packed_nw<MODE, P, 8, UNI>(ctx, L, name);
 }
 
-// Streaming only the varied rows costs 6 + (1 - u) * pitch bytes per site against 4 + pitch, for a uniform fraction u, plus a
-// rebuild whenever the data change.  tools/packed_site_pass.py --sweep times the two passes across u at the C2 shape (H100
-// SXM, 700 W): 0.48 against 0.54 ms at u = 20 %, 0.50 against 0.54 at 10 %, 0.52 against 0.54 at 5 %, 0.55 against 0.54 at
-// 1 %.  The stream is kept from u >= 1/8 on, where its gain is clear of the run-to-run spread.
+// Streaming only the varied rows costs 6 + (1 - u) * (pitch + 2) bytes per site (position, code; row, slot) against
+// 4 + pitch, for a uniform fraction u, plus a rebuild whenever the data change.  tools/packed_site_pass.py --sweep times the
+// two passes across u at the C2 shape (H100 80GB HBM3, 700 W): 0.48 against 0.55 ms at u = 20 %, 0.52 against 0.55 at 10 %,
+// 0.553 against 0.555 at 5 %, 0.57 against 0.555 at 1 %.  The stream is kept from u >= 1/8 on, where its gain is clear of the
+// run-to-run spread.
 constexpr double UNI_MIN_FRACTION = 0.125;
 
 // (Re)builds c.us for the current data and plan when they changed: one host synchronisation per rebuild, nothing on a
@@ -1827,7 +2054,8 @@ int uniform_prepare(pg_ctx* ctx, K1Cache& c) {
     if (!forced && (double)(ctx->S - varied) < UNI_MIN_FRACTION * (double)ctx->S) return PG_OK;
     us.code_pitch = (pl.T + 7) / 8 * 8;
     const int chunks = ctx->packed_pitch / 16;
-    if (us.codes.ensure((size_t)nt * us.code_pitch * 2) != PG_OK || us.src.ensure((size_t)std::max<int64_t>(varied, 1) * 8) != PG_OK ||
+    if (us.codes.ensure((size_t)nt * us.code_pitch * 4) != PG_OK ||
+        us.src.ensure((size_t)std::max<int64_t>(varied, 1) * 8) != PG_OK ||
         us.rows.ensure((size_t)std::max<int64_t>(varied, 1) * ctx->packed_pitch) != PG_OK) {
         cudaGetLastError();                   // no memory for the stream: the packed pass streams every row
         us.rows.release();
@@ -1965,7 +2193,8 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
             c.lanepop = false;
             const int nw = k1_nw_for(ctx->packed_pitch);
             PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, 0, true));
-            c.uplan = pg_make_k1_plan_rows(ctx->S, ctx->packed_pitch, ctx->sm_count, table_bytes_of(c.pt), nw, 0, 2);
+            c.uplan = pg_make_k1_plan_rows(ctx->S, ctx->packed_pitch, ctx->sm_count, table_bytes_of(c.pt) + UNI_SMEM_BYTES, nw, 0,
+                                           4);
             if (!pg_k1_plan_ok(c.uplan)) c.uplan.stages = 0;    // no room for the codes: every row is streamed
         } else {
             // long rows, 4 or 8 real populations of <= 255 haplotypes: one lane per population (k1_site_pass_lp)
@@ -2014,6 +2243,10 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
         UL.prm.row0 = (const int64_t*)c.us.row0.p;
         UL.prm.codes = (const uint16_t*)c.us.codes.p;
         UL.prm.code_pitch = c.us.code_pitch;
+        const char* gv = getenv("PG_K1_UNI_GV");           // test hook: lanes per varied row (1, 2, 4, ... 32)
+        UL.prm.uni_gv = gv && *gv ? atoi(gv) : 0;
+        PG_CHECK(UL.prm.uni_gv >= 0 && UL.prm.uni_gv <= 32 && (UL.prm.uni_gv & (UL.prm.uni_gv - 1)) == 0,
+                 "PG_K1_UNI_GV must be a power of two up to 32");
         if (!wf) {
             if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 2, true>(ctx, UL, "k1_popgen")));
             else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 4, true>(ctx, UL, "k1_popgen")));
@@ -2079,6 +2312,15 @@ extern "C" int pg_debug_uniform(pg_ctx* ctx, int32_t* in_use, int64_t* varied_si
     const bool read = c && c->uni_last;
     *in_use = read ? 1 : 0;
     *varied_sites = (c && c->us.gen == ctx->data_gen) ? c->us.varied : ctx->S;
+    return PG_OK;
+}
+
+extern "C" int pg_debug_uniform_tile(pg_ctx* ctx, int32_t* out) {
+    PG_CHECK(ctx && out, "pg_debug_uniform_tile: null argument");
+    const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
+    const bool planned = c && c->valid && c->packed;
+    out[0] = planned ? c->uplan.T : 0;
+    out[1] = planned ? c->uplan.wpt : 0;
     return PG_OK;
 }
 

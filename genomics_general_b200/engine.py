@@ -562,6 +562,13 @@ class Engine:
         check(self._lib.pg_debug_uniform(self._ctx, C.byref(in_use), C.byref(varied)), "pg_debug_uniform")
         return bool(in_use.value), int(varied.value)
 
+    def uniform_tile(self):
+        """(sites per tile, warps per tile) of the varied-row stream's launch plan, as the last popgen call on the packed
+        companion made it ((0, 0) before any)."""
+        v = (C.c_int32 * 2)()
+        check(self._lib.pg_debug_uniform_tile(self._ctx, v), "pg_debug_uniform_tile")
+        return int(v[0]), int(v[1])
+
 
 def k1_plan(S: int, H: int, nw: int = 8, lanes: int = 0, table_bytes: int = 4096):
     """Host-only: the site-pass launch geometry for a shape (works without a GPU).  `nw` consumer warps per CTA (8, or 12

@@ -300,6 +300,9 @@ int pg_debug_packed(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* row_words, u
  * rows of sites whose haplotypes are not all the same (0: every packed row), *varied_sites = the varied sites it counted
  * (S when it did not count them). */
 int pg_debug_uniform(pg_ctx* ctx, int32_t* in_use, int64_t* varied_sites);
+/* Tile geometry of the varied-row stream after a popgen call: out[0] = sites per tile, out[1] = warps per tile (0 before any
+ * popgen call on the packed companion). */
+int pg_debug_uniform_tile(pg_ctx* ctx, int32_t* out);
 
 #ifdef __cplusplus
 }
