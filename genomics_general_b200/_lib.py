@@ -90,6 +90,9 @@ _SIGS = {
     "pg_debug_packed": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int32), C.c_void_p]),
     "pg_debug_uniform": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
     "pg_debug_uniform_tile": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
+    "pg_debug_uniform_ring": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
+    "pg_debug_uniform_tiles": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
+                                         C.POINTER(C.c_int32)]),
     "pg_nccl_unique_id": (C.c_int, [C.c_void_p]),
     "pg_nccl_init": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "pg_nccl_finalize": (C.c_int, [C.c_void_p]),

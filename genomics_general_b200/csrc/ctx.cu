@@ -280,12 +280,19 @@ K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw, 
     return pg_make_k1_plan_rows(S, pg_pitch_for(H), sm_count, table_bytes, nw, force_G);
 }
 
+// stages of tile_bytes each in the per-CTA dynamic shared memory we allow ourselves, at most 8 (PG_K1_STAGES lowers it)
+int pg_k1_ring_stages(int tile_bytes, int table_bytes) {
+    const int smem_cap = 227 * 1024 - 2048 - table_bytes;
+    int stages = smem_cap / tile_bytes;
+    if (stages > 8) stages = 8;
+    return std::min(stages, std::max(2, env_int("PG_K1_STAGES", stages)));
+}
+
 K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G, int code_bytes) {
     K1Plan p;
     memset(&p, 0, sizeof(p));
     p.pitch = pitch;
     p.chunks = p.pitch / 16;
-    const int smem_cap = 227 * 1024 - 2048 - table_bytes;   // per-CTA dynamic smem we allow ourselves
     const int tile_target = env_int("PG_K1_TILE_KB", 64) * 1024;
     int G = 1, wpt = 1, I = 1;
     // lanes per site: keep one lane's walk below ~64 chunks (long rows are shared by G lanes; PG_K1_G overrides),
@@ -315,10 +322,7 @@ K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes,
     // genotype rows + the tile's positions (+ code_bytes per site for its codes, in arrays of 2 bytes per site padded to
     // 16-byte pieces)
     p.tile_bytes = ((p.T * p.pitch + p.T * 4 + code_bytes * ((p.T + 7) / 8 * 8) + 127) / 128) * 128;
-    int stages = smem_cap / p.tile_bytes;
-    if (stages > 8) stages = 8;
-    stages = std::min(stages, std::max(2, env_int("PG_K1_STAGES", stages)));
-    p.stages = stages;                      // < 2 means the row is too long for this kernel
+    p.stages = pg_k1_ring_stages(p.tile_bytes, table_bytes);   // < 2 means the row is too long for this kernel
     p.smem_bytes = p.stages * p.tile_bytes + 256 + table_bytes;
     p.num_tiles = (S + p.T - 1) / p.T;
     int64_t ctas = sm_count;

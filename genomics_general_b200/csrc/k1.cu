@@ -48,11 +48,16 @@ struct K1Params {
     int wd;
     // packed pass with uniform sites elided (UniformStream): geno holds only the varied rows, tile t's being rows
     // [row0[t], row0[t + 1]); codes holds tile t's 16-bit codes, one per site, at t * 2 * code_pitch, and code_pitch further
-    // the site index in the tile (slot) of each of its varied rows; uni_gv > 0 forces the lanes per varied row (PG_K1_UNI_GV)
+    // the site index in the tile (slot) of each of its varied rows; uni_gv > 0 forces the lanes per varied row (PG_K1_UNI_GV).
+    // Tile t covers the sites [site_lo[t], site_lo[t + 1]): at most T (Tmax) of them and at most row_cap (R) varied rows.  A
+    // stage holds row_cap rows, then the positions from the tile's first site rounded down to 4 (T + 4 of them), then its
+    // codes and slots.
     const int64_t* row0;
+    const int64_t* site_lo;
     const uint16_t* codes;
     int code_pitch;
     int uni_gv;
+    int row_cap;
     // segments / slots
     const int64_t* brk;
     int nseg;
@@ -334,7 +339,9 @@ __device__ __forceinline__ void k1_producer(const K1Params& prm, uint8_t* tiles,
 }
 
 // Producer of the packed pass over the varied rows only (the whole producer warp): a tile is its varied rows
-// [row0[t], row0[t + 1]), then its T positions, then its codes (code_pitch of them) and the slots of its varied rows.  The
+// [row0[t], row0[t + 1]) (room for row_cap of them), then the positions of its sites [site_lo[t], site_lo[t + 1]) from the first
+// one rounded down to a multiple of 4 (bulk copies take 16-byte-aligned sources; the consumers apply the offset), then its
+// codes (code_pitch of them) and the slots of its varied rows.  The
 // count of varied rows goes to s_nvar[stage] before the stage is armed, so the mbarrier's phase publishes it.  A tile is
 // about a microsecond of HBM time, as long as a dependent load of row0, so the 32 lanes load the offsets of the next 32 tiles
 // while the current 32 are issued.
@@ -342,21 +349,23 @@ __device__ __forceinline__ void k1_producer_uniform(const K1Params& prm, uint8_t
                                                     volatile int* s_issued, volatile int* s_nvar, int ntiles, int64_t t0,
                                                     int lane) {
     auto ld_row0 = [&](int64_t t) { return t <= prm.num_tiles ? __ldg(prm.row0 + t) : (int64_t)0; };
-    int64_t cur = ld_row0(t0 + lane);            // lane l: row0 of tile t0 + g + l
+    auto ld_site = [&](int64_t t) { return t <= prm.num_tiles ? __ldg(prm.site_lo + t) : (int64_t)0; };
+    int64_t cur = ld_row0(t0 + lane), cur_s = ld_site(t0 + lane);       // lane l: row0 and site_lo of tile t0 + g + l
     for (int g = 0; g < ntiles; g += 32) {
-        const int64_t nxt = ld_row0(t0 + g + 32 + lane);
+        const int64_t nxt = ld_row0(t0 + g + 32 + lane), nxt_s = ld_site(t0 + g + 32 + lane);
         const int kn = min(32, ntiles - g);
         for (int k = 0; k < kn; ++k) {
             const int64_t r0 = __shfl_sync(0xffffffffu, cur, k);
             const int64_t r1 = k < 31 ? __shfl_sync(0xffffffffu, cur, k + 1) : __shfl_sync(0xffffffffu, nxt, 0);
+            const int64_t s0 = __shfl_sync(0xffffffffu, cur_s, k);
+            const int64_t s1 = k < 31 ? __shfl_sync(0xffffffffu, cur_s, k + 1) : __shfl_sync(0xffffffffu, nxt_s, 0);
             if (lane == 0) {
                 const int it = g + k;
                 const int stage = it % prm.stages;
                 if (it >= prm.stages) mbar_wait(&empty[stage], (uint32_t)(((it / prm.stages) - 1) & 1));
                 const int64_t tile = t0 + it;
-                const int64_t s_lo = prm.site_begin + tile * prm.T;
-                int64_t rows = prm.site_end - s_lo;
-                if (rows > prm.T) rows = prm.T;
+                const int64_t s_lo = s0 & ~(int64_t)3;
+                const int64_t rows = s1 - s_lo;
                 const int nvar = (int)(r1 - r0);
                 const uint32_t bytes = (uint32_t)(nvar * prm.pitch);
                 const uint32_t pbytes = (uint32_t)(((rows * 4 + 15) / 16) * 16);
@@ -369,14 +378,16 @@ __device__ __forceinline__ void k1_producer_uniform(const K1Params& prm, uint8_t
                     const uint32_t n = (bytes - off) < 32768u ? (bytes - off) : 32768u;
                     bulk_g2s(dst + off, src + off, n, &full[stage]);
                 }
-                bulk_g2s(dst + (size_t)prm.T * prm.pitch, prm.pos + s_lo, pbytes, &full[stage]);
-                bulk_g2s(dst + (size_t)prm.T * (prm.pitch + 4), prm.codes + tile * 2 * prm.code_pitch, cbytes, &full[stage]);
+                const size_t pos_off = (size_t)prm.row_cap * prm.pitch;
+                bulk_g2s(dst + pos_off, prm.pos + s_lo, pbytes, &full[stage]);
+                bulk_g2s(dst + pos_off + (size_t)(prm.T + 4) * 4, prm.codes + tile * 2 * prm.code_pitch, cbytes, &full[stage]);
                 __threadfence_block();
                 atomicExch(const_cast<int*>(s_issued), it + 1);
             }
             __syncwarp();
         }
         cur = nxt;
+        cur_s = nxt_s;
     }
 }
 
@@ -1259,7 +1270,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             if (lane == 0) mbar_arrive(&empty[stage]);
         }
     } else {
-        const size_t codes_off = (size_t)prm.T * (prm.pitch + 4);
+        const size_t pos_off = (size_t)prm.row_cap * prm.pitch, codes_off = pos_off + (size_t)(prm.T + 4) * 4;
         const int spv = 32 / Gv, gsub = lane / spv, sl = lane % spv;
         // Register budget: with 8 populations walk[] lives in shared memory and the counts are expanded once; with fewer, walk[]
         // stays in registers and the counts stay two words per population (the choices with the fewest spills, ptxas sm_90a)
@@ -1274,7 +1285,9 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             __syncwarp();
             mbar_wait(&full[stage], (uint32_t)((it / prm.stages) & 1));
             const uint8_t* tile = tiles + (size_t)stage * prm.tile_bytes;
-            const int64_t tile_site0 = prm.site_begin + (t0 + it) * prm.T;
+            const int64_t tile_site0 = __ldg(prm.site_lo + t0 + it);
+            const int nsites = (int)(__ldg(prm.site_lo + t0 + it + 1) - tile_site0);
+            const int32_t* s_pos = reinterpret_cast<const int32_t*>(tile + pos_off) + (tile_site0 & 3);
             const int nvar = s_nvar[stage];
             const uint16_t* s_slot = reinterpret_cast<const uint16_t*>(tile + codes_off) + prm.code_pitch;
 
@@ -1315,7 +1328,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             // ---- pass U: every slot of the tile, 32 per iteration, one lane each, no walk.  The warps that walked no row take
             // the iterations when they are at most two each, the whole team otherwise.  The lanes of an iteration hold
             // increasing sites, so those before the warp's segment end are a prefix of them ----
-            const int vw = min(prm.wpt, (nvar + spv - 1) / spv), nit = (prm.T + 31) / 32;
+            const int vw = min(prm.wpt, (nvar + spv - 1) / spv), nit = (nsites + 31) / 32;
             const bool idle_only = vw < prm.wpt && nit <= 2 * (prm.wpt - vw);
             const uint16_t* s_code = reinterpret_cast<const uint16_t*>(tile + codes_off);
             const int uw = idle_only ? prm.wpt - vw : prm.wpt, ul = idle_only ? lw - vw : lw;
@@ -1324,15 +1337,15 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             int64_t useg_end = ur.seg_end;
             long long upos = ur.pos;
             uint32_t upres = ur.npres;
-            for (int j0 = ul * 32; ul >= 0 && j0 < prm.T; j0 += uw * 32) {
+            for (int j0 = ul * 32; ul >= 0 && j0 < nsites; j0 += uw * 32) {
                 const int j = j0 + lane;
                 const int64_t site = tile_site0 + j;
-                const bool valid = j < prm.T && site < prm.site_end;
+                const bool valid = j < nsites;
                 uint32_t code = UNI_CODE | PG_CLS_MISSING;
                 int posv = 0;
                 if (valid) {
                     code = s_code[j];
-                    posv = reinterpret_cast<const int32_t*>(tile + (size_t)prm.T * prm.pitch)[j];
+                    posv = s_pos[j];
                 }
                 const unsigned up = __ballot_sync(0xffffffffu, (code & UNI_CODE) && (code & 7u) != PG_CLS_MISSING);
                 unsigned left = __ballot_sync(0xffffffffu, valid);
@@ -1711,62 +1724,115 @@ int push(pg_ctx* ctx, uint8_t* base, size_t& off, const T* src, size_t n, T** ou
 }
 
 // ---- the packed rows of the varied sites only (DESIGN.md "Uniform sites") -------------------------------------------
-// Derived from the companion and its site classes (ctx->d_site_cls) for one data generation and tile size T: per tile the
-// index of its first varied row (row0, int64 [tiles + 1]), a 16-bit code per site (UNI_CODE | class, or the rank among the
-// tile's varied sites; tile t's T codes at t * 2 * code_pitch), the slot (index in the tile) of each of a tile's varied rows,
-// behind its codes, and the varied rows, contiguous.
+// Derived from the companion and its site classes (ctx->d_site_cls) for one data generation, row budget R and tile bound
+// Tmax.  Tiles are cut by a budget of varied rows: group k holds the varied rows of ranks [k R, (k + 1) R) and runs from the
+// site of rank k R (site 0 for k = 0) to the next group's; a group of more than Tmax sites is split into pieces of Tmax.  So a
+// tile has at most R varied rows and at most Tmax sites, and tile t covers the sites [site_lo[t], site_lo[t + 1]).  Per tile:
+// the index of its first varied row (row0, int64 [tiles + 1]), a 16-bit code per site (UNI_CODE | class, or the rank among the
+// tile's varied sites; tile t's codes at t * 2 * code_pitch, code_pitch = Tmax), the slot (index in the tile) of each of its
+// varied rows, behind its codes; and the varied rows, contiguous.  bound holds the first site of each CTA's tiles (B + 1).
 struct UniformStream {
     uint64_t gen = 0;         // ctx->data_gen it describes (0: none)
-    int T = 0;
+    uint64_t serial = 0;      // counts the builds (the slot tables follow it)
+    int R = 0, Tmax = 0;
     bool forced = false;
     bool in_use = false;      // false: too few uniform sites to pay off, or no memory; the packed pass streams every row
     int64_t varied = 0;
+    int64_t nt = 0;           // tiles
     int code_pitch = 0;
-    PgBuf cnt, row0, codes, src, rows, scan;
+    std::vector<int64_t> bound;
+    PgBuf cnt, row0, codes, src, rows, scan, site_lo, groups, info;
     void release() {
-        for (PgBuf* b : {&cnt, &row0, &codes, &src, &rows, &scan}) b->release();
+        for (PgBuf* b : {&cnt, &row0, &codes, &src, &rows, &scan, &site_lo, &groups, &info}) b->release();
         gen = 0;
     }
 };
 
-// varied sites per tile
-__global__ void __launch_bounds__(256) k1_uni_count(const uint8_t* __restrict__ cls, int64_t S, int T, int64_t* __restrict__ cnt) {
+// varied sites per tile: tile t is [site_lo[t], site_lo[t + 1]), or the T sites from t * T when site_lo is null
+__global__ void __launch_bounds__(256) k1_uni_count(const uint8_t* __restrict__ cls, int64_t S, const int64_t* __restrict__ site_lo,
+                                                    int T, int64_t* __restrict__ cnt) {
     __shared__ int s_n;
     if (threadIdx.x == 0) s_n = 0;
     __syncthreads();
-    const int64_t s0 = (int64_t)blockIdx.x * T;
+    const int64_t s0 = site_lo ? site_lo[blockIdx.x] : (int64_t)blockIdx.x * T;
+    const int64_t len = site_lo ? site_lo[blockIdx.x + 1] - s0 : (S - s0 < T ? S - s0 : (int64_t)T);
     int n = 0;
-    for (int j = threadIdx.x; j < T; j += blockDim.x)
-        if (s0 + j < S && cls[s0 + j] == PG_CLS_VARIED) ++n;
+    for (int j = threadIdx.x; j < len; j += blockDim.x)
+        if (cls[s0 + j] == PG_CLS_VARIED) ++n;
     n = __reduce_add_sync(0xffffffffu, n);
     if ((threadIdx.x & 31) == 0) atomicAdd(&s_n, n);
     __syncthreads();
     if (threadIdx.x == 0) cnt[blockIdx.x] = s_n;
 }
 
-// codes of tile blockIdx.x, and the slot and the source site of each of its varied rows
-__global__ void __launch_bounds__(256) k1_uni_codes(const uint8_t* __restrict__ cls, int64_t S, int T, int code_pitch,
-                                                    const int64_t* __restrict__ row0, uint16_t* __restrict__ codes,
-                                                    int64_t* __restrict__ src) {
+// codes of tile blockIdx.x (tiles as in k1_uni_count; none when codes is null), and the slot and the source site of each of its
+// varied rows
+__global__ void __launch_bounds__(256) k1_uni_codes(const uint8_t* __restrict__ cls, int64_t S, const int64_t* __restrict__ site_lo,
+                                                    int T, int code_pitch, const int64_t* __restrict__ row0,
+                                                    uint16_t* __restrict__ codes, int64_t* __restrict__ src) {
     typedef cub::BlockScan<int, 256> Scan;
     __shared__ typename Scan::TempStorage tmp;
-    const int64_t t = blockIdx.x, s0 = t * T, r0 = row0[t];
+    const int64_t t = blockIdx.x, r0 = row0[t];
+    const int64_t s0 = site_lo ? site_lo[t] : t * T;
+    const int64_t len = site_lo ? site_lo[t + 1] - s0 : (S - s0 < T ? S - s0 : (int64_t)T);
     int base = 0;
     for (int j0 = 0; j0 < code_pitch; j0 += 256) {
         const int j = j0 + threadIdx.x;
         const int64_t s = s0 + j;
-        const uint32_t k = (j < T && s < S) ? cls[s] : (uint32_t)PG_CLS_MISSING;
+        const uint32_t k = j < len ? cls[s] : (uint32_t)PG_CLS_MISSING;
         const int v = k == PG_CLS_VARIED ? 1 : 0;
         int rank, total;
         Scan(tmp).ExclusiveSum(v, rank, total);
         __syncthreads();
-        if (j < code_pitch) codes[t * 2 * code_pitch + j] = (uint16_t)(v ? (uint32_t)(base + rank) : (UNI_CODE | k));
+        if (codes && j < code_pitch) codes[t * 2 * code_pitch + j] = (uint16_t)(v ? (uint32_t)(base + rank) : (UNI_CODE | k));
         if (v) {
-            codes[(t * 2 + 1) * code_pitch + base + rank] = (uint16_t)j;
+            if (codes) codes[(t * 2 + 1) * code_pitch + base + rank] = (uint16_t)j;
             src[r0 + base + rank] = s;
         }
         base += total;
     }
+}
+
+// group k's first site (the site of varied rank k R; 0 for k = 0) and end (the next group's first site; S for the last)
+__device__ __forceinline__ void uni_group(const int64_t* src, int R, int64_t S, int64_t ng, int64_t k, int64_t& lo, int64_t& hi) {
+    lo = k == 0 ? 0 : src[k * R];
+    hi = k + 1 < ng ? src[(k + 1) * R] : S;
+}
+
+// pieces of at most tmax sites per group
+__global__ void __launch_bounds__(256) k1_uni_groups(const int64_t* __restrict__ src, int R, int64_t S, int tmax, int64_t ng,
+                                                     int64_t* __restrict__ pieces) {
+    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= ng) return;
+    int64_t lo, hi;
+    uni_group(src, R, S, ng, k, lo, hi);
+    const int64_t n = (hi - lo + tmax - 1) / tmax;
+    pieces[k] = n > 1 ? n : 1;
+}
+
+// site_lo of every tile from the groups' first pieces (base, the exclusive scan of the pieces: base[ng] = tiles); the entries
+// from the last tile on up to nt_max hold S (empty tiles)
+__global__ void __launch_bounds__(256) k1_uni_tiles(const int64_t* __restrict__ src, int R, int64_t S, int tmax, int64_t ng,
+                                                    const int64_t* __restrict__ base, int64_t nt_max, int64_t* __restrict__ site_lo) {
+    const int64_t nt = base[ng];
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= (ng > nt_max ? ng : nt_max);
+         i += (int64_t)gridDim.x * blockDim.x) {
+        if (i < ng) {
+            int64_t lo, hi;
+            uni_group(src, R, S, ng, i, lo, hi);
+            for (int64_t b = base[i], j = 0; b + j < base[i + 1]; ++j) site_lo[b + j] = lo + j * tmax;
+        }
+        if (i >= nt && i <= nt_max) site_lo[i] = S;
+    }
+}
+
+// info[0] = tiles, info[1 + b] = the first site of CTA b's tiles for b = 0 .. B (B = min(sm, tiles) CTAs, tiles b * nt / B on)
+__global__ void __launch_bounds__(256) k1_uni_bounds(const int64_t* __restrict__ base, int64_t ng, const int64_t* __restrict__ site_lo,
+                                                     int sm, int64_t* __restrict__ info) {
+    const int64_t nt = base[ng];
+    const int64_t B = nt < sm ? (nt > 1 ? nt : 1) : sm;
+    for (int64_t b = threadIdx.x; b <= B; b += blockDim.x) info[1 + b] = site_lo[b * nt / B];
+    if (threadIdx.x == 0) info[0] = nt;
 }
 
 // varied row r <- companion row src[r], 16 bytes per thread
@@ -1792,9 +1858,18 @@ struct K1Cache {
     DevTables dt;
     PopTables pt;
     PgBuf tables;
-    K1Plan uplan;             // packed: L.plan with room for the codes in each stage (same T, tiles and CTAs)
+    K1Plan uplan;             // packed: L.plan with room for the codes in each stage (its G, wpt and warps serve the stream)
+    int utable = 0;           // packed: shared-memory bytes of uplan's tables
     UniformStream us;         // packed: the varied rows (popgen cache only)
+    int uR = 0, uTmax = 0, ustages = 0, ubytes = 0;   // the stream's row budget, tile bound, and ring (uni_geometry)
     bool uni_last = false;    // the last popgen launch read us
+    // the slot tables of the stream's CTA ranges (slot_tables), for windows epoch uslots_epoch and build uslots_serial
+    PgBuf uslots;
+    int32_t *u_cta_seg_first = nullptr, *u_seg_cta_lo = nullptr, *u_seg_cta_hi = nullptr;
+    int64_t* u_cta_slot_off = nullptr;
+    int64_t utotal_slots = 0;
+    uint64_t uslots_epoch = 0, uslots_serial = 0;
+    int uslots_Q = 0;
 };
 
 // The one-hot rows' launch plan for this population map, or the error that refuses such rows.
@@ -1807,6 +1882,41 @@ int byte_plan(pg_ctx* ctx, const std::vector<int32_t>& hap_pop_local, int Ppad, 
     PG_CHECK(plan.stages >= 2, "rows of %d haplotypes are too long for the site-pass kernel (pitch %d bytes)", ctx->H,
              plan.pitch);
     return check_plan(plan);
+}
+
+// The slots of a launch whose CTA b adds the sites [bound[b], bound[b + 1]): each CTA gets nw slots of Q words per segment it
+// touches (cta_seg_first, cta_slot_off), and each segment the range of CTAs that touch it (seg_cta_lo / _hi), for k1_finalize.
+// Returns the slot words.
+int64_t slot_tables(const std::vector<int64_t>& brk, const std::vector<int64_t>& bound, int nw, int Q, K1Launch& L) {
+    const int B = (int)bound.size() - 1;
+    const int nseg = (int)brk.size() - 1;
+    L.cta_seg_first.assign(B, 0);
+    L.cta_slot_off.assign(B, 0);
+    L.seg_cta_lo.assign(std::max(nseg, 1), 0);
+    L.seg_cta_hi.assign(std::max(nseg, 1), -1);
+    std::vector<int> cta_seg_last(B, -1);
+    int64_t off = 0;
+    for (int b = 0; b < B; ++b) {
+        const int64_t s0 = bound[b], s1 = bound[b + 1];
+        L.cta_slot_off[b] = off;
+        if (s1 <= s0) continue;
+        const int g0 = seg_of(brk, s0), g1 = seg_of(brk, s1 - 1);
+        L.cta_seg_first[b] = g0;
+        cta_seg_last[b] = g1;
+        off += (int64_t)(g1 - g0 + 1) * nw * Q;
+    }
+    for (int g = 0; g < nseg; ++g) {
+        L.seg_cta_lo[g] = B;
+        L.seg_cta_hi[g] = -1;
+    }
+    for (int b = 0; b < B; ++b) {
+        if (cta_seg_last[b] < 0) continue;
+        for (int g = L.cta_seg_first[b]; g <= cta_seg_last[b]; ++g) {
+            L.seg_cta_lo[g] = std::min(L.seg_cta_lo[g], b);
+            L.seg_cta_hi[g] = std::max(L.seg_cta_hi[g], b);
+        }
+    }
+    return off;
 }
 
 // packed: plan and tables for the packed companion's rows (k1_site_pass_packed) instead of the one-hot rows
@@ -1832,34 +1942,9 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
     const K1Plan& pl = L.plan;
     const int B = pl.ctas;
     const int nseg = (int)ctx->brk.size() - 1;
-    L.cta_seg_first.assign(B, 0);
-    L.cta_slot_off.assign(B, 0);
-    L.seg_cta_lo.assign(std::max(nseg, 1), 0);
-    L.seg_cta_hi.assign(std::max(nseg, 1), -1);
-    std::vector<int> cta_seg_last(B, -1);
-    int64_t off = 0;
-    for (int b = 0; b < B; ++b) {
-        const int64_t t0 = (int64_t)b * pl.num_tiles / B, t1 = (int64_t)(b + 1) * pl.num_tiles / B;
-        const int64_t s0 = t0 * pl.T, s1 = std::min<int64_t>(t1 * pl.T, ctx->S);
-        L.cta_slot_off[b] = off;
-        if (s1 <= s0) continue;
-        const int g0 = seg_of(ctx->brk, s0), g1 = seg_of(ctx->brk, s1 - 1);
-        L.cta_seg_first[b] = g0;
-        cta_seg_last[b] = g1;
-        off += (int64_t)(g1 - g0 + 1) * nw * Q;
-    }
-    L.total_slots = off;
-    for (int g = 0; g < nseg; ++g) {
-        L.seg_cta_lo[g] = B;
-        L.seg_cta_hi[g] = -1;
-    }
-    for (int b = 0; b < B; ++b) {
-        if (cta_seg_last[b] < 0) continue;
-        for (int g = L.cta_seg_first[b]; g <= cta_seg_last[b]; ++g) {
-            L.seg_cta_lo[g] = std::min(L.seg_cta_lo[g], b);
-            L.seg_cta_hi[g] = std::max(L.seg_cta_hi[g], b);
-        }
-    }
+    std::vector<int64_t> bound(B + 1);
+    for (int b = 0; b <= B; ++b) bound[b] = std::min<int64_t>((int64_t)b * pl.num_tiles / B * pl.T, ctx->S);
+    L.total_slots = slot_tables(ctx->brk, bound, nw, Q, L);
     size_t bytes = 4096 + pt.ent_mask.size() * 4 + pt.ent_chunk.size() * 4 + pt.word_ent.size() * 4 + ctx->brk.size() * 8 +
                    (size_t)B * 12 + (size_t)std::max(nseg, 1) * 8 + (size_t)ctx->W * 24 + 17 * 16;
     PG_TRY(c.tables.ensure(bytes));
@@ -1920,8 +2005,8 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
 }
 
 // per-call part: zeroed slots
-int arm_slots(pg_ctx* ctx, K1Cache& c) {
-    const size_t bytes = (size_t)std::max<int64_t>(c.L.total_slots, 1) * 8;
+int arm_slots(pg_ctx* ctx, K1Cache& c, int64_t total_slots = -1) {
+    const size_t bytes = (size_t)std::max<int64_t>(total_slots >= 0 ? total_slots : c.L.total_slots, 1) * 8;
     PG_TRY(ctx->part.ensure(bytes));
     PG_CUDA(cudaMemsetAsync(ctx->part.p, 0, bytes, ctx->stream));
     c.L.prm.part = (unsigned long long*)ctx->part.p;
@@ -2020,62 +2105,150 @@ int launch_site_pass_packed(pg_ctx* ctx, const K1Launch& L, const char* name) {
 // run-to-run spread.
 constexpr double UNI_MIN_FRACTION = 0.125;
 
-// (Re)builds c.us for the current data and plan when they changed: one host synchronisation per rebuild, nothing on a
-// call over unchanged data.  PG_K1_UNIFORM_FORCE keeps the stream whatever the uniform fraction (tests on missing data).
+// Bytes of a stage of the stream's ring: R varied rows, the positions of Tmax sites from a 4-site boundary, Tmax codes, R slots.
+int uni_stage_bytes(int R, int Tmax, int pitch) {
+    return (int)align_up((size_t)R * pitch + (size_t)(Tmax + 4) * 4 + (size_t)Tmax * 2 + align_up((size_t)R * 2, 16), 128);
+}
+
+// The stream's geometry for the plan uplan: a tile bound of Tmax = 512 sites (PG_K1_UNI_TMAX, a multiple of 8 up to 32768), and a
+// budget of R varied rows per tile, one per lane of a team at the plan's lanes per site, halved (down to one warp's lanes)
+// while the ring would hold fewer than 2 stages (PG_K1_UNI_R sets R).  The ring: as many such stages as fit
+// (pg_k1_ring_stages).  tools/packed_site_pass.py --sweep (H100 80GB HBM3, 700 W): C2 (4 warps per team, 160-byte rows)
+// R = 32 / 64 / 128 / 256 0.50 / 0.30 / 0.22 / 0.23 ms; C5 (2 warps, 608-byte rows) R = 32 / 64 / 128 1.40 / 1.09 / 1.62 ms
+// (8, 5 and 2 stages): rows that fill the lanes matter more than stages beyond the teams' count.  Tmax = 256 / 512 / 2048:
+// C2 0.30 / 0.22 / 0.24 ms.
+void uni_geometry(K1Cache& c) {
+    const K1Plan& pl = c.uplan;
+    int Tmax = 512;
+    if (const char* e = getenv("PG_K1_UNI_TMAX")) Tmax = std::max(8, std::min(32768, (atoi(e) + 7) / 8 * 8));
+    const int lanes = 32 / std::max(1, pl.G);
+    int R = lanes * pl.wpt;
+    const char* er = getenv("PG_K1_UNI_R");
+    if (er && *er) {
+        R = std::max(1, std::min(0x7fff, atoi(er)));
+    } else {
+        while (R > lanes && pg_k1_ring_stages(uni_stage_bytes(R, Tmax, pl.pitch), c.utable) < 2) R /= 2;
+    }
+    c.uR = R;
+    c.uTmax = Tmax;
+    c.ubytes = uni_stage_bytes(R, Tmax, pl.pitch);
+    c.ustages = pl.stages >= 2 ? pg_k1_ring_stages(c.ubytes, c.utable) : 0;
+}
+
+// (Re)builds c.us for the current data and geometry when they changed: two host synchronisations per rebuild (the count of
+// varied rows, which sizes the buffers; the count of tiles with the CTAs' first sites, which size the launch and its slots),
+// nothing on a call over unchanged data.  PG_K1_UNIFORM_FORCE keeps the stream whatever the uniform fraction (tests on missing
+// data).
 int uniform_prepare(pg_ctx* ctx, K1Cache& c) {
     UniformStream& us = c.us;
     const bool forced = getenv("PG_K1_UNIFORM_FORCE") != nullptr;
-    const K1Plan& pl = c.uplan;
-    if (us.gen == ctx->data_gen && us.T == pl.T && us.forced == forced) return PG_OK;
+    const int R = c.uR, Tmax = c.uTmax;
+    if (us.gen == ctx->data_gen && us.R == R && us.Tmax == Tmax && us.forced == forced) return PG_OK;
     us.gen = ctx->data_gen;
-    us.T = pl.T;
+    us.R = R;
+    us.Tmax = Tmax;
     us.forced = forced;
     us.in_use = false;
     us.varied = ctx->S;
-    if (pl.stages < 2 || pl.T != c.L.plan.T || pl.num_tiles != c.L.plan.num_tiles) return PG_OK;
-    const int64_t nt = pl.num_tiles;
-    PG_TRY(us.cnt.ensure((size_t)(nt + 1) * 8));
-    PG_TRY(us.row0.ensure((size_t)(nt + 1) * 8));
+    us.serial += 1;
+    if (c.ustages < 2) return PG_OK;
+    const int64_t S = ctx->S;
+    constexpr int CH = 2048;                  // the chunks of the first pass (varied counts, then each varied row's site)
+    const int64_t nc = (S + CH - 1) / CH;
+    const int64_t nt_max = S / Tmax + 1 + (S + R - 1) / R + 1;   // groups + S / Tmax bound the pieces
+    const int64_t nscan = std::max(nc, nt_max) + 1;
+    PG_TRY(us.cnt.ensure((size_t)nscan * 8));
+    PG_TRY(us.row0.ensure((size_t)nscan * 8));
     int64_t* d_cnt = (int64_t*)us.cnt.p;
     int64_t* d_row0 = (int64_t*)us.row0.p;
     size_t scan_bytes = 0;
-    PG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_cnt, d_row0, nt + 1, ctx->stream));
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_cnt, d_row0, nscan, ctx->stream));
     PG_TRY(us.scan.ensure(scan_bytes));
     int ti = pg_time_begin(ctx, "k1_uniform");
-    PG_CUDA(cudaMemsetAsync(d_cnt + nt, 0, 8, ctx->stream));
-    k1_uni_count<<<(unsigned)nt, 256, 0, ctx->stream>>>(ctx->d_site_cls, ctx->S, pl.T, d_cnt);
+    PG_CUDA(cudaMemsetAsync(d_cnt + nc, 0, 8, ctx->stream));
+    k1_uni_count<<<(unsigned)nc, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, nullptr, CH, d_cnt);
     PG_CUDA(cudaGetLastError());
-    PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, scan_bytes, d_cnt, d_row0, nt + 1, ctx->stream));
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, scan_bytes, d_cnt, d_row0, nc + 1, ctx->stream));
     pg_time_end(ctx, ti);
     int64_t varied = 0;
-    PG_CUDA(cudaMemcpyAsync(&varied, d_row0 + nt, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    PG_CUDA(cudaMemcpyAsync(&varied, d_row0 + nc, 8, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
     us.varied = varied;
-    if (!forced && (double)(ctx->S - varied) < UNI_MIN_FRACTION * (double)ctx->S) return PG_OK;
-    us.code_pitch = (pl.T + 7) / 8 * 8;
+    if (!forced && (double)(S - varied) < UNI_MIN_FRACTION * (double)S) return PG_OK;
+    us.code_pitch = Tmax;
+    const int64_t ng = varied > 0 ? (varied + R - 1) / R : 1;
     const int chunks = ctx->packed_pitch / 16;
-    if (us.codes.ensure((size_t)nt * us.code_pitch * 4) != PG_OK ||
+    if (us.codes.ensure((size_t)nt_max * us.code_pitch * 4) != PG_OK ||
         us.src.ensure((size_t)std::max<int64_t>(varied, 1) * 8) != PG_OK ||
-        us.rows.ensure((size_t)std::max<int64_t>(varied, 1) * ctx->packed_pitch) != PG_OK) {
+        us.rows.ensure((size_t)std::max<int64_t>(varied, 1) * ctx->packed_pitch) != PG_OK ||
+        us.site_lo.ensure((size_t)(nt_max + 1) * 8) != PG_OK || us.groups.ensure((size_t)(ng + 1) * 8 * 2) != PG_OK ||
+        us.info.ensure((size_t)(ctx->sm_count + 2) * 8) != PG_OK) {
         cudaGetLastError();                   // no memory for the stream: the packed pass streams every row
         us.rows.release();
         us.src.release();
+        us.codes.release();
         return PG_OK;
     }
+    int64_t* d_src = (int64_t*)us.src.p;
+    int64_t* d_pieces = (int64_t*)us.groups.p;
+    int64_t* d_base = d_pieces + ng + 1;
+    int64_t* d_site_lo = (int64_t*)us.site_lo.p;
+    int64_t* d_info = (int64_t*)us.info.p;
     ti = pg_time_begin(ctx, "k1_uniform");
-    k1_uni_codes<<<(unsigned)nt, 256, 0, ctx->stream>>>(ctx->d_site_cls, ctx->S, pl.T, us.code_pitch, d_row0,
-                                                       (uint16_t*)us.codes.p, (int64_t*)us.src.p);
-    pg_time_end(ctx, ti);
+    // each varied row's site, then the groups of R rows, their pieces, the tiles' first sites and first rows, their codes
+    k1_uni_codes<<<(unsigned)nc, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, nullptr, CH, CH, d_row0, nullptr, d_src);
+    PG_CUDA(cudaGetLastError());
+    PG_CUDA(cudaMemsetAsync(d_pieces + ng, 0, 8, ctx->stream));
+    k1_uni_groups<<<(unsigned)((ng + 255) / 256), 256, 0, ctx->stream>>>(d_src, R, S, Tmax, ng, d_pieces);
+    PG_CUDA(cudaGetLastError());
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, scan_bytes, d_pieces, d_base, ng + 1, ctx->stream));
+    const int64_t nfill = std::max(ng, nt_max) + 1;
+    k1_uni_tiles<<<(unsigned)std::min<int64_t>((nfill + 255) / 256, (int64_t)ctx->sm_count * 16), 256, 0, ctx->stream>>>(
+        d_src, R, S, Tmax, ng, d_base, nt_max, d_site_lo);
+    PG_CUDA(cudaGetLastError());
+    PG_CUDA(cudaMemsetAsync(d_cnt + nt_max, 0, 8, ctx->stream));
+    k1_uni_count<<<(unsigned)nt_max, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, d_site_lo, Tmax, d_cnt);
+    PG_CUDA(cudaGetLastError());
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, scan_bytes, d_cnt, d_row0, nt_max + 1, ctx->stream));
+    k1_uni_codes<<<(unsigned)nt_max, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, d_site_lo, Tmax, us.code_pitch, d_row0,
+                                                           (uint16_t*)us.codes.p, d_src);
     PG_CUDA(cudaGetLastError());
     if (varied > 0) {
         const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((varied * chunks + 255) / 256, (int64_t)ctx->sm_count * 16));
-        ti = pg_time_begin(ctx, "k1_uniform");
-        k1_uni_gather<<<blocks, 256, 0, ctx->stream>>>((const uint4*)ctx->d_packed, (const int64_t*)us.src.p, varied, chunks,
-                                                       (uint4*)us.rows.p);
-        pg_time_end(ctx, ti);
+        k1_uni_gather<<<blocks, 256, 0, ctx->stream>>>((const uint4*)ctx->d_packed, d_src, varied, chunks, (uint4*)us.rows.p);
         PG_CUDA(cudaGetLastError());
     }
+    k1_uni_bounds<<<1, 256, 0, ctx->stream>>>(d_base, ng, d_site_lo, ctx->sm_count, d_info);
+    PG_CUDA(cudaGetLastError());
+    pg_time_end(ctx, ti);
+    std::vector<int64_t> info(ctx->sm_count + 2);
+    PG_CUDA(cudaMemcpyAsync(info.data(), d_info, info.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    us.nt = info[0];
+    const int B = (int)std::max<int64_t>(1, std::min<int64_t>(ctx->sm_count, us.nt));
+    us.bound.assign(info.begin() + 1, info.begin() + 2 + B);
     us.in_use = true;
+    return PG_OK;
+}
+
+// The slot tables of the stream's CTA ranges, rebuilt when the windows (epoch), the stream or the slot width changed.
+int uniform_slots(pg_ctx* ctx, K1Cache& c, int Q) {
+    if (c.uslots_epoch == ctx->epoch && c.uslots_serial == c.us.serial && c.uslots_Q == Q) return PG_OK;
+    K1Launch T;
+    c.utotal_slots = slot_tables(ctx->brk, c.us.bound, c.L.prm.nw, Q, T);
+    const size_t B = T.cta_seg_first.size(), ns = T.seg_cta_lo.size();
+    PG_TRY(c.uslots.ensure(B * 12 + ns * 8 + 4 * 16));
+    uint8_t* base = (uint8_t*)c.uslots.p;
+    size_t o = 0;
+    PG_TRY(push(ctx, base, o, T.cta_seg_first.data(), B, &c.u_cta_seg_first));
+    PG_TRY(push(ctx, base, o, T.cta_slot_off.data(), B, &c.u_cta_slot_off));
+    PG_TRY(push(ctx, base, o, T.seg_cta_lo.data(), ns, &c.u_seg_cta_lo));
+    PG_TRY(push(ctx, base, o, T.seg_cta_hi.data(), ns, &c.u_seg_cta_hi));
+    PG_CHECK(o <= c.uslots.cap, "internal: slot table buffer overflow");
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));     // the host vectors must outlive the copies
+    c.uslots_epoch = ctx->epoch;
+    c.uslots_serial = c.us.serial;
+    c.uslots_Q = Q;
     return PG_OK;
 }
 
@@ -2193,8 +2366,8 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
             c.lanepop = false;
             const int nw = k1_nw_for(ctx->packed_pitch);
             PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, 0, true));
-            c.uplan = pg_make_k1_plan_rows(ctx->S, ctx->packed_pitch, ctx->sm_count, table_bytes_of(c.pt) + UNI_SMEM_BYTES, nw, 0,
-                                           4);
+            c.utable = table_bytes_of(c.pt) + UNI_SMEM_BYTES;
+            c.uplan = pg_make_k1_plan_rows(ctx->S, ctx->packed_pitch, ctx->sm_count, c.utable, nw, 0, 4);
             if (!pg_k1_plan_ok(c.uplan)) c.uplan.stages = 0;    // no room for the codes: every row is streamed
         } else {
             // long rows, 4 or 8 real populations of <= 255 haplotypes: one lane per population (k1_site_pass_lp)
@@ -2231,16 +2404,33 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     // The packed pass streams only the varied rows when enough sites are uniform (uniform_prepare); PG_K1_NO_UNIFORM keeps
     // every row streamed, for the tests that compare the two.
     const bool uni = c.packed && ctx->d_site_cls && !getenv("PG_K1_NO_UNIFORM");
+    if (c.packed) uni_geometry(c);
     if (uni) PG_TRY(uniform_prepare(ctx, c));
     c.uni_last = uni && c.us.in_use;
-    PG_TRY(arm_slots(ctx, c));
+    if (c.uni_last) PG_TRY(uniform_slots(ctx, c, Q));
+    PG_TRY(arm_slots(ctx, c, c.uni_last ? c.utotal_slots : -1));
     if (c.uni_last) {
+        // Tiles of at most R varied rows and Tmax sites, a stage sized for such a tile: at 70 % uniform sites it is less than
+        // half a fixed tile's bytes, so the ring has more stages than teams and a team's next tile is in flight while it works
+        // on this one.  Its CTAs own the stream's tile ranges and add into the stream's slots.
         K1Launch UL = c.L;
         UL.plan = c.uplan;
-        UL.prm.stages = c.uplan.stages;
-        UL.prm.tile_bytes = c.uplan.tile_bytes;
+        UL.plan.T = c.uTmax;
+        UL.plan.num_tiles = c.us.nt;
+        UL.plan.ctas = (int)c.us.bound.size() - 1;
+        UL.plan.tile_bytes = c.ubytes;
+        UL.plan.stages = c.ustages;
+        UL.plan.smem_bytes = UL.plan.stages * UL.plan.tile_bytes + 256 + c.utable;
+        UL.prm.T = c.uTmax;
+        UL.prm.num_tiles = c.us.nt;
+        UL.prm.stages = UL.plan.stages;
+        UL.prm.tile_bytes = UL.plan.tile_bytes;
+        UL.prm.row_cap = c.uR;
+        UL.prm.cta_seg_first = c.u_cta_seg_first;
+        UL.prm.cta_slot_off = c.u_cta_slot_off;
         UL.prm.geno = (const uint8_t*)c.us.rows.p;
         UL.prm.row0 = (const int64_t*)c.us.row0.p;
+        UL.prm.site_lo = (const int64_t*)c.us.site_lo.p;
         UL.prm.codes = (const uint16_t*)c.us.codes.p;
         UL.prm.code_pitch = c.us.code_pitch;
         const char* gv = getenv("PG_K1_UNI_GV");           // test hook: lanes per varied row (1, 2, 4, ... 32)
@@ -2282,6 +2472,12 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     PG_CUDA(cudaMemsetAsync(d_cnt, 0, 4, ctx->stream));
     FinParams fp;
     fill_fin(fp, ctx, c, Q, Q);
+    if (c.uni_last) {
+        fp.cta_seg_first = c.u_cta_seg_first;
+        fp.cta_slot_off = c.u_cta_slot_off;
+        fp.seg_cta_lo = c.u_seg_cta_lo;
+        fp.seg_cta_hi = c.u_seg_cta_hi;
+    }
     fp.P = P;
     fp.Ppad = Pp;
     fp.min_sites = min_sites;
@@ -2319,8 +2515,35 @@ extern "C" int pg_debug_uniform_tile(pg_ctx* ctx, int32_t* out) {
     PG_CHECK(ctx && out, "pg_debug_uniform_tile: null argument");
     const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
     const bool planned = c && c->valid && c->packed;
-    out[0] = planned ? c->uplan.T : 0;
+    out[0] = planned ? c->uTmax : 0;
     out[1] = planned ? c->uplan.wpt : 0;
+    return PG_OK;
+}
+
+extern "C" int pg_debug_uniform_ring(pg_ctx* ctx, int32_t* out) {
+    PG_CHECK(ctx && out, "pg_debug_uniform_ring: null argument");
+    const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
+    const bool read = c && c->uni_last;
+    out[0] = read ? c->uR : 0;
+    out[1] = read ? c->ustages : 0;
+    out[2] = read ? c->ubytes : 0;
+    return PG_OK;
+}
+
+extern "C" int pg_debug_uniform_tiles(pg_ctx* ctx, int64_t cap, int64_t* site_lo, int64_t* row0, int64_t* ntiles,
+                                      int32_t* geometry) {
+    PG_CHECK(ctx && ntiles && geometry, "pg_debug_uniform_tiles: null argument");
+    const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
+    const bool read = c && c->uni_last;
+    *ntiles = read ? c->us.nt : 0;
+    geometry[0] = read ? c->uR : 0;
+    geometry[1] = read ? c->uTmax : 0;
+    if (!read || cap < c->us.nt + 1) return PG_OK;
+    PG_CHECK(site_lo && row0, "pg_debug_uniform_tiles: null table");
+    PG_CUDA(cudaSetDevice(ctx->device));
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    PG_CUDA(cudaMemcpy(site_lo, c->us.site_lo.p, (size_t)(c->us.nt + 1) * 8, cudaMemcpyDeviceToHost));
+    PG_CUDA(cudaMemcpy(row0, c->us.row0.p, (size_t)(c->us.nt + 1) * 8, cudaMemcpyDeviceToHost));
     return PG_OK;
 }
 

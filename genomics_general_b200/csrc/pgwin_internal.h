@@ -75,6 +75,7 @@ K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw =
 // rows of `pitch` bytes; code_bytes: bytes per site that a tile carries behind its positions (the uniform-site codes and
 // varied-row slots), an even number
 K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G, int code_bytes = 0);
+int pg_k1_ring_stages(int tile_bytes, int table_bytes);   // ring depth for stages of tile_bytes (< 2: does not fit)
 int pg_k1_plan_ok(const K1Plan& p);   // 1 if the site-pass kernels can run this plan
 int pg_pitch_for(int H);
 int pg_packed_pitch_for(int H);       // bytes per row of the packed companion

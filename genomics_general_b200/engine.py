@@ -569,6 +569,26 @@ class Engine:
         check(self._lib.pg_debug_uniform_tile(self._ctx, v), "pg_debug_uniform_tile")
         return int(v[0]), int(v[1])
 
+    def uniform_ring(self):
+        """(varied rows per tile at most, stages, bytes per stage) of the ring the last popgen call streamed the varied rows
+        through ((0, 0, 0) when it did not read the stream)."""
+        v = (C.c_int32 * 3)()
+        check(self._lib.pg_debug_uniform_ring(self._ctx, v), "pg_debug_uniform_ring")
+        return int(v[0]), int(v[1]), int(v[2])
+
+    def uniform_tiles(self):
+        """(R, Tmax, site_lo, row0) of the varied-row stream the last popgen call read: tile t covers the sites
+        [site_lo[t], site_lo[t + 1]) and the varied rows [row0[t], row0[t + 1]); None when it did not read the stream."""
+        nt, geo = C.c_int64(0), (C.c_int32 * 2)()
+        check(self._lib.pg_debug_uniform_tiles(self._ctx, 0, None, None, C.byref(nt), geo), "pg_debug_uniform_tiles")
+        if nt.value == 0:
+            return None
+        site_lo = np.empty(nt.value + 1, np.int64)
+        row0 = np.empty(nt.value + 1, np.int64)
+        check(self._lib.pg_debug_uniform_tiles(self._ctx, nt.value + 1, _ptr(site_lo), _ptr(row0), C.byref(nt), geo),
+              "pg_debug_uniform_tiles")
+        return int(geo[0]), int(geo[1]), site_lo, row0
+
 
 def k1_plan(S: int, H: int, nw: int = 8, lanes: int = 0, table_bytes: int = 4096):
     """Host-only: the site-pass launch geometry for a shape (works without a GPU).  `nw` consumer warps per CTA (8, or 12

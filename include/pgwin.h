@@ -300,9 +300,16 @@ int pg_debug_packed(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* row_words, u
  * rows of sites whose haplotypes are not all the same (0: every packed row), *varied_sites = the varied sites it counted
  * (S when it did not count them). */
 int pg_debug_uniform(pg_ctx* ctx, int32_t* in_use, int64_t* varied_sites);
-/* Tile geometry of the varied-row stream after a popgen call: out[0] = sites per tile, out[1] = warps per tile (0 before any
+/* Tile geometry of the varied-row stream after a popgen call: out[0] = sites per tile at most (Tmax), out[1] = warps per tile (0 before any
  * popgen call on the packed companion). */
 int pg_debug_uniform_tile(pg_ctx* ctx, int32_t* out);
+/* Ring of the varied-row stream's last popgen call: out[0] = varied rows a tile may hold (R), out[1] = stages, out[2] = bytes per
+ * stage (all 0 when the last call did not read the stream). */
+int pg_debug_uniform_ring(pg_ctx* ctx, int32_t* out);
+/* Tiles of the varied-row stream the last popgen call read: *ntiles, geometry[0] = R (varied rows per tile at most),
+ * geometry[1] = Tmax (sites per tile at most); when cap >= *ntiles + 1, site_lo / row0 get each tile's first site / first
+ * varied row and the totals (S, varied rows) at [ntiles].  All 0 when the last call did not read the stream. */
+int pg_debug_uniform_tiles(pg_ctx* ctx, int64_t cap, int64_t* site_lo, int64_t* row0, int64_t* ntiles, int32_t* geometry);
 
 #ifdef __cplusplus
 }

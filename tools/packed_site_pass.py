@@ -3,10 +3,11 @@ the packed companion (PG_K1_NO_UNIFORM), and on the packed rows of the varied si
 enough sites are uniform: a walk over the varied rows on all the team's lanes, then a pass over every slot without a walk),
 at the C2 shape (4 x 50 diploid samples, H = 400, 10 M sites) and the C5 shape (8 x 100 diploid samples, H = 1600, 12.5 M
 sites).  Per pass and shape: median / min / max of the k1_popgen kernel time (CUDA events) over the rounds, the bytes the
-pass reads per site, the achieved GB/s, the time of the varied-row build (k1_uniform, once per data change), and whether the
+pass reads per site, the achieved GB/s, the time of the varied-row build (k1_uniform, once per data change), the varied-row
+stream's geometry (row budget R, tile bound Tmax, ring stages and bytes, tiles, mean rows and sites per tile), and whether the
 records of the three passes are bit-identical.
 
---sweep adds, at C2: the elided pass under PG_K1_TILE_KB / PG_K1_STAGES settings, and the packed pass against the elided one
+--sweep adds, at C2 and C5: the elided pass under PG_K1_UNI_R / PG_K1_UNI_TMAX / PG_K1_STAGES settings; at C2: and the packed pass against the elided one
 (forced on) at small uniform fractions, the measurement behind the fraction from which the stream is kept.
 Prints one JSON line with the card's name and power limit.
 
@@ -114,6 +115,11 @@ def main():
                         build_ms.append(t["k1_uniform"]["ms"])
                         used, varied = eng.uniform_stream()
                         assert used
+                        R, stages, stage_bytes = eng.uniform_ring()
+                        _, Tmax, site_lo, row0 = eng.uniform_tiles()
+                        geometry = {"R": R, "Tmax": Tmax, "stages": stages, "stage_bytes": stage_bytes,
+                                    "tiles": len(site_lo) - 1, "rows_per_tile_mean": float(np.diff(row0).mean()),
+                                    "sites_per_tile_mean": float(np.diff(site_lo).mean())}
                     rec.setdefault(kind, records(r))
                     ms[kind].extend(timed(eng, args.calls))
             set_env({})
@@ -123,12 +129,28 @@ def main():
             # position + code per site; packed row + its slot per varied site
             res["varied_rows"] = stats(ms["varied_rows"], S, 6 + varied / S * (packed + 2))
             res["varied_rows"]["k1_uniform_build_ms_median"] = float(np.median(build_ms))
+            res["varied_rows"]["geometry"] = geometry
             res["speedup_varied_rows_vs_packed"] = (res["packed"]["k1_popgen_ms_median"] /
                                                     res["varied_rows"]["k1_popgen_ms_median"])
             res["records_bit_identical"] = all(np.array_equal(rec["byte"][k], rec[o][k])
                                                for k in rec["byte"] for o in ("packed", "varied_rows"))
             out["shapes"][name] = res
         if args.sweep:
+            for name, P, spp, S, w in (("C2", 4, 50, args.c2_sites, 50_000), ("C5", 8, 100, args.c5_sites, 5000)):
+                load(eng, P, spp, S, w)
+                geo = {}
+                for r, tm, st in ((0, 0, 0), (32, 0, 0), (64, 0, 0), (128, 0, 0), (256, 0, 0), (0, 256, 0), (0, 2048, 0),
+                                  (0, 0, 4)):
+                    env = {k: str(v) for k, v in (("PG_K1_UNI_R", r), ("PG_K1_UNI_TMAX", tm), ("PG_K1_STAGES", st)) if v}
+                    set_env(env)
+                    eng.popgen(1, 0.01)
+                    a = np.array(timed(eng, args.calls * 2))
+                    geo[" ".join("%s=%s" % kv for kv in env.items()) or "default"] = {
+                        "ms_median": float(np.median(a)), "ring": eng.uniform_ring()}
+                    for k in ("PG_K1_UNI_R", "PG_K1_UNI_TMAX"):
+                        os.environ.pop(k, None)
+                set_env({})
+                out[name.lower() + "_budget_sweep"] = geo
             S = args.c2_sites
             H = load(eng, 4, 50, S, 50_000)
             geo = {}
