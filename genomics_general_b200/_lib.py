@@ -108,6 +108,11 @@ _SIGS = {
                                  C.POINTER(C.c_int64)]),
     "pg_ingest_meta": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_ingest_release": (C.c_int, [C.c_void_p]),
+    "pg_ingest_set_strict": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pg_filter": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_uint8)]),
+    "pg_filter_emit": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64),
+                                 C.POINTER(C.c_size_t)]),
+    "pg_filter_stats": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_void_p] * 8),
     "pg_format_freq_rows": (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_size_t, C.c_int32, C.c_void_p]),
     "pg_format_matrix_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t,
@@ -122,6 +127,17 @@ _SIGS = {
 }
 
 EXPORTS = tuple(_SIGS)
+
+
+class FilterSpec(C.Structure):
+    """pg_filter_spec (include/pgwin.h)"""
+    _fields_ = [("n_samp", C.c_int32), ("samp_hap0", C.c_void_p), ("samp_ploidy", C.c_void_p), ("P", C.c_int32),
+                ("pop_off", C.c_void_p), ("pop_members", C.c_void_p), ("min_calls", C.c_int32), ("min_alleles", C.c_int32), ("max_alleles", C.c_double),
+                ("min_var_count", C.c_int32), ("has_max_het", C.c_int32), ("max_het", C.c_double),
+                ("min_freq", C.c_double), ("max_freq", C.c_double), ("min_pop_calls", C.c_void_p),
+                ("min_pop_alleles", C.c_void_p), ("max_pop_alleles", C.c_void_p), ("fixed_diffs", C.c_int32),
+                ("has_nearly_fixed", C.c_int32), ("nearly_fixed_diff", C.c_double), ("partial_to_missing", C.c_int32),
+                ("no_test", C.c_int32), ("thin_dist", C.c_int32), ("pod_size", C.c_int32)]
 
 
 def lib():

@@ -71,6 +71,7 @@ extern "C" int pg_ctx_destroy(pg_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     pg_k1_cache_free(ctx);
+    pg_filter_free(ctx);
     pg_nccl_finalize(ctx);
     ctx->gather.release();
     ctx->gather_flag.release();
@@ -81,7 +82,8 @@ extern "C" int pg_ctx_destroy(pg_ctx* ctx) {
     PgBuf* bufs[] = {&ctx->tables, &ctx->part, &ctx->segmeta, &ctx->winmeta, &ctx->out_d, &ctx->out_i,
                      &ctx->planes, &ctx->planes2, &ctx->pairs, &ctx->misc, &ctx->misc2, &ctx->misc3, &ctx->misc4, &ctx->misc5, &ctx->text, &ctx->starts, &ctx->meta,
                      &ctx->sfs_acc_k[0], &ctx->sfs_acc_k[1], &ctx->sfs_acc_r[0], &ctx->sfs_acc_r[1], &ctx->sfs_slab,
-                     &ctx->sfs_merge, &ctx->sfs_cub};
+                     &ctx->sfs_merge, &ctx->sfs_cub, &ctx->flt_aux, &ctx->flt_tab,
+                     &ctx->flt_stats, &ctx->flt_rows, &ctx->flt_off, &ctx->flt_out, &ctx->flt_cub};
     for (PgBuf* b : bufs) b->release();
     for (cudaEvent_t ev : ctx->event_pool) cudaEventDestroy(ev);
     ctx->stage[0].release();

@@ -106,10 +106,21 @@ struct ParseParams {
     int pitch;
     int32_t* pos;
     unsigned long long* scaf_hash;
-    unsigned long long* err;    // [0] = code (0 ok), [1] = data line (1-based), [2] = genotype column (1-based)
+    unsigned long long* err;    // all ones = ok, else (data line << 28) | (genotype column << 4) | code, 1-based
+    // strict tokens (pg_ingest_set_strict): a token must be exactly as wide as the sample's ploidy and hold only A C G T N
+    // (phased / pairs) or a letter of genomics.py:14 DIPLOTYPES (diplo, diploid samples only); the phase character of each
+    // sample (token[1] of a phased token of ploidy >= 2, else '/', genomics.py:335) goes to aux[line * H + first_hap]
+    int strict;
+    uint8_t* aux;
+    int aux_stride;
 };
 
-enum { ERR_NONE = 0, ERR_POS = 1, ERR_PLOIDY = 2, ERR_MISSING_COLS = 3, ERR_NO_POS = 4 };
+enum { ERR_NONE = 0, ERR_POS = 1, ERR_PLOIDY = 2, ERR_MISSING_COLS = 3, ERR_NO_POS = 4, ERR_CHAR = 5 };
+
+__device__ __forceinline__ bool acgtn(unsigned c) { return c == 'A' || c == 'C' || c == 'G' || c == 'T' || c == 'N'; }
+__device__ __forceinline__ bool diplotype(unsigned c) {
+    return acgtn(c) || c == 'K' || c == 'M' || c == 'S' || c == 'R' || c == 'W' || c == 'Y';
+}
 
 __device__ __forceinline__ unsigned onehot(unsigned c) {
     return c == 'A' ? 0x01u : (c == 'C' ? 0x04u : (c == 'G' ? 0x10u : (c == 'T' ? 0x40u : 0u)));
@@ -133,10 +144,9 @@ __device__ __forceinline__ void diplo_alleles(unsigned c, unsigned& a0, unsigned
 }
 
 __device__ __forceinline__ void report(const ParseParams& pp, int code, int64_t line, int col) {
-    if (atomicCAS(pp.err, 0ull, (unsigned long long)code) == 0ull) {
-        pp.err[1] = (unsigned long long)(line + 1);
-        pp.err[2] = (unsigned long long)(col + 1);
-    }
+    // the first offending line wins (then the lowest column): line, column and code packed into one word for atomicMin
+    const unsigned long long c1 = (unsigned long long)min(max(col + 1, 0), (1 << 24) - 1);
+    atomicMin(pp.err, ((unsigned long long)(line + 1) << 28) | (c1 << 4) | (unsigned long long)code);
 }
 
 // byte at absolute offset i of the text ('\n' past the end, so that every field terminates)
@@ -238,6 +248,23 @@ __global__ void __launch_bounds__(256) k_parse_lines(const __grid_constant__ Par
                         const unsigned c = byte_at(pp, q + tl);
                         if (c == '\n' || is_ws_dev(c)) break;
                         ++tl;
+                    }
+                    if (pp.strict) {
+                        const int want = pp.fmt == 0 ? 2 * pl - 1 : (pp.fmt == 1 ? 1 : pl);
+                        if (tl != want || (pp.fmt == 1 && pl != 2)) {
+                            report(pp, ERR_PLOIDY, line, col);
+                            continue;
+                        }
+                        bool ok = true;
+                        if (pp.fmt == 1) ok = diplotype(byte_at(pp, q));
+                        else
+                            for (int a = 0; a < pl; ++a) ok = ok && acgtn(byte_at(pp, q + (pp.fmt == 0 ? 2 * a : a)));
+                        if (!ok) {
+                            report(pp, ERR_CHAR, line, col);
+                            continue;
+                        }
+                        pp.aux[(size_t)line * pp.aux_stride + hap0] =
+                            (uint8_t)(pp.fmt == 0 && pl >= 2 ? byte_at(pp, q + 1) : (unsigned)'/');
                     }
                     if (pp.fmt == 0) {                                  // phased: characters 0,2,4,...
                         if ((tl + 1) / 2 != pl) {
@@ -489,7 +516,7 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
     int8_t* d_flags = (int8_t*)(d_hash + S);
     PG_TRY(ctx->out_i.ensure(64));
     unsigned long long* d_err = (unsigned long long*)ctx->out_i.p;
-    PG_CUDA(cudaMemsetAsync(d_err, 0, 24, ctx->stream));
+    PG_CUDA(cudaMemsetAsync(d_err, 0xff, 8, ctx->stream));       // no error: all ones
     ParseParams pp;
     pp.buf = d_text;
     pp.len = len;
@@ -505,6 +532,14 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
     pp.pos = ctx->d_pos;
     pp.scaf_hash = d_hash;
     pp.err = d_err;
+    pp.strict = ctx->ingest_strict;
+    pp.aux = nullptr;
+    pp.aux_stride = H_out;
+    if (pp.strict) {
+        PG_TRY(ctx->flt_aux.ensure((size_t)S * H_out + 64));
+        pp.aux = (uint8_t*)ctx->flt_aux.p;
+    }
+    ctx->ingest_fmt = fmt;
     {
         const int ti = pg_time_begin(ctx, "ingest_parse");
         const unsigned grid = (unsigned)std::min<int64_t>((S + 7) / 8, (int64_t)ctx->sm_count * 64);
@@ -516,10 +551,12 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
         ctx->launches += 1;
     }
     PG_TRY(pg_pack_rows(ctx, 0, S));
-    unsigned long long h_err[3] = {0, 0, 0};
-    PG_CUDA(cudaMemcpyAsync(h_err, d_err, 24, cudaMemcpyDeviceToHost, ctx->stream));
+    unsigned long long packed = ~0ull;
+    PG_CUDA(cudaMemcpyAsync(&packed, d_err, 8, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
     ctx->ingest_sites = S;
+    // [0] = code, [1] = data line (1-based), [2] = genotype column (1-based)
+    const unsigned long long h_err[3] = {packed == ~0ull ? 0ull : (packed & 15ull), packed >> 28, (packed >> 4) & 0xffffffull};
     switch ((int)h_err[0]) {
         case ERR_NONE: break;
         case ERR_POS:
@@ -529,6 +566,10 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
         case ERR_PLOIDY:
             pg_set_error("pg_ingest_text: data line %llu, genotype column %llu: the token's allele count does not match the "
                          "sample's ploidy (genomics.py:1111 asserts the same)", h_err[1], h_err[2]);
+            return PG_ERR;
+        case ERR_CHAR:
+            pg_set_error("pg_ingest_text: data line %llu, genotype column %llu: a character other than A, C, G, T or N (the "
+                         "reference makes such a genotype missing but writes it out unchanged)", h_err[1], h_err[2]);
             return PG_ERR;
         default:
             pg_set_error("pg_ingest_text: data line %llu: %llu genotype columns, not every requested sample found", h_err[1],
@@ -554,6 +595,13 @@ extern "C" int pg_ingest_meta(pg_ctx* ctx, int32_t* pos, int8_t* new_scaffold, i
                                 cudaMemcpyDeviceToHost, ctx->stream));
     if (line_off) PG_CUDA(cudaMemcpyAsync(line_off, ctx->starts.p, (size_t)S * 8, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    return PG_OK;
+}
+
+// Strict tokens for the next ingests of this ctx (off by default): see ParseParams::strict.
+extern "C" int pg_ingest_set_strict(pg_ctx* ctx, int32_t on) {
+    PG_CHECK(ctx != nullptr, "pg_ingest_set_strict: null ctx");
+    ctx->ingest_strict = on ? 1 : 0;
     return PG_OK;
 }
 

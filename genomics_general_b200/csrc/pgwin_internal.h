@@ -122,6 +122,12 @@ struct pg_ctx {
     PgBuf tables, part, segmeta, winmeta, out_d, out_i, planes, planes2, pairs, misc, misc2, misc3, misc4, misc5;
     PgBuf text, starts, meta;                 // device-side text ingest (ingest.cu)
     int64_t ingest_sites = -1;
+    int32_t ingest_fmt = 0;                   // format of the last text ingest
+    int32_t ingest_strict = 0;                // pg_ingest_set_strict
+    // filterGenotypes (filter.cu): phase character per sample of the strict ingest, sample tables, per-site statistics,
+    // kept rows, their byte offsets and the output slab
+    PgBuf flt_aux, flt_tab, flt_stats, flt_rows, flt_off, flt_out, flt_cub;
+    void* flt_state = nullptr;                // host-side state of the last pg_filter (owned by filter.cu)
     void* h_text[2] = {nullptr, nullptr};     // pinned staging of the text
     cudaEvent_t h_text_free[2] = {nullptr, nullptr};
     // upload pipeline: copy stream + two staging buffers
@@ -202,6 +208,7 @@ int pg_k2t_het(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const int6
 int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, const int64_t* win_lo, const int64_t* win_hi,
                          int32_t min_sites, double min_data, void* d_rec, int RC);
 void pg_k1_cache_free(pg_ctx* ctx);
+void pg_filter_free(pg_ctx* ctx);        // filter.cu
 int pg_nccl_allreduce_i64(pg_ctx* ctx, void* d_buf, size_t count);   // nccl_gather.cu
 int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t force_path, void* d_rec, int** h_count);
 int pg_popgen_resolve(pg_ctx* ctx, int32_t min_sites, double min_data, void* d_rec, int nk2);

@@ -349,14 +349,94 @@ class Engine:
         check(self._lib.pg_append_sites(self._ctx, geno.shape[0], _ptr(geno), _ptr(pos)), "pg_append_sites")
         self.S += geno.shape[0]
 
-    def ingest_meta(self, S: int):
-        """(pos int32 [S], new_scaffold int8 [S], line_off int64 [S]) of the last ingest_text."""
+    def ingest_meta(self, S: int, release: bool = True):
+        """(pos int32 [S], new_scaffold int8 [S], line_off int64 [S]) of the last ingest_text.  The device copy of the text
+        is freed unless release=False (filter_emit reads it)."""
         pos = np.empty(S, dtype=np.int32)
         newsc = np.empty(S, dtype=np.int8)
         off = np.empty(S, dtype=np.int64)
         check(self._lib.pg_ingest_meta(self._ctx, _ptr(pos), _ptr(newsc), _ptr(off)), "pg_ingest_meta")
-        check(self._lib.pg_ingest_release(self._ctx), "pg_ingest_release")
+        if release:
+            check(self._lib.pg_ingest_release(self._ctx), "pg_ingest_release")
         return pos, newsc, off
+
+    # ---- filterGenotypes.py ----
+    FILTER_FORMATS = {"phased": 0, "diplo": 1, "bases": 2, "alleles": 3, "coded": 4, "count": 5}
+
+    def set_strict_ingest(self, on: bool = True):
+        """Strict genotype tokens for the next ingests (pg_ingest_set_strict)."""
+        check(self._lib.pg_ingest_set_strict(self._ctx, 1 if on else 0), "pg_ingest_set_strict")
+
+    def filter(self, spec: dict, contig_mask=None, scaf_id=None):
+        """pg_filter over the sites of the last strict ingest.  spec keys: samp_hap0, samp_ploidy, pops (one list of sample
+        indices per population, in -p order; may overlap) and the scalar / per-population settings of pg_filter_spec
+        (None = off).  Returns (rows kept, OR of their flags)."""
+        from ._lib import FilterSpec
+        keep = []
+
+        def arr(v, dt):
+            if v is None:
+                return None
+            a = np.ascontiguousarray(v, dtype=dt)
+            keep.append(a)
+            return a.ctypes.data
+        fs = FilterSpec()
+        fs.n_samp = len(spec["samp_hap0"])
+        fs.samp_hap0 = arr(spec["samp_hap0"], np.int32)
+        fs.samp_ploidy = arr(spec["samp_ploidy"], np.int8)
+        pops = [list(m) for m in (spec.get("pops") or [])]
+        fs.P = len(pops)
+        if fs.P:
+            fs.pop_off = arr(np.concatenate([[0], np.cumsum([len(m) for m in pops])]), np.int32)
+            fs.pop_members = arr(np.array([k for m in pops for k in m] or [0]), np.int32)
+        fs.min_calls = int(spec.get("min_calls", 1))
+        fs.min_alleles = int(spec.get("min_alleles", 1))
+        fs.max_alleles = float(spec.get("max_alleles", float("inf")))
+        fs.min_var_count = int(spec.get("min_var_count") or 0)
+        fs.has_max_het = spec.get("max_het") is not None
+        fs.max_het = float(spec.get("max_het") or 0.0)
+        fs.min_freq = float(spec.get("min_freq") or 0.0)
+        fs.max_freq = float(spec.get("max_freq") or 0.0)
+        fs.min_pop_calls = arr(spec.get("min_pop_calls"), np.int32)
+        fs.min_pop_alleles = arr(spec.get("min_pop_alleles"), np.int32)
+        fs.max_pop_alleles = arr(spec.get("max_pop_alleles"), np.int32)
+        fs.fixed_diffs = 1 if spec.get("fixed_diffs") else 0
+        fs.has_nearly_fixed = spec.get("nearly_fixed_diff") is not None
+        fs.nearly_fixed_diff = float(spec.get("nearly_fixed_diff") or 0.0)
+        fs.partial_to_missing = 1 if spec.get("partial_to_missing") else 0
+        fs.no_test = 1 if spec.get("no_test") else 0
+        fs.thin_dist = int(spec.get("thin_dist") or 0)
+        fs.pod_size = int(spec.get("pod_size") or 10000)
+        cm = arr(contig_mask, np.uint8)
+        sc = arr(scaf_id, np.int32)
+        nk = C.c_int64(0)
+        fo = C.c_uint8(0)
+        check(self._lib.pg_filter(self._ctx, C.byref(fs), cm, sc, C.byref(nk), C.byref(fo)), "pg_filter")
+        self._filter_P = fs.P
+        return int(nk.value), int(fo.value)
+
+    def filter_emit(self, fmt: str, freq_order: bool, row0: int, buf, cap: int):
+        """Rows row0.. of the last filter as text into buf (a writable buffer of at least cap bytes, pinned for speed):
+        (rows, bytes) written."""
+        rows = C.c_int64(0)
+        nb = C.c_size_t(0)
+        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
+        check(self._lib.pg_filter_emit(self._ctx, self.FILTER_FORMATS[fmt], 1 if freq_order else 0, int(row0), C.c_void_p(addr),
+                                       int(cap), C.byref(rows), C.byref(nb)), "pg_filter_emit")
+        return int(rows.value), int(nb.value)
+
+    def filter_stats(self, site0: int = 0, n: int | None = None):
+        """Per-site statistics of the last filter (pg_filter_stats) as a dict of arrays."""
+        if n is None:
+            n = self.S - site0
+        P = getattr(self, "_filter_P", 0)
+        r = dict(called=np.empty(n, np.int32), het=np.empty(n, np.int32), counts=np.empty((n, 4), np.int32),
+                 pop_called=np.empty((n, P), np.int32), pop_mask=np.empty((n, P), np.uint8), flags=np.empty(n, np.uint8),
+                 keep=np.empty(n, np.uint8), final=np.empty(n, np.uint8))
+        check(self._lib.pg_filter_stats(self._ctx, int(site0), int(n), *[_ptr(r[k]) for k in
+                                        ("called", "het", "counts", "pop_called", "pop_mask", "flags", "keep", "final")]),
+              "pg_filter_stats")
+        return r
 
     def site_counts(self, site0: int = 0, n: int = None, out=None):
         """uint16 [n, P, 4] A,C,G,T counts per population (`out`: a caller-owned array to fill, e.g. one whose pages are

@@ -278,6 +278,65 @@ int pg_ingest_meta(pg_ctx* ctx, int32_t* pos, int8_t* new_scaffold, int64_t* lin
 /* Frees the device copy of the text. */
 int pg_ingest_release(pg_ctx* ctx);
 
+/* Strict genotype tokens for the next ingests of this ctx (off by default; filterGenotypes turns it on): a token must be
+ * exactly as wide as its sample's ploidy (2p-1 characters phased, p alleles, one letter diplo with diploid samples only), and
+ * hold only A C G T N (a diplo letter of genomics.py:14 DIPLOTYPES).  The reference makes a genotype with any other character
+ * missing but writes the character back out (genomics.py:351-352), which the one-hot matrix cannot do; such a line is an
+ * error naming its data line.  The ingest also keeps each sample's phase character (genomics.py:335) for pg_filter_emit. */
+int pg_ingest_set_strict(pg_ctx* ctx, int32_t on);
+
+/* ---- filterGenotypes.py ------------------------------------------------------------------------ */
+/* Filter settings (filterGenotypes.py:161-183 -> genomics.siteTest, genomics.py:742-799).  Samples are the selected
+ * samples in output order; populations are indices in -p order.  Pointers are host memory. */
+typedef struct pg_filter_spec {
+    int32_t n_samp;
+    const int32_t* samp_hap0;       /* [n_samp] first haplotype of the sample in the resident matrix */
+    const int8_t* samp_ploidy;      /* [n_samp] */
+    int32_t P;                      /* populations (<= 64), in -p order */
+    const int32_t* pop_off;         /* [P + 1] population p's members are pop_members[pop_off[p] .. pop_off[p + 1]) */
+    const int32_t* pop_members;     /* sample indices; a sample may be in several populations (siteTest visits each list
+                                       on its own, genomics.py:774-796).  A population with no member stands for every
+                                       sample, as GenomeSite.alleles / baseFreqs do for an empty list (genomics.py:521-523,
+                                       544-545), except for its called count, which is 0.  NULL both when P == 0 */
+    int32_t min_calls;              /* called samples (no missing allele) at least */
+    int32_t min_alleles;
+    double max_alleles;
+    int32_t min_var_count;          /* 0 = off; second largest base count, variable sites only */
+    int32_t has_max_het;
+    double max_het;                 /* het samples / called samples (numpy division: 0/0 nan passes, k/0 inf fails) */
+    double min_freq, max_freq;      /* 0 = off; second largest of count / n */
+    const int32_t* min_pop_calls;   /* [P] or NULL */
+    const int32_t* min_pop_alleles; /* [P] or NULL; min and max are both given or both NULL */
+    const int32_t* max_pop_alleles;
+    int32_t fixed_diffs;
+    int32_t has_nearly_fixed;
+    double nearly_fixed_diff;
+    int32_t partial_to_missing;     /* a sample with any missing allele becomes all missing */
+    int32_t no_test;                /* keep every site that survives the contig and thinning steps */
+    int32_t thin_dist;              /* 0 = off */
+    int32_t pod_size;               /* input lines per pod: thinning restarts at every pod; site 0 starts a pod */
+} pg_filter_spec;
+
+/* Replaces the per-line loop of filterGenotypes.py's analysisWrapper (filterGenotypes.py:33-55: the contig lists, the
+ * thinning and genomics.siteTest) over the resident sites of the last text ingest.  contig_mask uint8 [S] (NULL = all 1):
+ * 0 drops the line before anything else; scaf_id int32 [S]: equal ids = same scaffold (required with thin_dist).
+ * *n_kept = rows to write; *flags_or (may be NULL) = OR of the flags (see pg_filter_stats) of the kept sites. */
+int pg_filter(pg_ctx* ctx, const pg_filter_spec* spec, const uint8_t* contig_mask, const int32_t* scaf_id, int64_t* n_kept,
+              uint8_t* flags_or);
+/* Replaces the row assembly of filterGenotypes.py:53 (GenomeSite.asList, genomics.py:465-512) for the kept rows of the last
+ * pg_filter: rows row0, row0 + 1, ... as many as fit in cap bytes of out (host memory).  fmt: 0 phased, 1 diplo, 2 bases,
+ * 3 alleles, 4 coded, 5 count; freq_order = --alleleOrder freq.  Each row starts with the scaffold and position fields as
+ * they are in the text.  *rows / *bytes = what was written; a single row larger than cap is an error. */
+int pg_filter_emit(pg_ctx* ctx, int32_t fmt, int32_t freq_order, int64_t row0, char* out, size_t cap, int64_t* rows,
+                   size_t* bytes);
+/* Per-site statistics of the last pg_filter for sites [site0, site0 + n) (any pointer may be NULL): called, het int32 [n],
+ * counts int32 [n x 4] (A C G T over the selected samples), pop_called int32 [n x P], pop_mask uint8 [n x P] (alleles of the
+ * population, bit a = base a), flags uint8 [n] (1: two present alleles have the same count, so the frequency order is a tie
+ * that numpy's sort may break either way; 2: a sample is partly missing; 4: no allele), keep uint8 [n] (the siteTest
+ * verdict), final uint8 [n] (the row is written). */
+int pg_filter_stats(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* called, int32_t* het, int32_t* counts,
+                    int32_t* pop_called, uint8_t* pop_mask, uint8_t* flags, uint8_t* keep, uint8_t* final_);
+
 /* ---- introspection ---------------------------------------------------------------------------- */
 /* Device time (ms, CUDA events on the ctx stream) of the kernels launched by the last statistics call:
  * names[i] -> ms[i]; returns the number of entries through *count (at most cap). */
