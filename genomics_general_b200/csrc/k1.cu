@@ -1674,19 +1674,50 @@ int check_plan(const K1Plan& pl) {
     return PG_OK;
 }
 
-// Long rows of 4 or 8 populations prefer the lane-per-population kernel (G = P lanes per site), but its plan stops
-// fitting earlier than the general one (T = 8 sites at G = 4): take it only where it runs.
-bool lanepop_fits(int64_t S, int H, int sm_count, int table_bytes, int nw, int P) {
-    const K1Plan p = pg_make_k1_plan(S, H, sm_count, table_bytes, nw, P);
-    return pg_k1_plan_ok(p) != 0;
+// consumer warps per CTA.  The general kernels: 12 (+ the producer = 416 threads, 128 registers each) for rows below 1 KiB; 8
+// (up to 168 registers, no spills) for longer rows, where the 8-population instantiations need the registers
+// (tools/k1_sweep2.py compares the two).  The lane-per-population kernel: 12.  PG_K1_NW = 8 or 12 overrides either.
+int k1_nw_for(int pitch, bool lanepop) {
+    const char* e = getenv("PG_K1_NW");
+    const int v = (e && *e) ? atoi(e) : ((lanepop || pitch < 1024) ? 12 : 8);
+    return lanepop ? (v == 8 ? 8 : 12) : (v == 12 ? 12 : 8);
 }
+
+// Whether every population's counts fit a byte, so that the popgen byte pass packs them four to a word (PG_K1_NO_BYTES: never).
+bool byte_counts(int maxN) { return maxN <= 255 && !getenv("PG_K1_NO_BYTES"); }
+
+// Whether a byte-pass launch over S sites runs the lane-per-population kernel (k1_site_pass_lp, G = Pp lanes per site), and
+// with how many consumer warps.  Long rows of a full group of 4 or 8 populations prefer it, but its plan stops fitting
+// earlier than the general one (T = 8 sites at G = 4), so it is taken only where it runs.  The two callers differ in
+// narrow_counts alone: the popgen instantiations keep byte-packed counts, so popgen passes byte_counts() of its largest
+// population; the per-site counts fit their 16 bits in any case, so the counts launch passes true.  PG_K1_LANEPOP decides for
+// any row length and group wherever the kernel exists (tests).
+struct WarpChoice {
+    bool lanepop;
+    int nw;
+};
+WarpChoice choose_warps(const pg_ctx* ctx, int64_t S, int Pp, bool full_group, int table_bytes, bool narrow_counts) {
+    bool lp = (Pp == 4 || Pp == 8) && narrow_counts;
+    if (const char* e = getenv("PG_K1_LANEPOP")) lp = lp && atoi(e) != 0;
+    else
+        lp = lp && full_group && ctx->pitch >= 1024 &&
+             pg_k1_plan_ok(pg_make_k1_plan(S, ctx->H, ctx->sm_count, table_bytes, k1_nw_for(ctx->pitch, true), Pp));
+    return {lp, k1_nw_for(ctx->pitch, lp)};
+}
+
+// Where a launch's CTAs keep their sums, as device tables: CTA b's slots start at word cta_slot_off[b] with the segment
+// cta_seg_first[b], and segment g is touched by the CTAs seg_cta_lo[g] .. seg_cta_hi[g].  The site pass reads the first two
+// and k1_finalize all four, so both take them from the launch that runs (arm_slots, fill_fin).
+struct SlotTables {
+    int32_t *cta_seg_first = nullptr, *seg_cta_lo = nullptr, *seg_cta_hi = nullptr;
+    int64_t* cta_slot_off = nullptr;
+    int64_t words = 0;   // 8-byte words of all slots
+};
 
 struct K1Launch {
     K1Plan plan;
     K1Params prm;
-    std::vector<int32_t> cta_seg_first, seg_cta_lo, seg_cta_hi;
-    std::vector<int64_t> cta_slot_off;
-    int64_t total_slots = 0;   // 8-byte words
+    SlotTables slots;
 };
 
 int seg_of(const std::vector<int64_t>& brk, int64_t site) {
@@ -1694,18 +1725,14 @@ int seg_of(const std::vector<int64_t>& brk, int64_t site) {
     return (int)(std::upper_bound(brk.begin(), brk.end(), site) - brk.begin()) - 1;
 }
 
-// device layout of the uploaded tables inside ctx->tables:
-//   [ent_mask (16B each)] [ent_chunk] [word_ent (8B each)] [brk] [cta_seg_first] [cta_slot_off] [seg_cta_lo] [seg_cta_hi]
-//   [win_seg_lo] [win_seg_hi] [win_lo] [win_hi]
+// device layout of the uploaded tables inside K1Cache::tables:
+//   [ent_mask (16B each)] [ent_chunk] [word_ent (8B each)] [brk] [the launch's SlotTables] [win_seg_lo] [win_seg_hi] [win_lo]
+//   [win_hi]
 struct DevTables {
     uint4* ent_mask;
     int32_t* ent_chunk;
     uint2* word_ent;
     int64_t* brk;
-    int32_t* cta_seg_first;
-    int64_t* cta_slot_off;
-    int32_t* seg_cta_lo;
-    int32_t* seg_cta_hi;
     int32_t* win_seg_lo;
     int32_t* win_seg_hi;
     int64_t* win_lo;
@@ -1845,6 +1872,26 @@ __global__ void __launch_bounds__(256) k1_uni_gather(const uint4* __restrict__ p
     }
 }
 
+// The packed popgen pass over the varied rows only: the stream, its geometry, the slot tables of its CTA ranges and the
+// launch of k1_site_pass_packed<..., true> made of them.  uni_geometry sets the geometry on every call (its hooks);
+// uniform_prepare rebuilds the stream when the data or the geometry changed; uniform_slots rebuilds the slot tables and the
+// launch when the windows (epoch), the stream (serial), the slot width or the ring changed.
+struct UniformPass {
+    K1Plan plan;              // the cache's plan with room for the codes in each stage (its G, wpt and warps serve the stream)
+    int table_bytes = 0;      // shared-memory bytes of plan's tables
+    int R = 0, Tmax = 0, stages = 0, stage_bytes = 0;   // row budget, tile bound, and ring (uni_geometry)
+    UniformStream us;
+    PgBuf slot_buf;
+    uint64_t slots_epoch = 0, slots_serial = 0;
+    int slots_Q = 0;
+    K1Launch L;
+    bool last = false;        // the last popgen launch was L
+    void release() {
+        us.release();
+        slot_buf.release();
+    }
+};
+
 // Everything a windowed launch needs, cached per configuration (data shape, populations, windows): a repeated
 // statistics call on the same configuration only clears the slots and launches two kernels.
 struct K1Cache {
@@ -1858,18 +1905,7 @@ struct K1Cache {
     DevTables dt;
     PopTables pt;
     PgBuf tables;
-    K1Plan uplan;             // packed: L.plan with room for the codes in each stage (its G, wpt and warps serve the stream)
-    int utable = 0;           // packed: shared-memory bytes of uplan's tables
-    UniformStream us;         // packed: the varied rows (popgen cache only)
-    int uR = 0, uTmax = 0, ustages = 0, ubytes = 0;   // the stream's row budget, tile bound, and ring (uni_geometry)
-    bool uni_last = false;    // the last popgen launch read us
-    // the slot tables of the stream's CTA ranges (slot_tables), for windows epoch uslots_epoch and build uslots_serial
-    PgBuf uslots;
-    int32_t *u_cta_seg_first = nullptr, *u_seg_cta_lo = nullptr, *u_seg_cta_hi = nullptr;
-    int64_t* u_cta_slot_off = nullptr;
-    int64_t utotal_slots = 0;
-    uint64_t uslots_epoch = 0, uslots_serial = 0;
-    int uslots_Q = 0;
+    UniformPass up;           // packed (popgen cache only)
 };
 
 // The one-hot rows' launch plan for this population map, or the error that refuses such rows.
@@ -1886,8 +1922,15 @@ int byte_plan(pg_ctx* ctx, const std::vector<int32_t>& hap_pop_local, int Ppad, 
 
 // The slots of a launch whose CTA b adds the sites [bound[b], bound[b + 1]): each CTA gets nw slots of Q words per segment it
 // touches (cta_seg_first, cta_slot_off), and each segment the range of CTAs that touch it (seg_cta_lo / _hi), for k1_finalize.
-// Returns the slot words.
-int64_t slot_tables(const std::vector<int64_t>& brk, const std::vector<int64_t>& bound, int nw, int Q, K1Launch& L) {
+// On the host, until push_slots has uploaded them.
+struct HostSlots {
+    std::vector<int32_t> cta_seg_first, seg_cta_lo, seg_cta_hi;
+    std::vector<int64_t> cta_slot_off;
+    int64_t words = 0;
+    size_t bytes() const { return cta_seg_first.size() * 12 + seg_cta_lo.size() * 8 + 4 * 16; }   // on the device (push)
+};
+
+void slot_tables(const std::vector<int64_t>& brk, const std::vector<int64_t>& bound, int nw, int Q, HostSlots& L) {
     const int B = (int)bound.size() - 1;
     const int nseg = (int)brk.size() - 1;
     L.cta_seg_first.assign(B, 0);
@@ -1916,12 +1959,52 @@ int64_t slot_tables(const std::vector<int64_t>& brk, const std::vector<int64_t>&
             L.seg_cta_hi[g] = std::max(L.seg_cta_hi[g], b);
         }
     }
-    return off;
+    L.words = off;
+}
+
+// Uploads h behind base + o; the caller synchronises before h goes away.
+int push_slots(pg_ctx* ctx, uint8_t* base, size_t& o, const HostSlots& h, SlotTables& st) {
+    PG_TRY(push(ctx, base, o, h.cta_seg_first.data(), h.cta_seg_first.size(), &st.cta_seg_first));
+    PG_TRY(push(ctx, base, o, h.cta_slot_off.data(), h.cta_slot_off.size(), &st.cta_slot_off));
+    PG_TRY(push(ctx, base, o, h.seg_cta_lo.data(), h.seg_cta_lo.size(), &st.seg_cta_lo));
+    PG_TRY(push(ctx, base, o, h.seg_cta_hi.data(), h.seg_cta_hi.size(), &st.seg_cta_hi));
+    st.words = h.words;
+    return PG_OK;
+}
+
+// The fields of a launch's parameters that follow from its plan and the population tables (dt: the tables on the device;
+// packed: the companion's rows and (word, mask) entries instead of the one-hot rows and chunk masks).  The rest is zero and
+// its caller's: the site range; segments and slots of a windowed launch; counts_* of a counts launch.
+void fill_params(K1Params& p, const pg_ctx* ctx, const K1Plan& pl, const PopTables& pt, const DevTables& dt, bool packed) {
+    memset(&p, 0, sizeof(p));
+    p.geno = packed ? (const uint8_t*)ctx->d_packed : (const uint8_t*)ctx->d_geno;
+    p.pos = ctx->d_pos;
+    p.num_tiles = pl.num_tiles;
+    p.pitch = pl.pitch;
+    p.G = pl.G;
+    p.I = pl.I;
+    p.T = pl.T;
+    p.wpt = pl.wpt;
+    p.nw = pl.nw;
+    p.stages = pl.stages;
+    p.tile_bytes = pl.tile_bytes;
+    p.ent_chunk = dt.ent_chunk;
+    p.ent_mask = dt.ent_mask;
+    p.word_ent = dt.word_ent;
+    p.wd = (ctx->H + 31) / 32;
+    p.n_ent = packed ? (int)pt.word_ent.size() / 2 : (int)pt.ent_chunk.size();
+    for (int X = 0; X < PG_MAX_K1_POPS; ++X) {
+        p.ent_lo[X] = pt.ent_lo[X];
+        p.ent_hi[X] = pt.ent_hi[X];
+        p.full_lo[X] = pt.full_lo[X];
+        p.full_hi[X] = pt.full_hi[X];
+        p.popN[X] = pt.popN[X];
+    }
 }
 
 // packed: plan and tables for the packed companion's rows (k1_site_pass_packed) instead of the one-hot rows
-int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_pop_local, int Ppad, int Q, int nw,
-                     int force_G = 0, bool packed = false) {
+int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_pop_local, int Ppad, int Q, int nw, int force_G,
+                     bool packed) {
     K1Launch& L = c.L;
     DevTables& dt = c.dt;
     PopTables& pt = c.pt;
@@ -1937,16 +2020,15 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
     } else {
         PG_TRY(byte_plan(ctx, hap_pop_local, Ppad, nw, force_G, pt, L.plan));
     }
-    const int n_ent = packed ? (int)pt.word_ent.size() / 2 : (int)pt.ent_chunk.size();
     for (int X = 0; X < Ppad; ++X) PG_CHECK(pt.popN[X] <= 65535, "a population has more than 65535 haplotypes");
     const K1Plan& pl = L.plan;
     const int B = pl.ctas;
-    const int nseg = (int)ctx->brk.size() - 1;
     std::vector<int64_t> bound(B + 1);
     for (int b = 0; b <= B; ++b) bound[b] = std::min<int64_t>((int64_t)b * pl.num_tiles / B * pl.T, ctx->S);
-    L.total_slots = slot_tables(ctx->brk, bound, nw, Q, L);
+    HostSlots hs;
+    slot_tables(ctx->brk, bound, nw, Q, hs);
     size_t bytes = 4096 + pt.ent_mask.size() * 4 + pt.ent_chunk.size() * 4 + pt.word_ent.size() * 4 + ctx->brk.size() * 8 +
-                   (size_t)B * 12 + (size_t)std::max(nseg, 1) * 8 + (size_t)ctx->W * 24 + 17 * 16;
+                   hs.bytes() + (size_t)ctx->W * 24 + 13 * 16;
     PG_TRY(c.tables.ensure(bytes));
     uint8_t* base = (uint8_t*)c.tables.p;
     size_t o = 0;
@@ -1958,10 +2040,7 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
     PG_TRY(push(ctx, base, o, pt.word_ent.data(), pt.word_ent.size(), &d_word_ent));
     dt.word_ent = reinterpret_cast<uint2*>(d_word_ent);
     PG_TRY(push(ctx, base, o, ctx->brk.data(), ctx->brk.size(), &dt.brk));
-    PG_TRY(push(ctx, base, o, L.cta_seg_first.data(), L.cta_seg_first.size(), &dt.cta_seg_first));
-    PG_TRY(push(ctx, base, o, L.cta_slot_off.data(), L.cta_slot_off.size(), &dt.cta_slot_off));
-    PG_TRY(push(ctx, base, o, L.seg_cta_lo.data(), L.seg_cta_lo.size(), &dt.seg_cta_lo));
-    PG_TRY(push(ctx, base, o, L.seg_cta_hi.data(), L.seg_cta_hi.size(), &dt.seg_cta_hi));
+    PG_TRY(push_slots(ctx, base, o, hs, L.slots));
     PG_TRY(push(ctx, base, o, ctx->win_seg_lo.data(), ctx->win_seg_lo.size(), &dt.win_seg_lo));
     PG_TRY(push(ctx, base, o, ctx->win_seg_hi.data(), ctx->win_seg_hi.size(), &dt.win_seg_hi));
     PG_TRY(push(ctx, base, o, ctx->win_lo.data(), ctx->win_lo.size(), &dt.win_lo));
@@ -1971,131 +2050,84 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
 
     K1Params& p = L.prm;
-    memset(&p, 0, sizeof(p));
-    p.geno = packed ? (const uint8_t*)ctx->d_packed : (const uint8_t*)ctx->d_geno;
-    p.word_ent = dt.word_ent;
-    p.wd = (ctx->H + 31) / 32;
-    p.pos = ctx->d_pos;
+    fill_params(p, ctx, pl, pt, dt, packed);
     p.site_begin = 0;
     p.site_end = ctx->S;
-    p.num_tiles = pl.num_tiles;
-    p.pitch = pl.pitch;
-    p.G = pl.G;
-    p.I = pl.I;
-    p.T = pl.T;
-    p.wpt = pl.wpt;
-    p.nw = nw;
-    p.stages = pl.stages;
-    p.tile_bytes = pl.tile_bytes;
-    p.ent_chunk = dt.ent_chunk;
-    p.ent_mask = dt.ent_mask;
-    p.n_ent = n_ent;
-    for (int X = 0; X < PG_MAX_K1_POPS; ++X) {
-        p.ent_lo[X] = pt.ent_lo[X];
-        p.ent_hi[X] = pt.ent_hi[X];
-        p.full_lo[X] = pt.full_lo[X];
-        p.full_hi[X] = pt.full_hi[X];
-        p.popN[X] = pt.popN[X];
-    }
     p.brk = dt.brk;
-    p.nseg = nseg;
-    p.cta_seg_first = dt.cta_seg_first;
-    p.cta_slot_off = dt.cta_slot_off;
+    p.nseg = (int)ctx->brk.size() - 1;
+    p.cta_seg_first = L.slots.cta_seg_first;
+    p.cta_slot_off = L.slots.cta_slot_off;
     return PG_OK;
 }
 
-// per-call part: zeroed slots
-int arm_slots(pg_ctx* ctx, K1Cache& c, int64_t total_slots = -1) {
-    const size_t bytes = (size_t)std::max<int64_t>(total_slots >= 0 ? total_slots : c.L.total_slots, 1) * 8;
+// per-call part of the launch that runs: its slots zeroed, and the addresses that an upload of the same shape may have moved
+// (rows: what the launch streams)
+int arm_slots(pg_ctx* ctx, K1Launch& L, const void* rows) {
+    const size_t bytes = (size_t)std::max<int64_t>(L.slots.words, 1) * 8;
     PG_TRY(ctx->part.ensure(bytes));
     PG_CUDA(cudaMemsetAsync(ctx->part.p, 0, bytes, ctx->stream));
-    c.L.prm.part = (unsigned long long*)ctx->part.p;
-    c.L.prm.geno = c.packed ? (const uint8_t*)ctx->d_packed : (const uint8_t*)ctx->d_geno;
-    c.L.prm.pos = ctx->d_pos;
+    L.prm.part = (unsigned long long*)ctx->part.p;
+    L.prm.geno = (const uint8_t*)rows;
+    L.prm.pos = ctx->d_pos;
     return PG_OK;
 }
 
-template <int MODE, int P, int NW, bool BYTES>
-int launch_site_pass_nw(pg_ctx* ctx, const K1Launch& L, const char* name) {
-    auto kern = k1_site_pass<MODE, P, NW, BYTES>;
-    static bool attr_set[64] = {};    // per instantiation and per device (the attribute is per device)
-    if (!attr_set[ctx->device & 63]) {
-        PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set[ctx->device & 63] = true;
-    }
-    const int ti = pg_time_begin(ctx, name);
-    kern<<<L.plan.ctas, (NW + 1) * 32, L.plan.smem_bytes, ctx->stream>>>(L.prm);
-    pg_time_end(ctx, ti);
-    PG_CUDA(cudaGetLastError());
-    return PG_OK;
-}
-
-// consumer warps per CTA: 12 (+ the producer = 416 threads, 128 registers each) for rows below 1 KiB; 8 (up to 168
-// registers, no spills) for longer rows, where the 8-population instantiations need the registers (tools/k1_sweep2.py
-// compares the two)
-int k1_env_nw12() {
-    const char* e = getenv("PG_K1_NW");
-    return (e && *e && atoi(e) == 8) ? 8 : 12;
-}
-int k1_nw_for(int pitch) {
-    const char* e = getenv("PG_K1_NW");
-    const int v = (e && *e) ? atoi(e) : (pitch >= 1024 ? 8 : 12);
-    return v == 12 ? 12 : 8;
-}
-
-template <int MODE, int P, int NW>
-int launch_site_pass_lp(pg_ctx* ctx, const K1Launch& L, const char* name) {
-    auto kern = k1_site_pass_lp<MODE, P, NW>;
+// One site-pass kernel on the launch's grid, NW consumer warps and the producer warp per CTA.  The kernels take more dynamic
+// shared memory than the default limit, which needs an attribute: set once per kernel (the flags are the instantiation's) and
+// per device (the attribute is per device).
+template <auto Kern, int NW>
+int launch_kernel(pg_ctx* ctx, const K1Launch& L, const char* name) {
     static bool attr_set[64] = {};
     if (!attr_set[ctx->device & 63]) {
-        PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        PG_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set[ctx->device & 63] = true;
     }
     const int ti = pg_time_begin(ctx, name);
-    kern<<<L.plan.ctas, (NW + 1) * 32, L.plan.smem_bytes, ctx->stream>>>(L.prm);
+    Kern<<<L.plan.ctas, (NW + 1) * 32, L.plan.smem_bytes, ctx->stream>>>(L.prm);
     pg_time_end(ctx, ti);
     PG_CUDA(cudaGetLastError());
     return PG_OK;
 }
 
+// The byte pass: the lane-per-population kernel, the byte-packed counts or the general kernel, as the launch says.
 template <int MODE, int P>
 int launch_site_pass(pg_ctx* ctx, const K1Launch& L, const char* name) {
     constexpr bool POPGEN_MODE = (MODE == MODE_POPGEN || MODE == MODE_POPGEN_FREQ);
+    const bool w12 = L.prm.nw == 12;
     if constexpr ((POPGEN_MODE || MODE == MODE_COUNTS) && (P == 4 || P == 8)) {
-        if (L.prm.lanepop) {
-            if (L.prm.nw == 12) return launch_site_pass_lp<MODE, P, 12>(ctx, L, name);
-            return launch_site_pass_lp<MODE, P, 8>(ctx, L, name);
-        }
+        if (L.prm.lanepop)
+            return w12 ? launch_kernel<k1_site_pass_lp<MODE, P, 12>, 12>(ctx, L, name)
+                       : launch_kernel<k1_site_pass_lp<MODE, P, 8>, 8>(ctx, L, name);
     }
     if constexpr (POPGEN_MODE) {
-        if (L.prm.bytes) {
-            if (L.prm.nw == 12) return launch_site_pass_nw<MODE, P, 12, true>(ctx, L, name);
-            return launch_site_pass_nw<MODE, P, 8, true>(ctx, L, name);
-        }
+        if (L.prm.bytes)
+            return w12 ? launch_kernel<k1_site_pass<MODE, P, 12, true>, 12>(ctx, L, name)
+                       : launch_kernel<k1_site_pass<MODE, P, 8, true>, 8>(ctx, L, name);
     }
-    if (L.prm.nw == 12) return launch_site_pass_nw<MODE, P, 12, false>(ctx, L, name);
-    return launch_site_pass_nw<MODE, P, 8, false>(ctx, L, name);
+    return w12 ? launch_kernel<k1_site_pass<MODE, P, 12, false>, 12>(ctx, L, name)
+               : launch_kernel<k1_site_pass<MODE, P, 8, false>, 8>(ctx, L, name);
 }
 
-template <int MODE, int P, int NW, bool UNI>
-int launch_site_pass_packed_nw(pg_ctx* ctx, const K1Launch& L, const char* name) {
-    auto kern = k1_site_pass_packed<MODE, P, NW, UNI>;
-    static bool attr_set[64] = {};
-    if (!attr_set[ctx->device & 63]) {
-        PG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set[ctx->device & 63] = true;
-    }
-    const int ti = pg_time_begin(ctx, name);
-    kern<<<L.plan.ctas, (NW + 1) * 32, L.plan.smem_bytes, ctx->stream>>>(L.prm);
-    pg_time_end(ctx, ti);
-    PG_CUDA(cudaGetLastError());
-    return PG_OK;
-}
-
-template <int MODE, int P, bool UNI = false>
+template <int MODE, int P, bool UNI>
 int launch_site_pass_packed(pg_ctx* ctx, const K1Launch& L, const char* name) {
-    if (L.prm.nw == 12) return launch_site_pass_packed_nw<MODE, P, 12, UNI>(ctx, L, name);
-    return launch_site_pass_packed_nw<MODE, P, 8, UNI>(ctx, L, name);
+    return L.prm.nw == 12 ? launch_kernel<k1_site_pass_packed<MODE, P, 12, UNI>, 12>(ctx, L, name)
+                          : launch_kernel<k1_site_pass_packed<MODE, P, 8, UNI>, 8>(ctx, L, name);
+}
+
+// f(P) with the padded population count (2, 4 or 8) as a compile-time constant
+template <typename F>
+int with_pops(int Pp, F&& f) {
+    if (Pp == 2) return f(std::integral_constant<int, 2>());
+    if (Pp == 4) return f(std::integral_constant<int, 4>());
+    return f(std::integral_constant<int, 8>());
+}
+
+// f(MODE, P) for the popgen pass, with or without the popFreq counters
+template <typename F>
+int with_popgen_mode(bool with_freq, int Pp, F&& f) {
+    return with_pops(Pp, [&](auto P) {
+        return with_freq ? f(std::integral_constant<int, MODE_POPGEN_FREQ>(), P) : f(std::integral_constant<int, MODE_POPGEN>(), P);
+    });
 }
 
 // Streaming only the varied rows costs 6 + (1 - u) * (pitch + 2) bytes per site (position, code; row, slot) against
@@ -2110,15 +2142,15 @@ int uni_stage_bytes(int R, int Tmax, int pitch) {
     return (int)align_up((size_t)R * pitch + (size_t)(Tmax + 4) * 4 + (size_t)Tmax * 2 + align_up((size_t)R * 2, 16), 128);
 }
 
-// The stream's geometry for the plan uplan: a tile bound of Tmax = 512 sites (PG_K1_UNI_TMAX, a multiple of 8 up to 32768), and a
+// The stream's geometry for the plan u.plan: a tile bound of Tmax = 512 sites (PG_K1_UNI_TMAX, a multiple of 8 up to 32768), and a
 // budget of R varied rows per tile, one per lane of a team at the plan's lanes per site, halved (down to one warp's lanes)
 // while the ring would hold fewer than 2 stages (PG_K1_UNI_R sets R).  The ring: as many such stages as fit
 // (pg_k1_ring_stages).  tools/packed_site_pass.py --sweep (H100 80GB HBM3, 700 W): C2 (4 warps per team, 160-byte rows)
 // R = 32 / 64 / 128 / 256 0.50 / 0.30 / 0.22 / 0.23 ms; C5 (2 warps, 608-byte rows) R = 32 / 64 / 128 1.40 / 1.09 / 1.62 ms
 // (8, 5 and 2 stages): rows that fill the lanes matter more than stages beyond the teams' count.  Tmax = 256 / 512 / 2048:
 // C2 0.30 / 0.22 / 0.24 ms.
-void uni_geometry(K1Cache& c) {
-    const K1Plan& pl = c.uplan;
+void uni_geometry(UniformPass& u) {
+    const K1Plan& pl = u.plan;
     int Tmax = 512;
     if (const char* e = getenv("PG_K1_UNI_TMAX")) Tmax = std::max(8, std::min(32768, (atoi(e) + 7) / 8 * 8));
     const int lanes = 32 / std::max(1, pl.G);
@@ -2127,22 +2159,22 @@ void uni_geometry(K1Cache& c) {
     if (er && *er) {
         R = std::max(1, std::min(0x7fff, atoi(er)));
     } else {
-        while (R > lanes && pg_k1_ring_stages(uni_stage_bytes(R, Tmax, pl.pitch), c.utable) < 2) R /= 2;
+        while (R > lanes && pg_k1_ring_stages(uni_stage_bytes(R, Tmax, pl.pitch), u.table_bytes) < 2) R /= 2;
     }
-    c.uR = R;
-    c.uTmax = Tmax;
-    c.ubytes = uni_stage_bytes(R, Tmax, pl.pitch);
-    c.ustages = pl.stages >= 2 ? pg_k1_ring_stages(c.ubytes, c.utable) : 0;
+    u.R = R;
+    u.Tmax = Tmax;
+    u.stage_bytes = uni_stage_bytes(R, Tmax, pl.pitch);
+    u.stages = pl.stages >= 2 ? pg_k1_ring_stages(u.stage_bytes, u.table_bytes) : 0;
 }
 
-// (Re)builds c.us for the current data and geometry when they changed: two host synchronisations per rebuild (the count of
+// (Re)builds u.us for the current data and geometry when they changed: two host synchronisations per rebuild (the count of
 // varied rows, which sizes the buffers; the count of tiles with the CTAs' first sites, which size the launch and its slots),
 // nothing on a call over unchanged data.  PG_K1_UNIFORM_FORCE keeps the stream whatever the uniform fraction (tests on missing
 // data).
-int uniform_prepare(pg_ctx* ctx, K1Cache& c) {
-    UniformStream& us = c.us;
+int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
+    UniformStream& us = u.us;
     const bool forced = getenv("PG_K1_UNIFORM_FORCE") != nullptr;
-    const int R = c.uR, Tmax = c.uTmax;
+    const int R = u.R, Tmax = u.Tmax;
     if (us.gen == ctx->data_gen && us.R == R && us.Tmax == Tmax && us.forced == forced) return PG_OK;
     us.gen = ctx->data_gen;
     us.R = R;
@@ -2151,7 +2183,7 @@ int uniform_prepare(pg_ctx* ctx, K1Cache& c) {
     us.in_use = false;
     us.varied = ctx->S;
     us.serial += 1;
-    if (c.ustages < 2) return PG_OK;
+    if (u.stages < 2) return PG_OK;
     const int64_t S = ctx->S;
     constexpr int CH = 2048;                  // the chunks of the first pass (varied counts, then each varied row's site)
     const int64_t nc = (S + CH - 1) / CH;
@@ -2231,24 +2263,45 @@ int uniform_prepare(pg_ctx* ctx, K1Cache& c) {
     return PG_OK;
 }
 
-// The slot tables of the stream's CTA ranges, rebuilt when the windows (epoch), the stream or the slot width changed.
-int uniform_slots(pg_ctx* ctx, K1Cache& c, int Q) {
-    if (c.uslots_epoch == ctx->epoch && c.uslots_serial == c.us.serial && c.uslots_Q == Q) return PG_OK;
-    K1Launch T;
-    c.utotal_slots = slot_tables(ctx->brk, c.us.bound, c.L.prm.nw, Q, T);
-    const size_t B = T.cta_seg_first.size(), ns = T.seg_cta_lo.size();
-    PG_TRY(c.uslots.ensure(B * 12 + ns * 8 + 4 * 16));
-    uint8_t* base = (uint8_t*)c.uslots.p;
+// The slot tables of the stream's CTA ranges and the launch that uses them (L: the cache's packed launch, whose tables and
+// segments it shares), rebuilt when the windows (epoch), the stream, the slot width or the ring (PG_K1_STAGES) changed.
+// Tiles of at most R varied rows and Tmax sites, a stage sized for such a tile: at 70 % uniform sites it is less than half a
+// fixed tile's bytes, so the ring has more stages than teams and a team's next tile is in flight while it works on this one.
+// Its CTAs own the stream's tile ranges and add into slots of their own.
+int uniform_slots(pg_ctx* ctx, UniformPass& u, const K1Launch& L, int Q) {
+    if (u.slots_epoch == ctx->epoch && u.slots_serial == u.us.serial && u.slots_Q == Q && u.L.plan.stages == u.stages)
+        return PG_OK;
+    HostSlots hs;
+    slot_tables(ctx->brk, u.us.bound, L.prm.nw, Q, hs);
+    PG_TRY(u.slot_buf.ensure(hs.bytes()));
     size_t o = 0;
-    PG_TRY(push(ctx, base, o, T.cta_seg_first.data(), B, &c.u_cta_seg_first));
-    PG_TRY(push(ctx, base, o, T.cta_slot_off.data(), B, &c.u_cta_slot_off));
-    PG_TRY(push(ctx, base, o, T.seg_cta_lo.data(), ns, &c.u_seg_cta_lo));
-    PG_TRY(push(ctx, base, o, T.seg_cta_hi.data(), ns, &c.u_seg_cta_hi));
-    PG_CHECK(o <= c.uslots.cap, "internal: slot table buffer overflow");
+    PG_TRY(push_slots(ctx, (uint8_t*)u.slot_buf.p, o, hs, u.L.slots));
+    PG_CHECK(o <= u.slot_buf.cap, "internal: slot table buffer overflow");
     PG_CUDA(cudaStreamSynchronize(ctx->stream));     // the host vectors must outlive the copies
-    c.uslots_epoch = ctx->epoch;
-    c.uslots_serial = c.us.serial;
-    c.uslots_Q = Q;
+    K1Plan& pl = u.L.plan;
+    pl = u.plan;
+    pl.T = u.Tmax;
+    pl.num_tiles = u.us.nt;
+    pl.ctas = (int)u.us.bound.size() - 1;
+    pl.tile_bytes = u.stage_bytes;
+    pl.stages = u.stages;
+    pl.smem_bytes = pl.stages * pl.tile_bytes + 256 + u.table_bytes;
+    K1Params& p = u.L.prm;
+    p = L.prm;
+    p.T = pl.T;
+    p.num_tiles = pl.num_tiles;
+    p.stages = pl.stages;
+    p.tile_bytes = pl.tile_bytes;
+    p.row_cap = u.R;
+    p.cta_seg_first = u.L.slots.cta_seg_first;
+    p.cta_slot_off = u.L.slots.cta_slot_off;
+    p.row0 = (const int64_t*)u.us.row0.p;
+    p.site_lo = (const int64_t*)u.us.site_lo.p;
+    p.codes = (const uint16_t*)u.us.codes.p;
+    p.code_pitch = u.us.code_pitch;
+    u.slots_epoch = ctx->epoch;
+    u.slots_serial = u.us.serial;
+    u.slots_Q = Q;
     return PG_OK;
 }
 
@@ -2259,13 +2312,14 @@ K1Cache* cache_of(pg_ctx* ctx, int slot) {
     return static_cast<K1Cache*>(ctx->k1_cache[slot]);
 }
 
-void fill_fin(FinParams& fp, pg_ctx* ctx, const K1Cache& c, int Q, int QI) {
+// slots: those of the launch that filled ctx->part
+void fill_fin(FinParams& fp, pg_ctx* ctx, const K1Cache& c, const SlotTables& slots, int Q, int QI) {
     memset(&fp, 0, sizeof(fp));
     fp.part = (const unsigned long long*)ctx->part.p;
-    fp.seg_cta_lo = c.dt.seg_cta_lo;
-    fp.seg_cta_hi = c.dt.seg_cta_hi;
-    fp.cta_seg_first = c.dt.cta_seg_first;
-    fp.cta_slot_off = c.dt.cta_slot_off;
+    fp.seg_cta_lo = slots.seg_cta_lo;
+    fp.seg_cta_hi = slots.seg_cta_hi;
+    fp.cta_seg_first = slots.cta_seg_first;
+    fp.cta_slot_off = slots.cta_slot_off;
     fp.win_seg_lo = c.dt.win_seg_lo;
     fp.win_seg_hi = c.dt.win_seg_hi;
     fp.win_lo = c.dt.win_lo;
@@ -2286,6 +2340,111 @@ void fill_fin(FinParams& fp, pg_ctx* ctx, const K1Cache& c, int Q, int QI) {
     }
 }
 
+template <int MODE>
+int launch_finalize(pg_ctx* ctx, const FinParams& fp) {
+    const int ti = pg_time_begin(ctx, "k1_finalize");
+    k1_finalize<MODE><<<(unsigned)std::min<int64_t>(fp.W, 65535), 64, 0, ctx->stream>>>(fp);
+    pg_time_end(ctx, ti);
+    PG_CUDA(cudaGetLastError());
+    return PG_OK;
+}
+
+unsigned long long nan_bits() {
+    const double qn = NAN;
+    unsigned long long u;
+    memcpy(&u, &qn, 8);
+    return u;
+}
+
+// The matrix has no sites: every window's record is `one`.  On the ctx stream, so that work queued behind it (the pipelined
+// gather's read-back) sees the records.
+int put_empty_records(pg_ctx* ctx, const std::vector<unsigned long long>& one, void* d_rec) {
+    std::vector<unsigned long long> h;
+    h.reserve((size_t)ctx->W * one.size());
+    for (int64_t w = 0; w < ctx->W; ++w) h.insert(h.end(), one.begin(), one.end());
+    PG_CUDA(cudaMemcpyAsync(d_rec, h.data(), h.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    return PG_OK;
+}
+
+// smallest n with (double)n / N >= minData, N + 1 when there is none: the reference's test of a population's non-missing
+// count, exact in integers (genomics.py:1657-1660 for ABBABABA, 1597-1600 for fourPop)
+int min_count(int N, double min_data) {
+    for (int n = 0; n <= N; ++n)
+        if ((double)n * 1.0 / (double)N >= min_data) return n;
+    return N + 1;
+}
+
+// Site pass + finalize of a statistic over four selected populations (cache `slot`, Q words per slot), enqueued on the ctx
+// stream without synchronising: records of RC words [sites, pos_sum, statistics ...] are left in the DEVICE buffer d_rec.
+// With no sites the words [2, nan_end) of a record are NaN and the others 0.  launch(L) runs the site pass; `who` heads the
+// error messages.
+template <int FIN_MODE, typename Launch>
+int fourpop_enqueue(pg_ctx* ctx, const char* who, int slot, int Q, int RC, int nan_end, const int* sel, double min_data,
+                    int variant, void* d_rec, Launch launch) {
+    PG_CHECK(ctx->P >= 1, "%s: call pg_set_pops first", who);
+    for (int k = 0; k < 4; ++k) {
+        PG_CHECK(sel[k] >= 0 && sel[k] < ctx->P, "%s: population index %d out of range", who, sel[k]);
+        for (int j = 0; j < k; ++j) PG_CHECK(sel[j] != sel[k], "%s: populations must be distinct", who);
+    }
+    PG_CUDA(cudaSetDevice(ctx->device));
+    pg_timings_reset(ctx);
+    if (ctx->W == 0) return PG_OK;
+    if (ctx->S == 0) {
+        std::vector<unsigned long long> one(RC, 0ull);
+        std::fill(one.begin() + 2, one.begin() + nan_end, nan_bits());
+        return put_empty_records(ctx, one, d_rec);
+    }
+    K1Cache& c = *cache_of(ctx, slot);
+    if (!c.valid || c.epoch != ctx->epoch || memcmp(c.sel, sel, 4 * sizeof(int)) != 0) {
+        c.valid = false;
+        std::vector<int32_t> local(ctx->H, -1);
+        for (int h = 0; h < ctx->H; ++h)
+            for (int k = 0; k < 4; ++k)
+                if (ctx->hap_pop[h] == sel[k]) local[h] = k;
+        PG_TRY(prepare_windowed(ctx, c, local, 4, Q, k1_nw_for(ctx->pitch, false), /*force_G=*/0, /*packed=*/false));
+        for (int k = 0; k < 4; ++k) PG_CHECK(c.pt.popN[k] >= 1, "%s: population %d has no haplotypes", who, sel[k]);
+        memcpy(c.sel, sel, 4 * sizeof(int));
+        c.epoch = ctx->epoch;
+        c.valid = true;
+    }
+    for (int k = 0; k < 4; ++k) c.L.prm.thr[k] = min_count(c.pt.popN[k], min_data);
+    c.L.prm.variant = variant;
+    PG_TRY(arm_slots(ctx, c.L, ctx->d_geno));
+    PG_TRY(launch(c.L));
+    FinParams fp;
+    fill_fin(fp, ctx, c, c.L.slots, Q, 3);
+    fp.P = 4;
+    fp.Ppad = 4;
+    fp.rec = (unsigned long long*)d_rec;
+    fp.RC = RC;
+    return launch_finalize<FIN_MODE>(ctx, fp);
+}
+
+// Enqueue, read the records back and split them: [sites, pos_sum, RC - 3 statistics, sitesUsed]
+template <typename Enqueue>
+int fourpop_read(pg_ctx* ctx, int RC, Enqueue enqueue, double* out, double* sites_used, int64_t* n_sites, int64_t* pos_sum) {
+    const int64_t W = ctx->W;
+    PG_CUDA(cudaSetDevice(ctx->device));
+    PG_TRY(ctx->out_d.ensure((size_t)std::max<int64_t>(W, 1) * RC * 8 + 64));
+    PG_TRY(enqueue(ctx->out_d.p));
+    if (W == 0) return PG_OK;
+    void* hp = nullptr;
+    PG_TRY(pg_pinned(ctx, (size_t)W * RC * 8 + 64, &hp));
+    const unsigned long long* hrec = (const unsigned long long*)hp;
+    PG_CUDA(cudaMemcpyAsync(hp, ctx->out_d.p, (size_t)W * RC * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    const int n = RC - 3;
+    for (int64_t w = 0; w < W; ++w) {
+        const unsigned long long* r = hrec + (size_t)w * RC;
+        n_sites[w] = (int64_t)r[0];
+        pos_sum[w] = (int64_t)r[1];
+        memcpy(out + (size_t)w * n, r + 2, (size_t)n * 8);
+        memcpy(sites_used + w, r + 2 + n, 8);
+    }
+    return PG_OK;
+}
+
 }  // namespace
 
 void pg_k1_cache_free(pg_ctx* ctx) {
@@ -2293,7 +2452,7 @@ void pg_k1_cache_free(pg_ctx* ctx) {
         if (ctx->k1_cache[k]) {
             K1Cache* c = static_cast<K1Cache*>(ctx->k1_cache[k]);
             c->tables.release();
-            c->us.release();
+            c->up.release();
             delete c;
             ctx->k1_cache[k] = nullptr;
         }
@@ -2322,20 +2481,10 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     const int64_t W = ctx->W;
     if (W == 0) return PG_OK;
     if (ctx->S == 0) {
-        std::vector<unsigned long long> h((size_t)W * RC);
-        const double qn = NAN;
-        unsigned long long nanbits;
-        memcpy(&nanbits, &qn, 8);
-        for (int64_t w = 0; w < W; ++w) {
-            h[w * RC] = 0;
-            h[w * RC + 1] = 0;
-            h[w * RC + 2] = (0 < min_sites) ? 0 : 1;
-            for (int k = 3; k < RC; ++k) h[w * RC + k] = nanbits;
-        }
-        // on the ctx stream, so that work queued behind it (the pipelined gather's read-back) sees the records
-        PG_CUDA(cudaMemcpyAsync(d_rec, h.data(), h.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-        PG_CUDA(cudaStreamSynchronize(ctx->stream));
-        return PG_OK;
+        std::vector<unsigned long long> one(RC, nan_bits());
+        one[0] = one[1] = 0;
+        one[2] = (0 < min_sites) ? 0 : 1;
+        return put_empty_records(ctx, one, d_rec);
     }
     const int Pp = many ? 2 : pad_pops(P);
     const bool wf = ctx->want_freq && !many;
@@ -2344,12 +2493,15 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     // the byte pass runs when the context has no companion, and PG_K1_BYTE_PASS selects it for the tests that compare the two.
     const bool packed = ctx->d_packed != nullptr && !getenv("PG_K1_BYTE_PASS");
     K1Cache& c = *cache_of(ctx, 0);
+    UniformPass& u = c.up;
     if (!c.valid || c.epoch != ctx->epoch || c.packed != packed) {
         c.valid = false;
+        int maxN = 0;
         for (int x = 0; x < P; ++x) {
             int N = 0;
             for (int h = 0; h < ctx->H; ++h) N += ctx->hap_pop[h] == x;
             PG_CHECK(N >= 1, "pg_popgen: population %d has no haplotypes", x);
+            maxN = std::max(maxN, N);
         }
         std::vector<int32_t> collapsed;
         if (many) {
@@ -2357,127 +2509,64 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
             for (int32_t& v : collapsed) v = v >= 0 ? 0 : -1;
         }
         const std::vector<int32_t>& pop_map = many ? collapsed : ctx->hap_pop;
+        PopTables pt;
         if (packed) {
             // the rows the byte pass refuses are refused here too, so that whether a call runs never depends on the
             // companion having found memory
-            PopTables pt;
             K1Plan bp;
-            PG_TRY(byte_plan(ctx, pop_map, Pp, k1_nw_for(ctx->pitch), 0, pt, bp));
+            PG_TRY(byte_plan(ctx, pop_map, Pp, k1_nw_for(ctx->pitch, false), 0, pt, bp));
             c.lanepop = false;
-            const int nw = k1_nw_for(ctx->packed_pitch);
-            PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, 0, true));
-            c.utable = table_bytes_of(c.pt) + UNI_SMEM_BYTES;
-            c.uplan = pg_make_k1_plan_rows(ctx->S, ctx->packed_pitch, ctx->sm_count, c.utable, nw, 0, 4);
-            if (!pg_k1_plan_ok(c.uplan)) c.uplan.stages = 0;    // no room for the codes: every row is streamed
+            const int nw = k1_nw_for(ctx->packed_pitch, false);
+            PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, /*force_G=*/0, /*packed=*/true));
+            u.table_bytes = table_bytes_of(c.pt) + UNI_SMEM_BYTES;
+            u.plan = pg_make_k1_plan_rows(ctx->S, ctx->packed_pitch, ctx->sm_count, u.table_bytes, nw, 0, 4);
+            if (!pg_k1_plan_ok(u.plan)) u.plan.stages = 0;    // no room for the codes: every row is streamed
+            u.slots_epoch = 0;                                  // u.L follows c.L
         } else {
             // long rows, 4 or 8 real populations of <= 255 haplotypes: one lane per population (k1_site_pass_lp)
-            int maxN = 0;
-            for (int x = 0; x < P && !many; ++x) {
-                int N = 0;
-                for (int h = 0; h < ctx->H; ++h) N += ctx->hap_pop[h] == x;
-                maxN = std::max(maxN, N);
-            }
-            bool lp = !many && (Pp == 4 || Pp == 8) && Pp == P && maxN <= 255 && ctx->pitch >= 1024 && !getenv("PG_K1_NO_BYTES");
-            if (const char* e = getenv("PG_K1_LANEPOP")) {
-                lp = atoi(e) != 0 && !many && (Pp == 4 || Pp == 8) && maxN <= 255 && !getenv("PG_K1_NO_BYTES");
-            } else if (lp) {
-                PopTables pt;
-                build_tables(pop_map, ctx->H, ctx->pitch / 16, Pp, pt);
-                lp = lanepop_fits(ctx->S, ctx->H, ctx->sm_count, table_bytes_of(pt), k1_env_nw12(), Pp);
-            }
-            c.lanepop = lp;
-            const int nw = lp ? k1_env_nw12() : k1_nw_for(ctx->pitch);
-            PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, lp ? Pp : 0));
+            build_tables(pop_map, ctx->H, ctx->pitch / 16, Pp, pt);
+            const WarpChoice wc = choose_warps(ctx, ctx->S, Pp, Pp == P, table_bytes_of(pt), byte_counts(maxN));
+            c.lanepop = wc.lanepop;
+            PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, wc.nw, wc.lanepop ? Pp : 0, /*packed=*/false));
         }
         c.packed = packed;
         c.epoch = ctx->epoch;
         c.valid = true;
     }
-    {
-        long long maxN = 1;
-        for (int X = 0; X < Pp; ++X) maxN = std::max<long long>(maxN, c.pt.popN[X]);
-        c.L.prm.acc_limit = (int)std::max<long long>(1, std::min<long long>(0xffffffffll / (maxN * maxN), 1 << 30));
-        if (const char* e = getenv("PG_K1_ACC_LIMIT")) c.L.prm.acc_limit = std::max(1, atoi(e));   // test hook: force early flushes
-        c.L.prm.bytes = (maxN <= 255 && !getenv("PG_K1_NO_BYTES")) ? 1 : 0;
-        c.L.prm.lanepop = c.lanepop ? 1 : 0;
-    }
     // The packed pass streams only the varied rows when enough sites are uniform (uniform_prepare); PG_K1_NO_UNIFORM keeps
     // every row streamed, for the tests that compare the two.
     const bool uni = c.packed && ctx->d_site_cls && !getenv("PG_K1_NO_UNIFORM");
-    if (c.packed) uni_geometry(c);
-    if (uni) PG_TRY(uniform_prepare(ctx, c));
-    c.uni_last = uni && c.us.in_use;
-    if (c.uni_last) PG_TRY(uniform_slots(ctx, c, Q));
-    PG_TRY(arm_slots(ctx, c, c.uni_last ? c.utotal_slots : -1));
-    if (c.uni_last) {
-        // Tiles of at most R varied rows and Tmax sites, a stage sized for such a tile: at 70 % uniform sites it is less than
-        // half a fixed tile's bytes, so the ring has more stages than teams and a team's next tile is in flight while it works
-        // on this one.  Its CTAs own the stream's tile ranges and add into the stream's slots.
-        K1Launch UL = c.L;
-        UL.plan = c.uplan;
-        UL.plan.T = c.uTmax;
-        UL.plan.num_tiles = c.us.nt;
-        UL.plan.ctas = (int)c.us.bound.size() - 1;
-        UL.plan.tile_bytes = c.ubytes;
-        UL.plan.stages = c.ustages;
-        UL.plan.smem_bytes = UL.plan.stages * UL.plan.tile_bytes + 256 + c.utable;
-        UL.prm.T = c.uTmax;
-        UL.prm.num_tiles = c.us.nt;
-        UL.prm.stages = UL.plan.stages;
-        UL.prm.tile_bytes = UL.plan.tile_bytes;
-        UL.prm.row_cap = c.uR;
-        UL.prm.cta_seg_first = c.u_cta_seg_first;
-        UL.prm.cta_slot_off = c.u_cta_slot_off;
-        UL.prm.geno = (const uint8_t*)c.us.rows.p;
-        UL.prm.row0 = (const int64_t*)c.us.row0.p;
-        UL.prm.site_lo = (const int64_t*)c.us.site_lo.p;
-        UL.prm.codes = (const uint16_t*)c.us.codes.p;
-        UL.prm.code_pitch = c.us.code_pitch;
+    if (c.packed) uni_geometry(u);
+    if (uni) PG_TRY(uniform_prepare(ctx, u));
+    u.last = uni && u.us.in_use;
+    if (u.last) PG_TRY(uniform_slots(ctx, u, c.L, Q));
+    K1Launch& L = u.last ? u.L : c.L;
+    {
+        long long maxN = 1;
+        for (int X = 0; X < Pp; ++X) maxN = std::max<long long>(maxN, c.pt.popN[X]);
+        L.prm.acc_limit = (int)std::max<long long>(1, std::min<long long>(0xffffffffll / (maxN * maxN), 1 << 30));
+        if (const char* e = getenv("PG_K1_ACC_LIMIT")) L.prm.acc_limit = std::max(1, atoi(e));   // test hook: force early flushes
+        L.prm.bytes = byte_counts((int)maxN) ? 1 : 0;
+        L.prm.lanepop = c.lanepop ? 1 : 0;
         const char* gv = getenv("PG_K1_UNI_GV");           // test hook: lanes per varied row (1, 2, 4, ... 32)
-        UL.prm.uni_gv = gv && *gv ? atoi(gv) : 0;
-        PG_CHECK(UL.prm.uni_gv >= 0 && UL.prm.uni_gv <= 32 && (UL.prm.uni_gv & (UL.prm.uni_gv - 1)) == 0,
+        L.prm.uni_gv = u.last && gv && *gv ? atoi(gv) : 0;
+        PG_CHECK(L.prm.uni_gv >= 0 && L.prm.uni_gv <= 32 && (L.prm.uni_gv & (L.prm.uni_gv - 1)) == 0,
                  "PG_K1_UNI_GV must be a power of two up to 32");
-        if (!wf) {
-            if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 2, true>(ctx, UL, "k1_popgen")));
-            else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 4, true>(ctx, UL, "k1_popgen")));
-            else PG_TRY((launch_site_pass_packed<MODE_POPGEN, 8, true>(ctx, UL, "k1_popgen")));
-        } else {
-            if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 2, true>(ctx, UL, "k1_popgen")));
-            else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 4, true>(ctx, UL, "k1_popgen")));
-            else PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 8, true>(ctx, UL, "k1_popgen")));
-        }
-    } else if (c.packed) {
-        if (!wf) {
-            if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 2>(ctx, c.L, "k1_popgen")));
-            else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN, 4>(ctx, c.L, "k1_popgen")));
-            else PG_TRY((launch_site_pass_packed<MODE_POPGEN, 8>(ctx, c.L, "k1_popgen")));
-        } else {
-            if (Pp == 2) PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 2>(ctx, c.L, "k1_popgen")));
-            else if (Pp == 4) PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 4>(ctx, c.L, "k1_popgen")));
-            else PG_TRY((launch_site_pass_packed<MODE_POPGEN_FREQ, 8>(ctx, c.L, "k1_popgen")));
-        }
-    } else if (!wf) {
-        if (Pp == 2) PG_TRY((launch_site_pass<MODE_POPGEN, 2>(ctx, c.L, "k1_popgen")));
-        else if (Pp == 4) PG_TRY((launch_site_pass<MODE_POPGEN, 4>(ctx, c.L, "k1_popgen")));
-        else PG_TRY((launch_site_pass<MODE_POPGEN, 8>(ctx, c.L, "k1_popgen")));
-    } else {
-        if (Pp == 2) PG_TRY((launch_site_pass<MODE_POPGEN_FREQ, 2>(ctx, c.L, "k1_popgen")));
-        else if (Pp == 4) PG_TRY((launch_site_pass<MODE_POPGEN_FREQ, 4>(ctx, c.L, "k1_popgen")));
-        else PG_TRY((launch_site_pass<MODE_POPGEN_FREQ, 8>(ctx, c.L, "k1_popgen")));
     }
+    PG_TRY(arm_slots(ctx, L, u.last ? u.us.rows.p : c.packed ? (const void*)ctx->d_packed : ctx->d_geno));
+    PG_TRY(with_popgen_mode(wf, Pp, [&](auto M, auto PP) {
+        constexpr int MODE = decltype(M)::value, PT = decltype(PP)::value;
+        if (u.last) return launch_site_pass_packed<MODE, PT, true>(ctx, L, "k1_popgen");
+        if (c.packed) return launch_site_pass_packed<MODE, PT, false>(ctx, L, "k1_popgen");
+        return launch_site_pass<MODE, PT>(ctx, L, "k1_popgen");
+    }));
 
     PG_TRY(ctx->out_i.ensure((size_t)W * 4 + 128));
     int* d_cnt = (int*)ctx->out_i.p;
     int32_t* d_path = (int32_t*)ctx->out_i.p + 16;
     PG_CUDA(cudaMemsetAsync(d_cnt, 0, 4, ctx->stream));
     FinParams fp;
-    fill_fin(fp, ctx, c, Q, Q);
-    if (c.uni_last) {
-        fp.cta_seg_first = c.u_cta_seg_first;
-        fp.cta_slot_off = c.u_cta_slot_off;
-        fp.seg_cta_lo = c.u_seg_cta_lo;
-        fp.seg_cta_hi = c.u_seg_cta_hi;
-    }
+    fill_fin(fp, ctx, c, L.slots, Q, Q);
     fp.P = P;
     fp.Ppad = Pp;
     fp.min_sites = min_sites;
@@ -2489,10 +2578,7 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     fp.RC = RC;
     fp.path = d_path;
     fp.n_pairwise = d_cnt;
-    const int ti = pg_time_begin(ctx, "k1_finalize");
-    k1_finalize<MODE_POPGEN><<<(unsigned)std::min<int64_t>(W, 65535), 64, 0, ctx->stream>>>(fp);
-    pg_time_end(ctx, ti);
-    PG_CUDA(cudaGetLastError());
+    PG_TRY(launch_finalize<MODE_POPGEN>(ctx, fp));
     void* hp = nullptr;
     PG_TRY(pg_pinned(ctx, (size_t)W * 4 + 256, &hp));
     int* h_cnt = (int*)hp;
@@ -2505,9 +2591,9 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
 extern "C" int pg_debug_uniform(pg_ctx* ctx, int32_t* in_use, int64_t* varied_sites) {
     PG_CHECK(ctx && in_use && varied_sites, "pg_debug_uniform: null argument");
     const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
-    const bool read = c && c->uni_last;
+    const bool read = c && c->up.last;
     *in_use = read ? 1 : 0;
-    *varied_sites = (c && c->us.gen == ctx->data_gen) ? c->us.varied : ctx->S;
+    *varied_sites = (c && c->up.us.gen == ctx->data_gen) ? c->up.us.varied : ctx->S;
     return PG_OK;
 }
 
@@ -2515,18 +2601,18 @@ extern "C" int pg_debug_uniform_tile(pg_ctx* ctx, int32_t* out) {
     PG_CHECK(ctx && out, "pg_debug_uniform_tile: null argument");
     const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
     const bool planned = c && c->valid && c->packed;
-    out[0] = planned ? c->uTmax : 0;
-    out[1] = planned ? c->uplan.wpt : 0;
+    out[0] = planned ? c->up.Tmax : 0;
+    out[1] = planned ? c->up.plan.wpt : 0;
     return PG_OK;
 }
 
 extern "C" int pg_debug_uniform_ring(pg_ctx* ctx, int32_t* out) {
     PG_CHECK(ctx && out, "pg_debug_uniform_ring: null argument");
     const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
-    const bool read = c && c->uni_last;
-    out[0] = read ? c->uR : 0;
-    out[1] = read ? c->ustages : 0;
-    out[2] = read ? c->ubytes : 0;
+    const bool read = c && c->up.last;
+    out[0] = read ? c->up.R : 0;
+    out[1] = read ? c->up.stages : 0;
+    out[2] = read ? c->up.stage_bytes : 0;
     return PG_OK;
 }
 
@@ -2534,16 +2620,17 @@ extern "C" int pg_debug_uniform_tiles(pg_ctx* ctx, int64_t cap, int64_t* site_lo
                                       int32_t* geometry) {
     PG_CHECK(ctx && ntiles && geometry, "pg_debug_uniform_tiles: null argument");
     const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
-    const bool read = c && c->uni_last;
-    *ntiles = read ? c->us.nt : 0;
-    geometry[0] = read ? c->uR : 0;
-    geometry[1] = read ? c->uTmax : 0;
-    if (!read || cap < c->us.nt + 1) return PG_OK;
+    const bool read = c && c->up.last;
+    const UniformStream* us = read ? &c->up.us : nullptr;
+    *ntiles = read ? us->nt : 0;
+    geometry[0] = read ? c->up.R : 0;
+    geometry[1] = read ? c->up.Tmax : 0;
+    if (!read || cap < us->nt + 1) return PG_OK;
     PG_CHECK(site_lo && row0, "pg_debug_uniform_tiles: null table");
     PG_CUDA(cudaSetDevice(ctx->device));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    PG_CUDA(cudaMemcpy(site_lo, c->us.site_lo.p, (size_t)(c->us.nt + 1) * 8, cudaMemcpyDeviceToHost));
-    PG_CUDA(cudaMemcpy(row0, c->us.row0.p, (size_t)(c->us.nt + 1) * 8, cudaMemcpyDeviceToHost));
+    PG_CUDA(cudaMemcpy(site_lo, us->site_lo.p, (size_t)(us->nt + 1) * 8, cudaMemcpyDeviceToHost));
+    PG_CUDA(cudaMemcpy(row0, us->row0.p, (size_t)(us->nt + 1) * 8, cudaMemcpyDeviceToHost));
     return PG_OK;
 }
 
@@ -2662,88 +2749,17 @@ extern "C" int pg_popgen_freqstats(pg_ctx* ctx, double* l, double* S, double* th
 // Enqueue site pass + finalize of the ABBA-BABA statistics on the ctx stream; records [W x 8] 8-byte words
 // [sites, pos_sum, ABBA, BABA, D, fd, fdM, sitesUsed] are left in the DEVICE buffer d_rec.  No synchronisation.
 int pg_abba_enqueue(pg_ctx* ctx, const int* sel, double min_data, void* d_rec) {
-    PG_CHECK(ctx->P >= 1, "pg_abbababa: call pg_set_pops first");
-    for (int k = 0; k < 4; ++k) {
-        PG_CHECK(sel[k] >= 0 && sel[k] < ctx->P, "pg_abbababa: population index %d out of range", sel[k]);
-        for (int j = 0; j < k; ++j) PG_CHECK(sel[j] != sel[k], "pg_abbababa: populations must be distinct");
-    }
-    PG_CUDA(cudaSetDevice(ctx->device));
-    pg_timings_reset(ctx);
-    const int64_t W = ctx->W;
-    if (W == 0) return PG_OK;
-    const int Q = 9, RC = 8;
-    if (ctx->S == 0) {
-        std::vector<unsigned long long> h((size_t)W * RC, 0ull);
-        const double qn = NAN;
-        unsigned long long nanbits;
-        memcpy(&nanbits, &qn, 8);
-        for (int64_t w = 0; w < W; ++w)
-            for (int k = 2; k < RC; ++k) h[(size_t)w * RC + k] = nanbits;
-        PG_CUDA(cudaMemcpyAsync(d_rec, h.data(), h.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-        PG_CUDA(cudaStreamSynchronize(ctx->stream));
-        return PG_OK;
-    }
-    K1Cache& c = *cache_of(ctx, 1);
-    if (!c.valid || c.epoch != ctx->epoch || memcmp(c.sel, sel, 4 * sizeof(int)) != 0) {
-        c.valid = false;
-        std::vector<int32_t> local(ctx->H, -1);
-        for (int h = 0; h < ctx->H; ++h)
-            for (int k = 0; k < 4; ++k)
-                if (ctx->hap_pop[h] == sel[k]) local[h] = k;
-        PG_TRY(prepare_windowed(ctx, c, local, 4, Q, k1_nw_for(ctx->pitch)));
-        for (int k = 0; k < 4; ++k) PG_CHECK(c.pt.popN[k] >= 1, "pg_abbababa: population %d has no haplotypes", sel[k]);
-        memcpy(c.sel, sel, 4 * sizeof(int));
-        c.epoch = ctx->epoch;
-        c.valid = true;
-    }
-    for (int k = 0; k < 4; ++k) {
-        // smallest n with (double)n / N >= minData  (genomics.py:1657-1660, exact in integers)
-        int thr = c.pt.popN[k] + 1;
-        for (int n = 0; n <= c.pt.popN[k]; ++n)
-            if ((double)n * 1.0 / (double)c.pt.popN[k] >= min_data) {
-                thr = n;
-                break;
-            }
-        c.L.prm.thr[k] = thr;
-    }
-    PG_TRY(arm_slots(ctx, c));
-    PG_TRY((launch_site_pass<MODE_ABBA, 4>(ctx, c.L, "k1_abba")));
-    FinParams fp;
-    fill_fin(fp, ctx, c, Q, 3);
-    fp.P = 4;
-    fp.Ppad = 4;
-    fp.rec = (unsigned long long*)d_rec;
-    fp.RC = RC;
-    const int ti = pg_time_begin(ctx, "k1_finalize");
-    k1_finalize<MODE_ABBA><<<(unsigned)std::min<int64_t>(W, 65535), 64, 0, ctx->stream>>>(fp);
-    pg_time_end(ctx, ti);
-    PG_CUDA(cudaGetLastError());
-    return PG_OK;
+    return fourpop_enqueue<MODE_ABBA>(ctx, "pg_abbababa", 1, 9, 8, 8, sel, min_data, 0, d_rec, [&](const K1Launch& L) {
+        return launch_site_pass<MODE_ABBA, 4>(ctx, L, "k1_abba");
+    });
 }
 
 extern "C" int pg_abbababa(pg_ctx* ctx, int32_t p1, int32_t p2, int32_t p3, int32_t o, double min_data, double* out,
                            double* sites_used, int64_t* n_sites, int64_t* pos_sum) {
     PG_CHECK(ctx && out && sites_used && n_sites && pos_sum, "pg_abbababa: null argument");
     const int sel[4] = {p1, p2, p3, o};
-    const int RC = 8;
-    const int64_t W = ctx->W;
-    PG_CUDA(cudaSetDevice(ctx->device));
-    PG_TRY(ctx->out_d.ensure((size_t)std::max<int64_t>(W, 1) * RC * 8 + 64));
-    PG_TRY(pg_abba_enqueue(ctx, sel, min_data, ctx->out_d.p));
-    if (W == 0) return PG_OK;
-    void* hp = nullptr;
-    PG_TRY(pg_pinned(ctx, (size_t)W * RC * 8 + 64, &hp));
-    const unsigned long long* hrec = (const unsigned long long*)hp;
-    PG_CUDA(cudaMemcpyAsync(hp, ctx->out_d.p, (size_t)W * RC * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    for (int64_t w = 0; w < W; ++w) {
-        const unsigned long long* r = hrec + (size_t)w * RC;
-        n_sites[w] = (int64_t)r[0];
-        pos_sum[w] = (int64_t)r[1];
-        memcpy(out + (size_t)w * 5, r + 2, 40);
-        memcpy(sites_used + w, r + 7, 8);
-    }
-    return PG_OK;
+    return fourpop_read(ctx, 8, [&](void* d_rec) { return pg_abba_enqueue(ctx, sel, min_data, d_rec); }, out, sites_used,
+                        n_sites, pos_sum);
 }
 
 // ================================================================================================
@@ -2752,90 +2768,20 @@ extern "C" int pg_abbababa(pg_ctx* ctx, int32_t p1, int32_t p2, int32_t p3, int3
 // Enqueue site pass + finalize of genomics.fourPop; records [W x 17] words [sites, pos_sum, 14 statistics, sitesUsed]
 // are left in the DEVICE buffer d_rec.  No synchronisation.
 int pg_fourpop_enqueue(pg_ctx* ctx, const int* sel, double min_data, int mode, void* d_rec) {
-    PG_CHECK(ctx->P >= 1, "pg_fourpop: call pg_set_pops first");
     PG_CHECK(mode >= 0 && mode <= 2, "pg_fourpop: mode must be 0 (default), 1 (polarize) or 2 (fixed)");
-    for (int k = 0; k < 4; ++k) {
-        PG_CHECK(sel[k] >= 0 && sel[k] < ctx->P, "pg_fourpop: population index %d out of range", sel[k]);
-        for (int j = 0; j < k; ++j) PG_CHECK(sel[j] != sel[k], "pg_fourpop: populations must be distinct");
-    }
-    PG_CUDA(cudaSetDevice(ctx->device));
-    pg_timings_reset(ctx);
-    const int64_t W = ctx->W;
-    if (W == 0) return PG_OK;
-    const int Q = 19, RC = 17;
-    if (ctx->S == 0) {
-        std::vector<unsigned long long> h((size_t)W * RC, 0ull);       // sites, pos_sum, sitesUsed = 0.0
-        const double qn = NAN;
-        unsigned long long nanbits;
-        memcpy(&nanbits, &qn, 8);
-        for (int64_t w = 0; w < W; ++w)
-            for (int k = 2; k < 16; ++k) h[(size_t)w * RC + k] = nanbits;
-        PG_CUDA(cudaMemcpyAsync(d_rec, h.data(), h.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-        PG_CUDA(cudaStreamSynchronize(ctx->stream));
-        return PG_OK;
-    }
-    K1Cache& c = *cache_of(ctx, 2);
-    if (!c.valid || c.epoch != ctx->epoch || memcmp(c.sel, sel, 4 * sizeof(int)) != 0) {
-        c.valid = false;
-        std::vector<int32_t> local(ctx->H, -1);
-        for (int h = 0; h < ctx->H; ++h)
-            for (int k = 0; k < 4; ++k)
-                if (ctx->hap_pop[h] == sel[k]) local[h] = k;
-        PG_TRY(prepare_windowed(ctx, c, local, 4, Q, k1_nw_for(ctx->pitch)));
-        for (int k = 0; k < 4; ++k) PG_CHECK(c.pt.popN[k] >= 1, "pg_fourpop: population %d has no haplotypes", sel[k]);
-        memcpy(c.sel, sel, 4 * sizeof(int));
-        c.epoch = ctx->epoch;
-        c.valid = true;
-    }
-    for (int k = 0; k < 4; ++k) {
-        int thr = c.pt.popN[k] + 1;       // smallest n with (double)n / N >= minData (genomics.py:1597-1600)
-        for (int n = 0; n <= c.pt.popN[k]; ++n)
-            if ((double)n * 1.0 / (double)c.pt.popN[k] >= min_data) {
-                thr = n;
-                break;
-            }
-        c.L.prm.thr[k] = thr;
-    }
-    c.L.prm.variant = mode;
-    PG_TRY(arm_slots(ctx, c));
-    if (getenv("PG_K1_FOURPOP_QUEUE")) PG_TRY((launch_site_pass<MODE_FOURPOP_Q, 4>(ctx, c.L, "k1_fourpop")));
-    else PG_TRY((launch_site_pass<MODE_FOURPOP, 4>(ctx, c.L, "k1_fourpop")));
-    FinParams fp;
-    fill_fin(fp, ctx, c, Q, 3);
-    fp.P = 4;
-    fp.Ppad = 4;
-    fp.rec = (unsigned long long*)d_rec;
-    fp.RC = RC;
-    const int ti = pg_time_begin(ctx, "k1_finalize");
-    k1_finalize<MODE_FOURPOP><<<(unsigned)std::min<int64_t>(W, 65535), 64, 0, ctx->stream>>>(fp);
-    pg_time_end(ctx, ti);
-    PG_CUDA(cudaGetLastError());
-    return PG_OK;
+    // sitesUsed of a record without sites is 0.0, not NaN
+    return fourpop_enqueue<MODE_FOURPOP>(ctx, "pg_fourpop", 2, 19, 17, 16, sel, min_data, mode, d_rec, [&](const K1Launch& L) {
+        if (getenv("PG_K1_FOURPOP_QUEUE")) return launch_site_pass<MODE_FOURPOP_Q, 4>(ctx, L, "k1_fourpop");
+        return launch_site_pass<MODE_FOURPOP, 4>(ctx, L, "k1_fourpop");
+    });
 }
 
 extern "C" int pg_fourpop(pg_ctx* ctx, int32_t p1, int32_t p2, int32_t p3, int32_t p4, double min_data, int32_t mode,
                           double* out, double* sites_used, int64_t* n_sites, int64_t* pos_sum) {
     PG_CHECK(ctx && out && sites_used && n_sites && pos_sum, "pg_fourpop: null argument");
     const int sel[4] = {p1, p2, p3, p4};
-    const int RC = 17;
-    const int64_t W = ctx->W;
-    PG_CUDA(cudaSetDevice(ctx->device));
-    PG_TRY(ctx->out_d.ensure((size_t)std::max<int64_t>(W, 1) * RC * 8 + 64));
-    PG_TRY(pg_fourpop_enqueue(ctx, sel, min_data, mode, ctx->out_d.p));
-    if (W == 0) return PG_OK;
-    void* hp = nullptr;
-    PG_TRY(pg_pinned(ctx, (size_t)W * RC * 8 + 64, &hp));
-    const unsigned long long* hrec = (const unsigned long long*)hp;
-    PG_CUDA(cudaMemcpyAsync(hp, ctx->out_d.p, (size_t)W * RC * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    for (int64_t w = 0; w < W; ++w) {
-        const unsigned long long* r = hrec + (size_t)w * RC;
-        n_sites[w] = (int64_t)r[0];
-        pos_sum[w] = (int64_t)r[1];
-        memcpy(out + (size_t)w * 14, r + 2, 14 * 8);
-        memcpy(sites_used + w, r + 16, 8);
-    }
-    return PG_OK;
+    return fourpop_read(ctx, 17, [&](void* d_rec) { return pg_fourpop_enqueue(ctx, sel, min_data, mode, d_rec); }, out,
+                        sites_used, n_sites, pos_sum);
 }
 
 // ================================================================================================
@@ -2899,57 +2845,31 @@ int site_counts_slab(pg_ctx* ctx, int64_t first, int64_t cnt) {
             if (ctx->hap_pop[h] >= p0 && ctx->hap_pop[h] < p0 + pc) local[h] = ctx->hap_pop[h] - p0;
         PopTables pt;
         build_tables(local, ctx->H, ctx->pitch / 16, Pp, pt);
-        const int n_ent = (int)pt.ent_chunk.size();
         const int table_bytes = table_bytes_of(pt);
         PG_CHECK(table_bytes <= 48 * 1024, "population layout needs too many mask entries");
         K1Launch L;
-        // long rows, a full group of 4 or 8 populations: one lane per population (counts fit 16 bits in any case)
-        bool lp = (Pp == 4 || Pp == 8) && Pp == pc && ctx->pitch >= 1024;
-        if (const char* e = getenv("PG_K1_LANEPOP")) lp = atoi(e) != 0 && (Pp == 4 || Pp == 8);
-        else if (lp) lp = lanepop_fits(cnt, ctx->H, ctx->sm_count, table_bytes, k1_env_nw12(), Pp);
-        const int nw = lp ? k1_env_nw12() : k1_nw_for(ctx->pitch);
-        L.plan = pg_make_k1_plan(cnt, ctx->H, ctx->sm_count, table_bytes, nw, lp ? Pp : 0);
+        // long rows, a full group of 4 or 8 populations: one lane per population
+        const WarpChoice wc = choose_warps(ctx, cnt, Pp, Pp == pc, table_bytes, true);
+        L.plan = pg_make_k1_plan(cnt, ctx->H, ctx->sm_count, table_bytes, wc.nw, wc.lanepop ? Pp : 0);
         PG_CHECK(L.plan.stages >= 2, "rows of %d haplotypes are too long for the site-pass kernel", ctx->H);
         PG_TRY(check_plan(L.plan));
-        PG_TRY(ctx->tables.ensure((size_t)n_ent * 20 + 4096));
+        PG_TRY(ctx->tables.ensure(pt.ent_chunk.size() * 20 + 4096));
         uint8_t* base = (uint8_t*)ctx->tables.p;
         size_t o = 0;
+        DevTables dt = {};
         uint32_t* d_mask_words = nullptr;
-        int32_t* d_chunk = nullptr;
         PG_TRY(push(ctx, base, o, pt.ent_mask.data(), pt.ent_mask.size(), &d_mask_words));
-        PG_TRY(push(ctx, base, o, pt.ent_chunk.data(), pt.ent_chunk.size(), &d_chunk));
+        dt.ent_mask = reinterpret_cast<uint4*>(d_mask_words);
+        PG_TRY(push(ctx, base, o, pt.ent_chunk.data(), pt.ent_chunk.size(), &dt.ent_chunk));
         K1Params& p = L.prm;
-        memset(&p, 0, sizeof(p));
-        p.geno = (const uint8_t*)ctx->d_geno;
-        p.pos = ctx->d_pos;
+        fill_params(p, ctx, L.plan, pt, dt, /*packed=*/false);
         p.site_begin = first;
         p.site_end = first + cnt;
-        p.num_tiles = L.plan.num_tiles;
-        p.pitch = L.plan.pitch;
-        p.G = L.plan.G;
-        p.I = L.plan.I;
-        p.T = L.plan.T;
-        p.wpt = L.plan.wpt;
-        p.nw = nw;
-        p.stages = L.plan.stages;
-        p.tile_bytes = L.plan.tile_bytes;
-        p.ent_chunk = d_chunk;
-        p.ent_mask = reinterpret_cast<uint4*>(d_mask_words);
-        p.n_ent = n_ent;
-        for (int X = 0; X < PG_MAX_K1_POPS; ++X) {
-            p.ent_lo[X] = pt.ent_lo[X];
-            p.ent_hi[X] = pt.ent_hi[X];
-            p.full_lo[X] = pt.full_lo[X];
-            p.full_hi[X] = pt.full_hi[X];
-            p.popN[X] = pt.popN[X];
-        }
         p.counts_out = (uint16_t*)ctx->misc.p + (size_t)p0 * 4;
         p.counts_stride = stride;
         p.counts_pops = pc;
-        p.lanepop = lp ? 1 : 0;
-        if (Pp == 2) PG_TRY((launch_site_pass<MODE_COUNTS, 2>(ctx, L, "k1_counts")));
-        else if (Pp == 4) PG_TRY((launch_site_pass<MODE_COUNTS, 4>(ctx, L, "k1_counts")));
-        else PG_TRY((launch_site_pass<MODE_COUNTS, 8>(ctx, L, "k1_counts")));
+        p.lanepop = wc.lanepop ? 1 : 0;
+        PG_TRY(with_pops(Pp, [&](auto PP) { return launch_site_pass<MODE_COUNTS, decltype(PP)::value>(ctx, L, "k1_counts"); }));
         // the table buffer (and the host vectors behind the async copies) are reused by the next group
         PG_CUDA(cudaStreamSynchronize(ctx->stream));
     }
