@@ -2072,16 +2072,10 @@ int arm_slots(pg_ctx* ctx, K1Launch& L, const void* rows) {
     return PG_OK;
 }
 
-// One site-pass kernel on the launch's grid, NW consumer warps and the producer warp per CTA.  The kernels take more dynamic
-// shared memory than the default limit, which needs an attribute: set once per kernel (the flags are the instantiation's) and
-// per device (the attribute is per device).
+// One site-pass kernel on the launch's grid, NW consumer warps and the producer warp per CTA.
 template <auto Kern, int NW>
 int launch_kernel(pg_ctx* ctx, const K1Launch& L, const char* name) {
-    static bool attr_set[64] = {};
-    if (!attr_set[ctx->device & 63]) {
-        PG_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set[ctx->device & 63] = true;
-    }
+    PG_TRY(pg_smem_limit<Kern>(ctx, 227 * 1024));
     const int ti = pg_time_begin(ctx, name);
     Kern<<<L.plan.ctas, (NW + 1) * 32, L.plan.smem_bytes, ctx->stream>>>(L.prm);
     pg_time_end(ctx, ti);

@@ -1,15 +1,22 @@
-// K2 — the pairwise path: per-window haplotype-pair matrices diff_ij / n_ij (integers) from bit-planes,
-// then the reference's mean-of-ratios epilogues.
-//
-//   k2_build_planes : int8 [S x pitch] -> 3 bit-planes per haplotype (allele bit0, allele bit1, valid),
-//                     haplotype-major, 32 sites per word           -- replaces Alignment.nanMask/numArray rows
-//   k2_pair         : diff_ij = popc(((b0_i^b0_j)|(b1_i^b1_j)) & m_i & m_j), n_ij = popc(m_i & m_j) summed over
-//                     the window's words; 64x64 haplotype tiles, 4x4 pairs per thread, cp.async ring
-//                     -- replaces distMatrix + pairNonNan (genomics.py:907-916, 1042-1047)
-//   k2_popgen_epi   : d_ij = diff/n, minSites mask, nanmean_min block means -> pi / dxy / Fst (genomics.py:956-995)
+// K2 — the pairwise path: per-window haplotype-pair matrices diff_ij / n_ij (integers), then the reference's
+// mean-of-ratios epilogues.  The matrices come from one of two sets of operand planes:
+//   - the tensor-core path (k2t.cu), the default: bit-packed planes and wgmma Gram kernels;
+//   - the POPC path (this file), where the tensor path's plane builders cannot take the width (pg_k2t_fits, about 4000
+//     haplotype columns) or PG_K2_POPC is set; the tests also compare the tensor path against it:
+//       k2_build_planes : int8 [S x pitch] -> 3 bit-planes per haplotype (allele bit0, allele bit1, valid),
+//                         haplotype-major, 32 sites per word           -- replaces Alignment.nanMask/numArray rows
+//       k2_hash_rows / k2_verify_rows : plane rows with identical valid planes share one mask row of n_ij
+//       k2_pair         : diff_ij = popc(((b0_i^b0_j)|(b1_i^b1_j)) & m_i & m_j), n_ij = popc(m_i & m_j) summed over
+//                         the window's words; 64x64 haplotype tiles, 4x4 pairs per thread, cp.async ring
+//                         -- replaces distMatrix + pairNonNan (genomics.py:907-916, 1042-1047)
+//       k2_het, k2_seq_nonnan : sampleHet / seqNonNan from the bit-planes
+//     These kernels are integer-issue bound (LOP3/POPC), not HBM bound (DESIGN.md §K2).
+// The epilogues here read the matrices of either path:
+//   k2_popgen_epi_* : d_ij = diff/n, minSites mask, nanmean_min block means -> pi / dxy / Fst (genomics.py:956-995)
 //   k2_ind_epi      : individual x individual nanmean of ploidy blocks (genomics.py:934-954)
-//
-// This path is integer-issue bound (LOP3/POPC), not HBM bound (DESIGN.md §K2).
+//   k2_hap_epi      : H12 / H2 clustering (genomics.py:1079-1098)
+//   k2_reduce_pairs, k2_ind_epi64 : --windType cat, chunk matrices summed as int64
+// The host half at the end of this file serves both paths: the entry points, their window batches and their scratch.
 #include <stdlib.h>
 
 #include <algorithm>
@@ -883,78 +890,74 @@ __global__ void __launch_bounds__(256) k2_ind_epi64(const __grid_constant__ IndE
 
 // ------------------------------------------------------------------------------------------------
 // host orchestration
+//
+// Scratch of one call.  Each buffer keeps what it holds until the call returns, except misc4:
+//   planes   the plane set: the POPC bit-planes and their mask tables (d_mid, d_rowmap), or the tensor path's valid plane,
+//            site scans and mask rows (k2t.cu)
+//   planes2  the tensor path's pseudo-site map and P / Q planes
+//   misc     the group starts (ind_start / pop_start); pg_k2_popgen_windows keeps the batch's window indices behind them
+//   misc2    the plane builders' column tables
+//   misc3    the batch's window bounds d_lo | d_hi (for_each_batch)
+//   misc4    short-lived scratch within one step: the POPC row hashes and their check, the Gram kernels' tile groups
+//   misc5    pg_k2_popgen_windows' block sums, pg_pairdist_cat's int64 accumulator
+//   pairs    the batch's pair matrices diff | n (run_pair_batch)
+//   out_d    the batch's output rows, copied back to the caller's arrays
+// pg_k2_popgen_windows never touches out_d or out_i: its caller keeps the record table and the path column there (k1.cu).
 // ------------------------------------------------------------------------------------------------
+
+// The operand planes of one site span: the tensor path's (k2t.cu) or the POPC kernels' three bit-planes.  The epilogues read
+// the same fields of both: Hk plane rows, Hm mask rows (n_ij is computed per mask row) and each plane row's mask row, on the
+// host (mid) and on the device (d_mid).  Every pointer stays valid until the call returns.
 struct PlaneSet {
     int Hk = 0;
+    int Hm = 0;
+    std::vector<int32_t> mid;
+    const int32_t* d_mid = nullptr;
+    bool tensor = false;
+    K2TPlanes t;                       // the tensor path's planes
+    // the POPC path's planes
     int64_t site_base = 0;
     int64_t NWp = 0;
-    uint32_t* planes = nullptr;
-    int Hm = 0;                        // unique valid-masks
-    std::vector<int32_t> mid;          // [Hk] mask id per row
-    const int32_t* d_mid = nullptr;    // device copy
-    const int32_t* d_rowmap = nullptr; // [Hm] mask id -> a representative plane row
-    bool tensor = false;               // planes of the tensor-core path (k2t.cu) instead of the three bit-planes
-    K2TPlanes t;
+    uint32_t* planes = nullptr;        // [3][Hk][NWp]: allele bit 0, allele bit 1, valid
+    const int32_t* d_rowmap = nullptr; // [Hm] mask row -> a representative plane row
 };
 
-// Build bit-planes for sites [lo, hi) of the haplotype columns listed in `order` (plane row r = column order[r]).
-int build_planes(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int64_t hi, PlaneSet& ps) {
+// The POPC bit-planes of sites [lo, hi), with the plane rows grouped by identical valid plane into mask rows.
+int build_popc_planes(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int64_t hi, PlaneSet& ps) {
     const int Hk = (int)order.size();
-    PG_CHECK(Hk >= 1, "pairwise path: no haplotypes selected");
-    // the plane builders of the tensor path stage 16 bytes per column in shared memory: beyond ~4000 haplotype columns the
-    // bit-plane POPC kernels (any width) take over
-    const bool fits = (size_t)16 * ctx->pitch + (size_t)((Hk + 15) / 16 * 16) * 8 <= 96 * 1024;
-    if (pg_k2_use_tensor() && fits) {
-        PG_TRY(pg_k2t_build(ctx, order, lo, hi, ps.t));
-        ps.tensor = true;
-        ps.Hk = Hk;
-        ps.site_base = ps.t.site_base;
-        ps.Hm = ps.t.Hm;                           // mask rows: one per row, or one per sample (see K2TPlanes)
-        ps.mid.resize(Hk);
-        for (int r = 0; r < Hk; ++r) ps.mid[r] = (ps.t.Hm == Hk) ? r : r / 2;
-        ps.d_mid = ps.t.d_mid;
-        return PG_OK;
-    }
     const int64_t sb = lo & ~(int64_t)(BP_SITES - 1);
     const int64_t nblk = (hi - sb + BP_SITES - 1) / BP_SITES;
     const int64_t NWp = nblk * 8 + KW + 8;     // zero tail: chunk over-reads contribute nothing
     const size_t bytes = (size_t)3 * Hk * NWp * 4;
-    PG_TRY(ctx->planes.ensure(bytes));
+    PG_TRY(ctx->planes.ensure(bytes + (size_t)Hk * 8));       // the planes, then the mask tables d_mid | d_rowmap
     PG_CUDA(cudaMemsetAsync(ctx->planes.p, 0, bytes, ctx->stream));
     std::vector<int32_t> c2r(ctx->pitch, -1);
     for (int r = 0; r < Hk; ++r) c2r[order[r]] = r;
     PG_TRY(ctx->misc2.ensure((size_t)ctx->pitch * 4 + 64));
     PG_CUDA(cudaMemcpyAsync(ctx->misc2.p, c2r.data(), (size_t)ctx->pitch * 4, cudaMemcpyHostToDevice, ctx->stream));
-    PG_CUDA(cudaFuncSetAttribute(k2_build_planes, cudaFuncAttributeMaxDynamicSharedMemorySize, BP_SMEM));
+    PG_TRY(pg_smem_limit<k2_build_planes>(ctx, BP_SMEM));
     const int colblocks = (ctx->pitch + BP_COLS - 1) / BP_COLS;
     for (int64_t y0 = 0; y0 < nblk; y0 += 65535) {
         const int64_t ny = std::min<int64_t>(65535, nblk - y0);
-        dim3 grid((unsigned)colblocks, (unsigned)ny);
-        const int ti = pg_time_begin(ctx, "k2_planes");
-        k2_build_planes<<<grid, 256, BP_SMEM, ctx->stream>>>((const uint8_t*)ctx->d_geno, ctx->pitch, ctx->S,
-                                                             sb + y0 * BP_SITES, (const int32_t*)ctx->misc2.p,
-                                                             (uint32_t*)ctx->planes.p + y0 * 8, Hk, NWp);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
+        PG_TRY(pg_timed(ctx, "k2_planes", [&] {
+            k2_build_planes<<<dim3((unsigned)colblocks, (unsigned)ny), 256, BP_SMEM, ctx->stream>>>(
+                (const uint8_t*)ctx->d_geno, ctx->pitch, ctx->S, sb + y0 * BP_SITES, (const int32_t*)ctx->misc2.p,
+                (uint32_t*)ctx->planes.p + y0 * 8, Hk, NWp);
+        }));
     }
     ps.Hk = Hk;
     ps.site_base = sb;
     ps.NWp = NWp;
     ps.planes = (uint32_t*)ctx->planes.p;
+    int32_t* d_mid = (int32_t*)(ps.planes + bytes / 4);
+    int32_t* d_rowmap = d_mid + Hk;
     // group rows by identical valid plane: hash, group on the host, verify on the device
-    PG_TRY(ctx->misc4.ensure((size_t)Hk * 8 + (size_t)Hk * 12 + 256));
+    PG_TRY(ctx->misc4.ensure((size_t)Hk * 12 + 256));
     unsigned long long* d_hash = (unsigned long long*)ctx->misc4.p;
     int32_t* d_rep = (int32_t*)(d_hash + Hk);
-    int32_t* d_mid = d_rep + Hk;
-    int32_t* d_rowmap = d_mid + Hk;
-    int* d_flag = (int*)(d_rowmap + Hk);
+    int* d_flag = (int*)(d_rep + Hk);
     const uint32_t* mplane = ps.planes + (size_t)2 * Hk * NWp;
-    {
-        const int ti = pg_time_begin(ctx, "k2_mask_groups");
-        k2_hash_rows<<<Hk, 256, 0, ctx->stream>>>(mplane, NWp, d_hash);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-    }
+    PG_TRY(pg_timed(ctx, "k2_mask_groups", [&] { k2_hash_rows<<<Hk, 256, 0, ctx->stream>>>(mplane, NWp, d_hash); }));
     std::vector<unsigned long long> hh(Hk);
     PG_CUDA(cudaMemcpyAsync(hh.data(), d_hash, (size_t)Hk * 8, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -979,12 +982,7 @@ int build_planes(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int
     }
     PG_CUDA(cudaMemcpyAsync(d_rep, rep.data(), (size_t)Hk * 4, cudaMemcpyHostToDevice, ctx->stream));
     PG_CUDA(cudaMemsetAsync(d_flag, 0, 4, ctx->stream));
-    {
-        const int ti = pg_time_begin(ctx, "k2_mask_groups");
-        k2_verify_rows<<<Hk, 256, 0, ctx->stream>>>(mplane, NWp, d_rep, d_flag);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-    }
+    PG_TRY(pg_timed(ctx, "k2_mask_groups", [&] { k2_verify_rows<<<Hk, 256, 0, ctx->stream>>>(mplane, NWp, d_rep, d_flag); }));
     int flag = 0;
     PG_CUDA(cudaMemcpyAsync(&flag, d_flag, 4, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1002,29 +1000,32 @@ int build_planes(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int
     return PG_OK;
 }
 
-size_t pair_budget_bytes() {
-    const char* e = getenv("PG_PAIR_SCRATCH_MB");
-    size_t mb = e ? (size_t)atoll(e) : 3072;
-    if (mb < 1) mb = 1;
-    return mb << 20;
+// Planes for sites [lo, hi) of the haplotype columns listed in `order` (plane row r = column order[r]): the tensor path's
+// unless PG_K2_POPC is set or its plane builders cannot take the width.
+int build_planes(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int64_t hi, PlaneSet& ps) {
+    const int Hk = (int)order.size();
+    PG_CHECK(Hk >= 1, "pairwise path: no haplotypes selected");
+    ps.tensor = pg_k2_use_tensor() && pg_k2t_fits(ctx->pitch, Hk);
+    if (!ps.tensor) return build_popc_planes(ctx, order, lo, hi, ps);
+    PG_TRY(pg_k2t_build(ctx, order, lo, hi, ps.t));
+    ps.Hk = Hk;
+    ps.Hm = ps.t.Hm;                           // mask rows: one per row, or one per sample (see K2TPlanes)
+    ps.mid.resize(Hk);
+    for (int r = 0; r < Hk; ++r) ps.mid[r] = (ps.t.Hm == Hk) ? r : r / 2;
+    ps.d_mid = ps.t.d_mid;
+    return PG_OK;
 }
 
-// Pair matrices for a batch of non-empty windows (absolute site ranges) -> ctx->pairs: diff [nb][Hk^2] | n [nb][Hm^2]
-int run_pair_batch(pg_ctx* ctx, const PlaneSet& ps, const std::vector<int64_t>& lo, const std::vector<int64_t>& hi,
-                   int32_t** d_diff, int32_t** d_n) {
-    const int nb = (int)lo.size();
+// Pair matrices of a batch of nb windows (site bounds on the device) -> ctx->pairs: diff [nb][Hk^2] | n [nb][Hm^2]
+int run_pair_batch(pg_ctx* ctx, const PlaneSet& ps, const int64_t* d_lo, const int64_t* d_hi, int nb, int32_t** d_diff,
+                   int32_t** d_n) {
     const size_t HH = (size_t)ps.Hk * ps.Hk, MM = (size_t)ps.Hm * ps.Hm;
     PG_TRY(ctx->pairs.ensure((size_t)nb * (HH + MM) * 4 + 64));
-    PG_TRY(ctx->misc3.ensure((size_t)nb * 16 + 64));
-    int64_t* d_lo = (int64_t*)ctx->misc3.p;
-    int64_t* d_hi = d_lo + nb;
-    PG_CUDA(cudaMemcpyAsync(d_lo, lo.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, ctx->stream));
-    PG_CUDA(cudaMemcpyAsync(d_hi, hi.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, ctx->stream));
-    if (ps.tensor) {
-        *d_diff = (int32_t*)ctx->pairs.p;
-        *d_n = (int32_t*)ctx->pairs.p + (size_t)nb * HH;
-        return pg_k2t_pairs(ctx, ps.t, d_lo, d_hi, nb, *d_diff, *d_n);
-    }
+    *d_diff = (int32_t*)ctx->pairs.p;
+    *d_n = *d_diff + (size_t)nb * HH;
+    if (ps.tensor) return pg_k2t_pairs(ctx, ps.t, d_lo, d_hi, nb, *d_diff, *d_n);
+    PG_TRY(pg_smem_limit<k2_pair<PAIR_DIFF>>(ctx, PairGeom<PAIR_DIFF>::SMEM));
+    PG_TRY(pg_smem_limit<k2_pair<PAIR_N>>(ctx, PairGeom<PAIR_N>::SMEM));
     PairParams pp;
     pp.planes = ps.planes;
     pp.Hk = ps.Hk;
@@ -1032,38 +1033,137 @@ int run_pair_batch(pg_ctx* ctx, const PlaneSet& ps, const std::vector<int64_t>& 
     pp.site_base = ps.site_base;
     pp.win_lo = d_lo;
     pp.win_hi = d_hi;
-    static bool attr_dev[64] = {};      // per device
-    if (!attr_dev[ctx->device & 63]) {
-        PG_CUDA(cudaFuncSetAttribute(k2_pair<PAIR_DIFF>, cudaFuncAttributeMaxDynamicSharedMemorySize, PairGeom<PAIR_DIFF>::SMEM));
-        PG_CUDA(cudaFuncSetAttribute(k2_pair<PAIR_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, PairGeom<PAIR_N>::SMEM));
-        attr_dev[ctx->device & 63] = true;
-    }
     // diff over all haplotype rows
     pp.n_rows = ps.Hk;
     pp.row_map = nullptr;
     pp.ntile = (ps.Hk + TS - 1) / TS;
-    pp.out = (int32_t*)ctx->pairs.p;
-    {
-        dim3 grid((unsigned)(pp.ntile * (pp.ntile + 1) / 2), (unsigned)nb);
-        const int ti = pg_time_begin(ctx, "k2_pair_diff");
-        k2_pair<PAIR_DIFF><<<grid, 256, PairGeom<PAIR_DIFF>::SMEM, ctx->stream>>>(pp);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-    }
-    *d_diff = pp.out;
+    pp.out = *d_diff;
+    PG_TRY(pg_timed(ctx, "k2_pair_diff", [&] {
+        k2_pair<PAIR_DIFF><<<dim3((unsigned)(pp.ntile * (pp.ntile + 1) / 2), (unsigned)nb), 256, PairGeom<PAIR_DIFF>::SMEM,
+                             ctx->stream>>>(pp);
+    }));
     // n over the unique valid-masks
     pp.n_rows = ps.Hm;
     pp.row_map = ps.d_rowmap;
     pp.ntile = (ps.Hm + TS - 1) / TS;
-    pp.out = (int32_t*)ctx->pairs.p + (size_t)nb * HH;
-    {
-        dim3 grid((unsigned)(pp.ntile * (pp.ntile + 1) / 2), (unsigned)nb);
-        const int ti = pg_time_begin(ctx, "k2_pair_n");
-        k2_pair<PAIR_N><<<grid, 256, PairGeom<PAIR_N>::SMEM, ctx->stream>>>(pp);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
+    pp.out = *d_n;
+    return pg_timed(ctx, "k2_pair_n", [&] {
+        k2_pair<PAIR_N><<<dim3((unsigned)(pp.ntile * (pp.ntile + 1) / 2), (unsigned)nb), 256, PairGeom<PAIR_N>::SMEM,
+                          ctx->stream>>>(pp);
+    });
+}
+
+// Alignment.sampleHet() rows of a batch of nb windows: [nb][n_ind] doubles
+int run_het(pg_ctx* ctx, const PlaneSet& ps, const int64_t* d_lo, const int64_t* d_hi, int nb, const int32_t* d_ind_start,
+            int n_ind, int min_sites, double* d_out) {
+    if (ps.tensor) return pg_k2t_het(ctx, ps.t, d_lo, d_hi, nb, d_ind_start, n_ind, min_sites, d_out);
+    HetParams hp;
+    hp.planes = ps.planes;
+    hp.Hk = ps.Hk;
+    hp.NWp = ps.NWp;
+    hp.site_base = ps.site_base;
+    hp.win_lo = d_lo;
+    hp.win_hi = d_hi;
+    hp.ind_start = d_ind_start;
+    hp.n_ind = n_ind;
+    hp.min_sites = min_sites;
+    hp.out = d_out;
+    return pg_timed(ctx, "k2_het", [&] { k2_het<<<dim3((unsigned)n_ind, (unsigned)nb), 128, 0, ctx->stream>>>(hp); });
+}
+
+// non-missing sites of every plane row in a batch of nb windows: [nb][Hk] int64
+int run_seq_nonnan(pg_ctx* ctx, const PlaneSet& ps, const int64_t* d_lo, const int64_t* d_hi, int nb, long long* d_out) {
+    if (ps.tensor) return pg_k2t_seq_nonnan(ctx, ps.t, d_lo, d_hi, nb, d_out);
+    return pg_timed(ctx, "k2_seq_nonnan", [&] {
+        k2_seq_nonnan<<<dim3((unsigned)ps.Hk, (unsigned)nb), 128, 0, ctx->stream>>>(ps.planes + (size_t)2 * ps.Hk * ps.NWp,
+                                                                                   ps.NWp, ps.site_base, d_lo, d_hi, ps.Hk,
+                                                                                   d_out);
+    });
+}
+
+// Plane rows ordered by group: the haplotypes of group 0, then of group 1, ... (each in upload order); a haplotype of group
+// -1 gets no row.  start[g] = first row of group g, start[G] = rows.  `what` names a caller's map in the range check's
+// message; nullptr for ctx->hap_pop, which pg_set_pops checks.
+int group_rows(const pg_ctx* ctx, const int32_t* group, int G, const char* what, std::vector<int32_t>& order,
+               std::vector<int32_t>& start) {
+    for (int h = 0; what && h < ctx->H; ++h)
+        PG_CHECK(group[h] >= -1 && group[h] < G, "%s[%d]=%d out of range", what, h, group[h]);
+    start.assign(G + 1, 0);
+    for (int g = 0; g < G; ++g) {
+        start[g] = (int32_t)order.size();
+        for (int h = 0; h < ctx->H; ++h)
+            if (group[h] == g) order.push_back(h);
     }
-    *d_n = pp.out;
+    start[G] = (int32_t)order.size();
+    return PG_OK;
+}
+
+// every haplotype, in upload order
+std::vector<int32_t> all_rows(int H) {
+    std::vector<int32_t> order(H);
+    for (int h = 0; h < H; ++h) order[h] = h;
+    return order;
+}
+
+// non-empty windows and the site span they cover
+void nonempty_windows(const pg_ctx* ctx, std::vector<int64_t>& idx, int64_t& lo, int64_t& hi) {
+    lo = ctx->S;
+    hi = 0;
+    for (int64_t w = 0; w < ctx->W; ++w)
+        if (ctx->win_hi[w] > ctx->win_lo[w]) {
+            idx.push_back(w);
+            lo = std::min(lo, ctx->win_lo[w]);
+            hi = std::max(hi, ctx->win_hi[w]);
+        }
+}
+
+// Windows per batch of a caller of the pair matrices: a batch's diff and n (8 bytes per plane-row pair) and `extra` bytes
+// per window fit PG_PAIR_SCRATCH_MB (default 3 GiB), and a batch is one grid dimension (at most 65535).
+size_t pair_batch_size(int Hk, size_t extra) {
+    const char* e = getenv("PG_PAIR_SCRATCH_MB");
+    size_t mb = e ? (size_t)atoll(e) : 3072;
+    if (mb < 1) mb = 1;
+    return std::max<size_t>(1, std::min<size_t>((mb << 20) / ((size_t)Hk * Hk * 8 + extra), 65535));
+}
+
+// Cuts the windows `wins` (window w spans sites [lo[w], hi[w])) into batches of at most per_batch, uploads each batch's bounds
+// and runs body(b0, nb, d_lo, d_hi) on windows wins[b0 .. b0 + nb).
+template <class Body>
+int for_each_batch(pg_ctx* ctx, const std::vector<int64_t>& wins, const int64_t* lo, const int64_t* hi, size_t per_batch,
+                   Body&& body) {
+    for (size_t b0 = 0; b0 < wins.size(); b0 += per_batch) {
+        const size_t nb = std::min(per_batch, wins.size() - b0);
+        std::vector<int64_t> blo(nb), bhi(nb);
+        for (size_t k = 0; k < nb; ++k) {
+            blo[k] = lo[wins[b0 + k]];
+            bhi[k] = hi[wins[b0 + k]];
+        }
+        PG_TRY(ctx->misc3.ensure(nb * 16 + 64));
+        int64_t* d_lo = (int64_t*)ctx->misc3.p;
+        int64_t* d_hi = d_lo + nb;
+        PG_CUDA(cudaMemcpyAsync(d_lo, blo.data(), nb * 8, cudaMemcpyHostToDevice, ctx->stream));
+        PG_CUDA(cudaMemcpyAsync(d_hi, bhi.data(), nb * 8, cudaMemcpyHostToDevice, ctx->stream));
+        PG_TRY(body(b0, nb, (const int64_t*)d_lo, (const int64_t*)d_hi));
+    }
+    return PG_OK;
+}
+
+// Copies batch rows 0 .. nb (row_bytes each) of a device buffer to the rows of windows wins[b0 .. b0 + nb) of a host array,
+// one copy per run of consecutive windows, then synchronises.  staged: through pg_d2h_staged, for large rows into pageable
+// memory.
+int copy_rows_back(pg_ctx* ctx, const std::vector<int64_t>& wins, size_t b0, size_t nb, const void* d_src, void* h_dst,
+                   size_t row_bytes, bool staged = false) {
+    size_t k = 0;
+    while (k < nb) {
+        size_t e = k + 1;
+        while (e < nb && wins[b0 + e] == wins[b0 + e - 1] + 1) ++e;
+        uint8_t* dst = (uint8_t*)h_dst + (size_t)wins[b0 + k] * row_bytes;
+        const uint8_t* src = (const uint8_t*)d_src + k * row_bytes;
+        if (staged) PG_TRY(pg_d2h_staged(ctx, dst, src, (e - k) * row_bytes));
+        else PG_CUDA(cudaMemcpyAsync(dst, src, (e - k) * row_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        k = e;
+    }
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));
     return PG_OK;
 }
 
@@ -1075,15 +1175,8 @@ int run_pair_batch(pg_ctx* ctx, const PlaneSet& ps, const std::vector<int64_t>& 
 int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, const int64_t* win_lo, const int64_t* win_hi,
                          int32_t min_sites, double min_data, void* d_rec, int RC) {
     const int P = ctx->P;
-    // plane rows: haplotypes that belong to a population, sorted by population (stable)
-    std::vector<int32_t> order;
-    std::vector<int32_t> pop_start(P + 1, 0);
-    for (int X = 0; X < P; ++X) {
-        pop_start[X] = (int32_t)order.size();
-        for (int h = 0; h < ctx->H; ++h)
-            if (ctx->hap_pop[h] == X) order.push_back(h);
-    }
-    pop_start[P] = (int32_t)order.size();
+    std::vector<int32_t> order, pop_start;
+    PG_TRY(group_rows(ctx, ctx->hap_pop.data(), P, nullptr, order, pop_start));
     // empty windows cannot be "ragged"; every window here has at least one site
     int64_t lo = ctx->S, hi = 0;
     for (int64_t w : wins) {
@@ -1092,20 +1185,13 @@ int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, const in
     }
     PlaneSet ps;
     PG_TRY(build_planes(ctx, order, lo, hi, ps));
-    const size_t HH = (size_t)ps.Hk * ps.Hk;
-    const size_t per_batch = std::max<size_t>(1, std::min<size_t>(pair_budget_bytes() / (HH * 8), 65535));
+    const size_t per_batch = pair_batch_size(ps.Hk, 0);
     PG_TRY(ctx->misc.ensure((size_t)(P + 1) * 4 + per_batch * 8 + 128));
     PG_CUDA(cudaMemcpyAsync(ctx->misc.p, pop_start.data(), (size_t)(P + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
     int64_t* d_widx = reinterpret_cast<int64_t*>((uint8_t*)ctx->misc.p + (((size_t)(P + 1) * 4 + 63) / 64) * 64);
-    for (size_t b0 = 0; b0 < wins.size(); b0 += per_batch) {
-        const size_t nb = std::min(per_batch, wins.size() - b0);
-        std::vector<int64_t> blo(nb), bhi(nb);
-        for (size_t k = 0; k < nb; ++k) {
-            blo[k] = win_lo[wins[b0 + k]];
-            bhi[k] = win_hi[wins[b0 + k]];
-        }
+    return for_each_batch(ctx, wins, win_lo, win_hi, per_batch, [&](size_t b0, size_t nb, const int64_t* d_lo, const int64_t* d_hi) {
         int32_t *d_diff = nullptr, *d_n = nullptr;
-        PG_TRY(run_pair_batch(ctx, ps, blo, bhi, &d_diff, &d_n));
+        PG_TRY(run_pair_batch(ctx, ps, d_lo, d_hi, (int)nb, &d_diff, &d_n));
         PG_CUDA(cudaMemcpyAsync(d_widx, wins.data() + b0, nb * 8, cudaMemcpyHostToDevice, ctx->stream));
         PopEpiParams ep;
         ep.diff = d_diff;
@@ -1127,19 +1213,18 @@ int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, const in
         // sample-pair walk: mask ids are r >> 1 (the tensor path's per-sample n rows) and populations start on even rows
         bool by_pairs = ps.tensor && ps.Hm * 2 == ps.Hk && (size_t)nblk * 64 <= 48 * 1024;
         for (int X = 0; X <= P; ++X) by_pairs = by_pairs && (pop_start[X] % 2 == 0);
-        // the timing label names the stage-1 kernel, so that a caller can tell which epilogue ran
-        const int ti = pg_time_begin(ctx, by_pairs ? "k2_popgen_epi_pairs" : "k2_popgen_epi_blocks");
         // one CTA per window when there are many windows, else the blocks of a window over several CTAs (~8 CTAs per SM)
         const unsigned nsplit = (unsigned)std::max<int64_t>(1, std::min<int64_t>(nblk, (8 * (int64_t)ctx->sm_count + (int64_t)nb - 1) / (int64_t)nb));
-        if (by_pairs) k2_popgen_epi_pairs<<<dim3((unsigned)nb, nsplit), 128, (size_t)nblk * 64, ctx->stream>>>(ep);
-        else k2_popgen_epi_blocks<<<dim3((unsigned)nblk, (unsigned)nb), 256, 0, ctx->stream>>>(ep);
-        k2_popgen_epi_final<<<(unsigned)((nb + 127) / 128), 128, 0, ctx->stream>>>(ep, (int)nb);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
+        // the timing label names the stage-1 kernel, so that a caller can tell which epilogue ran
+        PG_TRY(pg_timed(ctx, by_pairs ? "k2_popgen_epi_pairs" : "k2_popgen_epi_blocks", [&] {
+            if (by_pairs) k2_popgen_epi_pairs<<<dim3((unsigned)nb, nsplit), 128, (size_t)nblk * 64, ctx->stream>>>(ep);
+            else k2_popgen_epi_blocks<<<dim3((unsigned)nblk, (unsigned)nb), 256, 0, ctx->stream>>>(ep);
+            k2_popgen_epi_final<<<(unsigned)((nb + 127) / 128), 128, 0, ctx->stream>>>(ep, (int)nb);
+        }));
         ctx->launches += 1;
         PG_CUDA(cudaStreamSynchronize(ctx->stream));     // host vectors and scratch are reused by the next batch
-    }
-    return PG_OK;
+        return PG_OK;
+    });
 }
 
 extern "C" int pg_pairdist(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_ind, int32_t include_same_with_same,
@@ -1151,30 +1236,19 @@ extern "C" int pg_pairdist(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_ind, i
     pg_timings_reset(ctx);
     const int64_t W = ctx->W;
     if (W == 0) return PG_OK;
-    std::vector<int32_t> order, ind_start(n_ind + 1, 0);
-    for (int h = 0; h < ctx->H; ++h)
-        PG_CHECK(hap_ind[h] >= -1 && hap_ind[h] < n_ind, "pg_pairdist: hap_ind[%d]=%d out of range", h, hap_ind[h]);
-    for (int a = 0; a < n_ind; ++a) {
-        ind_start[a] = (int32_t)order.size();
-        for (int h = 0; h < ctx->H; ++h)
-            if (hap_ind[h] == a) order.push_back(h);
-    }
-    ind_start[n_ind] = (int32_t)order.size();
+    std::vector<int32_t> order, ind_start;
+    PG_TRY(group_rows(ctx, hap_ind, n_ind, "pg_pairdist: hap_ind", order, ind_start));
     const size_t nn = (size_t)n_ind * n_ind;
-    // sites / position sums on the host side of the library: prefix sums of the positions are cheap, but the
-    // positions live on the device — read them back once (4 bytes per site).
-    std::vector<int64_t> nonempty;
-    int64_t lo = ctx->S, hi = 0;
+    std::vector<int64_t> wins;
+    int64_t lo, hi;
+    nonempty_windows(ctx, wins, lo, hi);
     for (int64_t w = 0; w < W; ++w) {
         if (n_sites) n_sites[w] = ctx->win_hi[w] - ctx->win_lo[w];
-        if (ctx->win_hi[w] > ctx->win_lo[w]) {
-            nonempty.push_back(w);
-            lo = std::min(lo, ctx->win_lo[w]);
-            hi = std::max(hi, ctx->win_hi[w]);
-        } else {
+        if (ctx->win_hi[w] <= ctx->win_lo[w])
             for (size_t k = 0; k < nn; ++k) dist[(size_t)w * nn + k] = NAN;
-        }
     }
+    // sites / position sums on the host side of the library: prefix sums of the positions are cheap, but the
+    // positions live on the device — read them back once (4 bytes per site).
     if (pos_sum) {
         std::vector<int32_t> hp((size_t)std::max<int64_t>(ctx->S, 1));
         if (ctx->S > 0)
@@ -1183,23 +1257,17 @@ extern "C" int pg_pairdist(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_ind, i
         for (int64_t s = 0; s < ctx->S; ++s) pre[s + 1] = pre[s] + hp[s];
         for (int64_t w = 0; w < W; ++w) pos_sum[w] = pre[ctx->win_hi[w]] - pre[ctx->win_lo[w]];
     }
-    if (nonempty.empty()) return PG_OK;
+    if (wins.empty()) return PG_OK;
     PlaneSet ps;
     PG_TRY(build_planes(ctx, order, lo, hi, ps));
-    const size_t HH = (size_t)ps.Hk * ps.Hk;
-    const size_t per_batch = std::max<size_t>(1, std::min<size_t>(pair_budget_bytes() / (HH * 8 + nn * 8), 65535));
+    const size_t per_batch = pair_batch_size(ps.Hk, nn * 8);
     PG_TRY(ctx->misc.ensure((size_t)(n_ind + 1) * 4 + 64));
     PG_CUDA(cudaMemcpyAsync(ctx->misc.p, ind_start.data(), (size_t)(n_ind + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
     PG_TRY(ctx->out_d.ensure(per_batch * nn * 8 + 64));
-    for (size_t b0 = 0; b0 < nonempty.size(); b0 += per_batch) {
-        const size_t nb = std::min(per_batch, nonempty.size() - b0);
-        std::vector<int64_t> blo(nb), bhi(nb);
-        for (size_t k = 0; k < nb; ++k) {
-            blo[k] = ctx->win_lo[nonempty[b0 + k]];
-            bhi[k] = ctx->win_hi[nonempty[b0 + k]];
-        }
+    return for_each_batch(ctx, wins, ctx->win_lo.data(), ctx->win_hi.data(), per_batch,
+                          [&](size_t b0, size_t nb, const int64_t* d_lo, const int64_t* d_hi) {
         int32_t *d_diff = nullptr, *d_n = nullptr;
-        PG_TRY(run_pair_batch(ctx, ps, blo, bhi, &d_diff, &d_n));
+        PG_TRY(run_pair_batch(ctx, ps, d_lo, d_hi, (int)nb, &d_diff, &d_n));
         IndEpiParams ep;
         ep.diff = d_diff;
         ep.n = d_n;
@@ -1211,22 +1279,12 @@ extern "C" int pg_pairdist(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_ind, i
         ep.include_same = include_same_with_same ? 1 : 0;
         ep.min_sites = min_sites;
         ep.out = (double*)ctx->out_d.p;
-        dim3 grid((unsigned)std::min<int>((n_ind + 7) / 8, 64), (unsigned)nb);
-        const int ti = pg_time_begin(ctx, "k2_ind_epi");
-        k2_ind_epi<<<grid, 256, 0, ctx->stream>>>(ep);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-        // consecutive non-empty windows are usually consecutive in `dist`: copy run by run
-        size_t k = 0;
-        while (k < nb) {
-            size_t e = k + 1;
-            while (e < nb && nonempty[b0 + e] == nonempty[b0 + e - 1] + 1) ++e;
-            PG_TRY(pg_d2h_staged(ctx, dist + (size_t)nonempty[b0 + k] * nn, (double*)ctx->out_d.p + k * nn, (e - k) * nn * 8));
-            k = e;
-        }
-        PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    }
-    return PG_OK;
+        PG_TRY(pg_timed(ctx, "k2_ind_epi", [&] {
+            k2_ind_epi<<<dim3((unsigned)std::min<int>((n_ind + 7) / 8, 64), (unsigned)nb), 256, 0, ctx->stream>>>(ep);
+        }));
+        // n_ind^2 doubles per window, possibly into pageable memory: staged copies
+        return copy_rows_back(ctx, wins, b0, nb, ctx->out_d.p, dist, nn * 8, true);
+    });
 }
 
 extern "C" int pg_pair_counts(pg_ctx* ctx, int64_t window, int32_t* diff, int32_t* n) {
@@ -1242,13 +1300,13 @@ extern "C" int pg_pair_counts(pg_ctx* ctx, int64_t window, int32_t* diff, int32_
         memset(n, 0, HH * 4);
         return PG_OK;
     }
-    std::vector<int32_t> order(H);
-    for (int h = 0; h < H; ++h) order[h] = h;
     PlaneSet ps;
-    PG_TRY(build_planes(ctx, order, lo, hi, ps));
-    std::vector<int64_t> blo(1, lo), bhi(1, hi);
+    PG_TRY(build_planes(ctx, all_rows(H), lo, hi, ps));
     int32_t *d_diff = nullptr, *d_n = nullptr;
-    PG_TRY(run_pair_batch(ctx, ps, blo, bhi, &d_diff, &d_n));
+    PG_TRY(for_each_batch(ctx, std::vector<int64_t>(1, window), ctx->win_lo.data(), ctx->win_hi.data(), 1,
+                          [&](size_t, size_t, const int64_t* d_lo, const int64_t* d_hi) {
+        return run_pair_batch(ctx, ps, d_lo, d_hi, 1, &d_diff, &d_n);
+    }));
     std::vector<int32_t> nu((size_t)ps.Hm * ps.Hm);
     PG_CUDA(cudaMemcpyAsync(diff, d_diff, HH * 4, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaMemcpyAsync(nu.data(), d_n, nu.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1262,35 +1320,6 @@ extern "C" int pg_pair_counts(pg_ctx* ctx, int64_t window, int32_t* diff, int32_
     return PG_OK;
 }
 
-namespace {
-// non-empty windows and the site span they cover
-void nonempty_windows(const pg_ctx* ctx, std::vector<int64_t>& idx, int64_t& lo, int64_t& hi) {
-    lo = ctx->S;
-    hi = 0;
-    for (int64_t w = 0; w < ctx->W; ++w)
-        if (ctx->win_hi[w] > ctx->win_lo[w]) {
-            idx.push_back(w);
-            lo = std::min(lo, ctx->win_lo[w]);
-            hi = std::max(hi, ctx->win_hi[w]);
-        }
-}
-
-// scatter batch rows (row_doubles each) of a device buffer to the windows' rows of a host array
-int copy_rows_back(pg_ctx* ctx, const std::vector<int64_t>& wins, size_t b0, size_t nb, const double* d_src,
-                   double* h_dst, size_t row_doubles) {
-    size_t k = 0;
-    while (k < nb) {
-        size_t e = k + 1;
-        while (e < nb && wins[b0 + e] == wins[b0 + e - 1] + 1) ++e;
-        PG_CUDA(cudaMemcpyAsync(h_dst + (size_t)wins[b0 + k] * row_doubles, d_src + k * row_doubles,
-                                (e - k) * row_doubles * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        k = e;
-    }
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    return PG_OK;
-}
-}  // namespace
-
 // Alignment.sampleHet() (genomics.py:918-929) for every window: het [W x n_ind]
 extern "C" int pg_ind_het(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_ind, int32_t min_sites, double* het) {
     PG_CHECK(ctx && hap_ind && het, "pg_ind_het: null argument");
@@ -1300,15 +1329,8 @@ extern "C" int pg_ind_het(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_ind, in
     pg_timings_reset(ctx);
     const int64_t W = ctx->W;
     if (W == 0) return PG_OK;
-    std::vector<int32_t> order, ind_start(n_ind + 1, 0);
-    for (int h = 0; h < ctx->H; ++h)
-        PG_CHECK(hap_ind[h] >= -1 && hap_ind[h] < n_ind, "pg_ind_het: hap_ind[%d]=%d out of range", h, hap_ind[h]);
-    for (int a = 0; a < n_ind; ++a) {
-        ind_start[a] = (int32_t)order.size();
-        for (int h = 0; h < ctx->H; ++h)
-            if (hap_ind[h] == a) order.push_back(h);
-    }
-    ind_start[n_ind] = (int32_t)order.size();
+    std::vector<int32_t> order, ind_start;
+    PG_TRY(group_rows(ctx, hap_ind, n_ind, "pg_ind_het: hap_ind", order, ind_start));
     for (size_t k = 0; k < (size_t)W * n_ind; ++k) het[k] = NAN;
     std::vector<int64_t> wins;
     int64_t lo, hi;
@@ -1316,45 +1338,14 @@ extern "C" int pg_ind_het(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_ind, in
     if (wins.empty() || order.empty()) return PG_OK;
     PlaneSet ps;
     PG_TRY(build_planes(ctx, order, lo, hi, ps));
-    const size_t per_batch = 65535;
     PG_TRY(ctx->misc.ensure((size_t)(n_ind + 1) * 4 + 64));
     PG_CUDA(cudaMemcpyAsync(ctx->misc.p, ind_start.data(), (size_t)(n_ind + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-    for (size_t b0 = 0; b0 < wins.size(); b0 += per_batch) {
-        const size_t nb = std::min(per_batch, wins.size() - b0);
-        std::vector<int64_t> blo(nb), bhi(nb);
-        for (size_t k = 0; k < nb; ++k) {
-            blo[k] = ctx->win_lo[wins[b0 + k]];
-            bhi[k] = ctx->win_hi[wins[b0 + k]];
-        }
-        PG_TRY(ctx->misc3.ensure(nb * 16 + 64));
+    return for_each_batch(ctx, wins, ctx->win_lo.data(), ctx->win_hi.data(), 65535,
+                          [&](size_t b0, size_t nb, const int64_t* d_lo, const int64_t* d_hi) {
         PG_TRY(ctx->out_d.ensure(nb * (size_t)n_ind * 8 + 64));
-        int64_t* d_lo = (int64_t*)ctx->misc3.p;
-        int64_t* d_hi = d_lo + nb;
-        PG_CUDA(cudaMemcpyAsync(d_lo, blo.data(), nb * 8, cudaMemcpyHostToDevice, ctx->stream));
-        PG_CUDA(cudaMemcpyAsync(d_hi, bhi.data(), nb * 8, cudaMemcpyHostToDevice, ctx->stream));
-        if (ps.tensor) {
-            PG_TRY(pg_k2t_het(ctx, ps.t, d_lo, d_hi, (int)nb, (const int32_t*)ctx->misc.p, n_ind, min_sites, (double*)ctx->out_d.p));
-            PG_TRY(copy_rows_back(ctx, wins, b0, nb, (const double*)ctx->out_d.p, het, (size_t)n_ind));
-            continue;
-        }
-        HetParams hp;
-        hp.planes = ps.planes;
-        hp.Hk = ps.Hk;
-        hp.NWp = ps.NWp;
-        hp.site_base = ps.site_base;
-        hp.win_lo = d_lo;
-        hp.win_hi = d_hi;
-        hp.ind_start = (const int32_t*)ctx->misc.p;
-        hp.n_ind = n_ind;
-        hp.min_sites = min_sites;
-        hp.out = (double*)ctx->out_d.p;
-        const int ti = pg_time_begin(ctx, "k2_het");
-        k2_het<<<dim3((unsigned)n_ind, (unsigned)nb), 128, 0, ctx->stream>>>(hp);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-        PG_TRY(copy_rows_back(ctx, wins, b0, nb, (const double*)ctx->out_d.p, het, (size_t)n_ind));
-    }
-    return PG_OK;
+        PG_TRY(run_het(ctx, ps, d_lo, d_hi, (int)nb, (const int32_t*)ctx->misc.p, n_ind, min_sites, (double*)ctx->out_d.p));
+        return copy_rows_back(ctx, wins, b0, nb, ctx->out_d.p, het, (size_t)n_ind * 8);
+    });
 }
 
 // Alignment.H12stats(maxDist) (genomics.py:1079-1098) for every window and population of pg_set_pops:
@@ -1370,17 +1361,13 @@ extern "C" int pg_hapstats(pg_ctx* ctx, double max_dist, int32_t min_sites, int3
     const int64_t W = ctx->W;
     const int P = ctx->P;
     if (W == 0) return PG_OK;
-    std::vector<int32_t> order;
-    std::vector<int32_t> pop_start(P + 1, 0);
+    std::vector<int32_t> order, pop_start;
+    PG_TRY(group_rows(ctx, ctx->hap_pop.data(), P, nullptr, order, pop_start));
     int maxN = 0;
     for (int X = 0; X < P; ++X) {
-        pop_start[X] = (int32_t)order.size();
-        for (int h = 0; h < ctx->H; ++h)
-            if (ctx->hap_pop[h] == X) order.push_back(h);
-        maxN = std::max(maxN, (int)order.size() - pop_start[X]);
-        PG_CHECK((int)order.size() > pop_start[X], "pg_hapstats: population %d has no haplotypes", X);
+        PG_CHECK(pop_start[X + 1] > pop_start[X], "pg_hapstats: population %d has no haplotypes", X);
+        maxN = std::max(maxN, pop_start[X + 1] - pop_start[X]);
     }
-    pop_start[P] = (int32_t)order.size();
     const size_t smem = (size_t)maxN * ((maxN + 31) / 32) * 4 + (size_t)((maxN + 31) / 32) * 4 + (size_t)maxN * 4 + 64;
     PG_CHECK(smem <= 200 * 1024, "pg_hapstats: a population of %d haplotypes is too large for the clustering kernel", maxN);
     for (size_t k = 0; k < (size_t)W * P * 3; ++k) out[k] = NAN;
@@ -1390,20 +1377,14 @@ extern "C" int pg_hapstats(pg_ctx* ctx, double max_dist, int32_t min_sites, int3
     if (wins.empty()) return PG_OK;
     PlaneSet ps;
     PG_TRY(build_planes(ctx, order, lo, hi, ps));
-    const size_t HH = (size_t)ps.Hk * ps.Hk;
-    const size_t per_batch = std::max<size_t>(1, std::min<size_t>(pair_budget_bytes() / (HH * 8), 65535));
     PG_TRY(ctx->misc.ensure((size_t)(P + 1) * 4 + 64));
     PG_CUDA(cudaMemcpyAsync(ctx->misc.p, pop_start.data(), (size_t)(P + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+    // the shared memory of k2_hap_epi follows the largest population: set on every call
     PG_CUDA(cudaFuncSetAttribute(k2_hap_epi, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    for (size_t b0 = 0; b0 < wins.size(); b0 += per_batch) {
-        const size_t nb = std::min(per_batch, wins.size() - b0);
-        std::vector<int64_t> blo(nb), bhi(nb);
-        for (size_t k = 0; k < nb; ++k) {
-            blo[k] = ctx->win_lo[wins[b0 + k]];
-            bhi[k] = ctx->win_hi[wins[b0 + k]];
-        }
+    return for_each_batch(ctx, wins, ctx->win_lo.data(), ctx->win_hi.data(), pair_batch_size(ps.Hk, 0),
+                          [&](size_t b0, size_t nb, const int64_t* d_lo, const int64_t* d_hi) {
         int32_t *d_diff = nullptr, *d_n = nullptr;
-        PG_TRY(run_pair_batch(ctx, ps, blo, bhi, &d_diff, &d_n));
+        PG_TRY(run_pair_batch(ctx, ps, d_lo, d_hi, (int)nb, &d_diff, &d_n));
         PG_TRY(ctx->out_d.ensure(nb * (size_t)P * 24 + 64));
         HapEpiParams ep;
         ep.diff = d_diff;
@@ -1417,13 +1398,11 @@ extern "C" int pg_hapstats(pg_ctx* ctx, double max_dist, int32_t min_sites, int3
         ep.diag_nan = diag_nan ? 1 : 0;
         ep.max_dist = max_dist;
         ep.out = (double*)ctx->out_d.p;
-        const int ti = pg_time_begin(ctx, "k2_hap_epi");
-        k2_hap_epi<<<dim3((unsigned)P, (unsigned)nb), 256, smem, ctx->stream>>>(ep);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-        PG_TRY(copy_rows_back(ctx, wins, b0, nb, (const double*)ctx->out_d.p, out, (size_t)P * 3));
-    }
-    return PG_OK;
+        PG_TRY(pg_timed(ctx, "k2_hap_epi", [&] {
+            k2_hap_epi<<<dim3((unsigned)P, (unsigned)nb), 256, smem, ctx->stream>>>(ep);
+        }));
+        return copy_rows_back(ctx, wins, b0, nb, ctx->out_d.p, out, (size_t)P * 24);
+    });
 }
 
 // distMat.py --windType cat (distMat.py:303-314: parseGenoFile -> ONE window over every site): dist [n_ind x n_ind].
@@ -1437,15 +1416,8 @@ extern "C" int pg_pairdist_cat(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_in
     PG_CHECK(ctx->H > 0, "pg_pairdist_cat: upload genotypes first");
     PG_CUDA(cudaSetDevice(ctx->device));
     pg_timings_reset(ctx);
-    std::vector<int32_t> order, ind_start(n_ind + 1, 0);
-    for (int h = 0; h < ctx->H; ++h)
-        PG_CHECK(hap_ind[h] >= -1 && hap_ind[h] < n_ind, "pg_pairdist_cat: hap_ind[%d]=%d out of range", h, hap_ind[h]);
-    for (int a = 0; a < n_ind; ++a) {
-        ind_start[a] = (int32_t)order.size();
-        for (int h = 0; h < ctx->H; ++h)
-            if (hap_ind[h] == a) order.push_back(h);
-    }
-    ind_start[n_ind] = (int32_t)order.size();
+    std::vector<int32_t> order, ind_start;
+    PG_TRY(group_rows(ctx, hap_ind, n_ind, "pg_pairdist_cat: hap_ind", order, ind_start));
     const int Hk = (int)order.size();
     PG_CHECK(Hk >= 1, "pg_pairdist_cat: no haplotypes selected");
     const size_t HH = (size_t)Hk * Hk;
@@ -1461,24 +1433,23 @@ extern "C" int pg_pairdist_cat(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_in
         PlaneSet ps;
         PG_TRY(build_planes(ctx, order, 0, ctx->S, ps));
         const int64_t CH = 32768;                                  // sites per chunk (1024 plane words)
-        const int64_t nchunks = (ctx->S + CH - 1) / CH;
-        const size_t per_batch = std::max<size_t>(1, std::min<size_t>(pair_budget_bytes() / (HH * 8), 65535));
-        for (int64_t c0 = 0; c0 < nchunks; c0 += (int64_t)per_batch) {
-            const size_t nb = (size_t)std::min<int64_t>((int64_t)per_batch, nchunks - c0);
-            std::vector<int64_t> blo(nb), bhi(nb);
-            for (size_t k = 0; k < nb; ++k) {
-                blo[k] = (c0 + (int64_t)k) * CH;
-                bhi[k] = std::min<int64_t>(blo[k] + CH, ctx->S);
-            }
-            int32_t *d_diff = nullptr, *d_n = nullptr;
-            PG_TRY(run_pair_batch(ctx, ps, blo, bhi, &d_diff, &d_n));
-            const int ti = pg_time_begin(ctx, "k2_reduce_pairs");
-            k2_reduce_pairs<<<(unsigned)std::min<size_t>((HH + 255) / 256, 4096), 256, 0, ctx->stream>>>(d_diff, d_n, ps.d_mid, Hk,
-                                                                                                       ps.Hm, (int)nb, d_acc);
-            pg_time_end(ctx, ti);
-            PG_CUDA(cudaGetLastError());
-            PG_CUDA(cudaStreamSynchronize(ctx->stream));           // host vectors / scratch are reused by the next batch
+        std::vector<int64_t> chunks, clo, chi;
+        for (int64_t c = 0; c * CH < ctx->S; ++c) {
+            chunks.push_back(c);
+            clo.push_back(c * CH);
+            chi.push_back(std::min<int64_t>(c * CH + CH, ctx->S));
         }
+        PG_TRY(for_each_batch(ctx, chunks, clo.data(), chi.data(), pair_batch_size(Hk, 0),
+                              [&](size_t, size_t nb, const int64_t* d_lo, const int64_t* d_hi) {
+            int32_t *d_diff = nullptr, *d_n = nullptr;
+            PG_TRY(run_pair_batch(ctx, ps, d_lo, d_hi, (int)nb, &d_diff, &d_n));
+            PG_TRY(pg_timed(ctx, "k2_reduce_pairs", [&] {
+                k2_reduce_pairs<<<(unsigned)std::min<size_t>((HH + 255) / 256, 4096), 256, 0, ctx->stream>>>(
+                    d_diff, d_n, ps.d_mid, Hk, ps.Hm, (int)nb, d_acc);
+            }));
+            PG_CUDA(cudaStreamSynchronize(ctx->stream));           // host vectors / scratch are reused by the next batch
+            return PG_OK;
+        }));
     }
     if (ctx->nccl_comm && ctx->nccl_ranks > 1) PG_TRY(pg_nccl_allreduce_i64(ctx, d_acc, 2 * HH + 1));
     PG_TRY(ctx->misc.ensure((size_t)(n_ind + 1) * 4 + 64));
@@ -1491,10 +1462,9 @@ extern "C" int pg_pairdist_cat(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_in
     ep.ind_start = (const int32_t*)ctx->misc.p;
     ep.include_same = include_same_with_same ? 1 : 0;
     ep.out = (double*)ctx->out_d.p;
-    const int ti = pg_time_begin(ctx, "k2_ind_epi");
-    k2_ind_epi64<<<(unsigned)std::min<size_t>((nn + 255) / 256, 1024), 256, 0, ctx->stream>>>(ep);
-    pg_time_end(ctx, ti);
-    PG_CUDA(cudaGetLastError());
+    PG_TRY(pg_timed(ctx, "k2_ind_epi", [&] {
+        k2_ind_epi64<<<(unsigned)std::min<size_t>((nn + 255) / 256, 1024), 256, 0, ctx->stream>>>(ep);
+    }));
     long long tot = 0;
     PG_CUDA(cudaMemcpyAsync(dist, ctx->out_d.p, nn * 8, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaMemcpyAsync(&tot, d_acc + 2 * HH, 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1517,36 +1487,12 @@ extern "C" int pg_seq_nonnan(pg_ctx* ctx, int64_t* out) {
     int64_t lo, hi;
     nonempty_windows(ctx, wins, lo, hi);
     if (wins.empty()) return PG_OK;
-    std::vector<int32_t> order(H);
-    for (int h = 0; h < H; ++h) order[h] = h;
     PlaneSet ps;
-    PG_TRY(build_planes(ctx, order, lo, hi, ps));
-    const size_t per_batch = 65535;
-    for (size_t b0 = 0; b0 < wins.size(); b0 += per_batch) {
-        const size_t nb = std::min(per_batch, wins.size() - b0);
-        std::vector<int64_t> blo(nb), bhi(nb);
-        for (size_t k = 0; k < nb; ++k) {
-            blo[k] = ctx->win_lo[wins[b0 + k]];
-            bhi[k] = ctx->win_hi[wins[b0 + k]];
-        }
-        PG_TRY(ctx->misc3.ensure(nb * 16 + 64));
+    PG_TRY(build_planes(ctx, all_rows(H), lo, hi, ps));
+    return for_each_batch(ctx, wins, ctx->win_lo.data(), ctx->win_hi.data(), 65535,
+                          [&](size_t b0, size_t nb, const int64_t* d_lo, const int64_t* d_hi) {
         PG_TRY(ctx->out_d.ensure(nb * (size_t)H * 8 + 64));
-        int64_t* d_lo = (int64_t*)ctx->misc3.p;
-        int64_t* d_hi = d_lo + nb;
-        PG_CUDA(cudaMemcpyAsync(d_lo, blo.data(), nb * 8, cudaMemcpyHostToDevice, ctx->stream));
-        PG_CUDA(cudaMemcpyAsync(d_hi, bhi.data(), nb * 8, cudaMemcpyHostToDevice, ctx->stream));
-        if (ps.tensor) {
-            PG_TRY(pg_k2t_seq_nonnan(ctx, ps.t, d_lo, d_hi, (int)nb, (long long*)ctx->out_d.p));
-            PG_TRY(copy_rows_back(ctx, wins, b0, nb, (const double*)ctx->out_d.p, (double*)out, (size_t)H));
-            continue;
-        }
-        const int ti = pg_time_begin(ctx, "k2_seq_nonnan");
-        k2_seq_nonnan<<<dim3((unsigned)H, (unsigned)nb), 128, 0, ctx->stream>>>(ps.planes + (size_t)2 * ps.Hk * ps.NWp, ps.NWp,
-                                                                               ps.site_base, d_lo, d_hi, H,
-                                                                               (long long*)ctx->out_d.p);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-        PG_TRY(copy_rows_back(ctx, wins, b0, nb, (const double*)ctx->out_d.p, (double*)out, (size_t)H));
-    }
-    return PG_OK;
+        PG_TRY(run_seq_nonnan(ctx, ps, d_lo, d_hi, (int)nb, (long long*)ctx->out_d.p));
+        return copy_rows_back(ctx, wins, b0, nb, ctx->out_d.p, out, (size_t)H * 8);
+    });
 }

@@ -845,30 +845,22 @@ int pg_k2t_build(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int
     const int64_t nchunk = (hi - sb + 63) / 64;
     PG_CHECK(nchunk * 64 < (int64_t)1 << 31, "pairwise path: site span too large for one call");
     const int pitch = ctx->pitch, pw = pitch / 4;
-    PG_CHECK((size_t)16 * pw * 4 + (size_t)R * 8 <= 96 * 1024, "pairwise path: %d haplotype columns are too many for the plane builders", pitch);
-    {
-        static bool attr_dev[64] = {};
-        if (!attr_dev[ctx->device & 63]) {
-            PG_CUDA(cudaFuncSetAttribute(k2t_build_pq, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-            PG_CUDA(cudaFuncSetAttribute(k2t_valid_class<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-            PG_CUDA(cudaFuncSetAttribute(k2t_valid_class<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-            attr_dev[ctx->device & 63] = true;
-        }
-    }
+    PG_CHECK(pg_k2t_fits(pitch, Hk), "pairwise path: %d haplotype columns are too many for the plane builders", pitch);
+    PG_TRY(pg_smem_limit<k2t_build_pq>(ctx, 96 * 1024));
+    PG_TRY(pg_smem_limit<k2t_valid_class<true>>(ctx, 96 * 1024));
+    PG_TRY(pg_smem_limit<k2t_valid_class<false>>(ctx, 96 * 1024));
     // column tables
     std::vector<int32_t> c2r(pitch, -1);
     for (int r = 0; r < Hk; ++r) c2r[order[r]] = r;
     std::vector<uint32_t> cmask(pw, 0u);
     for (int c = 0; c < pitch; ++c)
         if (c2r[c] >= 0) cmask[c / 4] |= 0xffu << (8 * (c % 4));
-    PG_TRY(ctx->misc2.ensure((size_t)pitch * 4 + (size_t)pw * 4 + (size_t)Hk * 4 + 256));
+    PG_TRY(ctx->misc2.ensure((size_t)pitch * 4 + (size_t)pw * 4 + 256));
     int32_t* d_c2r = (int32_t*)ctx->misc2.p;
     uint32_t* d_cmask = (uint32_t*)(d_c2r + pitch);
-    int32_t* d_iota = (int32_t*)(d_cmask + pw);
     PG_CUDA(cudaMemcpyAsync(d_c2r, c2r.data(), (size_t)pitch * 4, cudaMemcpyHostToDevice, ctx->stream));
     PG_CUDA(cudaMemcpyAsync(d_cmask, cmask.data(), (size_t)pw * 4, cudaMemcpyHostToDevice, ctx->stream));
-    k2t_iota<<<(Hk + 255) / 256, 256, 0, ctx->stream>>>(d_iota, Hk);
-    // plane memory: vplane | cls | chunk_tot | chunk_off | cps
+    // plane memory: vplane | cls | chunk_tot | chunk_off | cps | vpair | mask rows (halves) | mask rows (identity)
     const size_t span = (size_t)nchunk * 64;
     size_t off = 0;
     auto carve = [&](size_t bytes) {
@@ -880,9 +872,12 @@ int pg_k2t_build(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int
     const int R2 = (Hk / 2 + 15) / 16 * 16;
     const size_t o_v = carve((size_t)nchunk * R * 8), o_cls = carve(span), o_tot = carve((size_t)nchunk * 4),
                  o_off = carve((size_t)(nchunk + 2) * 4), o_cps = carve((span + 1) * 4),
-                 o_vp = carve(want_pairs ? (size_t)nchunk * R2 * 8 : 0), o_mid = carve((size_t)Hk * 4);
+                 o_vp = carve(want_pairs ? (size_t)nchunk * R2 * 8 : 0), o_mid = carve((size_t)Hk * 4),
+                 o_iota = carve((size_t)Hk * 4);
     PG_TRY(ctx->planes.ensure(off));
     uint8_t* base = (uint8_t*)ctx->planes.p;
+    int32_t* d_iota = (int32_t*)(base + o_iota);
+    k2t_iota<<<(Hk + 255) / 256, 256, 0, ctx->stream>>>(d_iota, Hk);
     VcParams vp;
     vp.geno32 = (const uint32_t*)ctx->d_geno;
     vp.pw = pw;
@@ -904,21 +899,13 @@ int pg_k2t_build(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int
     vp.pair_flag = d_off + nchunk + 1;
     PG_CUDA(cudaMemsetAsync(vp.pair_flag, 0, 4, ctx->stream));
     const int grid1 = (int)std::min<int64_t>(nchunk, (int64_t)ctx->sm_count * 8);
-    {
-        const int ti = pg_time_begin(ctx, "k2t_valid_class");
-        bool all_used = true;                    // unselected real columns? (padding columns hold 0 = missing and never count)
-        for (int c = 0; c < ctx->H; ++c) all_used = all_used && c2r[c] >= 0;
+    bool all_used = true;                        // unselected real columns? (padding columns hold 0 = missing and never count)
+    for (int c = 0; c < ctx->H; ++c) all_used = all_used && c2r[c] >= 0;
+    PG_TRY(pg_timed(ctx, "k2t_valid_class", [&] {
         if (all_used) k2t_valid_class<true><<<grid1, 256, (size_t)8 * pw * 4 + (size_t)R * 8, ctx->stream>>>(vp);
         else k2t_valid_class<false><<<grid1, 256, (size_t)8 * pw * 4 + (size_t)R * 8, ctx->stream>>>(vp);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-    }
-    {
-        const int ti = pg_time_begin(ctx, "k2t_scan");
-        k2t_scan<<<1, 1024, 0, ctx->stream>>>(vp.chunk_tot, d_off, nchunk);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-    }
+    }));
+    PG_TRY(pg_timed(ctx, "k2t_scan", [&] { k2t_scan<<<1, 1024, 0, ctx->stream>>>(vp.chunk_tot, d_off, nchunk); }));
     int32_t tf[2] = {0, 0};                       // pseudo-sites, "some sample's haplotypes differ in missingness"
     PG_CUDA(cudaMemcpyAsync(tf, d_off + nchunk, 8, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -929,13 +916,10 @@ int pg_k2t_build(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int
     const size_t o_inv = carve((size_t)std::max<int64_t>(total, 1) * 8), o_pq = carve((size_t)std::max<int64_t>(nchunk_d, 1) * 2 * R * 8);
     PG_TRY(ctx->planes2.ensure(off));
     uint8_t* base2 = (uint8_t*)ctx->planes2.p;
-    {
-        const int ti = pg_time_begin(ctx, "k2t_inv");
-        const int gridi = (int)std::min<int64_t>((nchunk + 7) / 8, (int64_t)ctx->sm_count * 16);
+    const int gridi = (int)std::min<int64_t>((nchunk + 7) / 8, (int64_t)ctx->sm_count * 16);
+    PG_TRY(pg_timed(ctx, "k2t_inv", [&] {
         k2t_inv<<<gridi, 256, 0, ctx->stream>>>(vp.cls, d_off, nchunk, d_cps, (uint2*)(base2 + o_inv));
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
-    }
+    }));
     if (nchunk_d > 0) {
         PqParams pp;
         pp.geno32 = vp.geno32;
@@ -951,10 +935,7 @@ int pg_k2t_build(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int
         pp.Hk = Hk;
         const size_t smem = (size_t)16 * pw * 4;
         const int grid2 = (int)std::min<int64_t>(nchunk_d, (int64_t)ctx->sm_count * 8);
-        const int ti = pg_time_begin(ctx, "k2t_build_pq");
-        k2t_build_pq<<<grid2, 256, smem, ctx->stream>>>(pp);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
+        PG_TRY(pg_timed(ctx, "k2t_build_pq", [&] { k2t_build_pq<<<grid2, 256, smem, ctx->stream>>>(pp); }));
     }
     ps.Hk = Hk;
     ps.R = R;
@@ -964,7 +945,6 @@ int pg_k2t_build(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int
     ps.cps = d_cps;
     ps.npseudo = total;
     ps.pq = (uint64_t*)(base2 + o_pq);
-    ps.d_iota = d_iota;
     // mask ids for the epilogues: row r -> r / 2 when the valid words are shared by consecutive rows
     ps.Hm = pairs_ok ? Hk / 2 : Hk;
     ps.R2 = R2;
@@ -1005,20 +985,17 @@ void gram_groups(int R, std::vector<GramGroup>& groups, int& brows, int& a_sep) 
 int pg_k2t_pairs(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const int64_t* d_hi, int nb, int32_t* d_diff,
                  int32_t* d_n) {
     const int budget = 227 * 1024 - 1024;      // dynamic shared memory; the barriers are static
-    static bool attr_dev[64] = {};
-    if (!attr_dev[ctx->device & 63]) {
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, budget));
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, budget));
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, budget));
-        PG_CUDA(cudaFuncSetAttribute(k2t_gram<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, budget));
-        attr_dev[ctx->device & 63] = true;
-    }
+    PG_TRY((pg_smem_limit<k2t_gram<1, 1>>(ctx, budget)));
+    PG_TRY((pg_smem_limit<k2t_gram<1, 2>>(ctx, budget)));
+    PG_TRY((pg_smem_limit<k2t_gram<1, 4>>(ctx, budget)));
+    PG_TRY((pg_smem_limit<k2t_gram<2, 1>>(ctx, budget)));
     // n_ij over the mask rows (one per sample when the haplotypes of a sample share their missingness), diff_ij over all rows
     const int Rn = ps.vpair ? ps.R2 : ps.R;
     std::vector<GramGroup> gn, gd;
     int brows_n, asep_n, brows_d, asep_d;
     gram_groups(Rn, gn, brows_n, asep_n);
     gram_groups(ps.R, gd, brows_d, asep_d);
+    // the tile groups only live for this call's two launches (misc4 is short-lived scratch, see k2.cu)
     PG_TRY(ctx->misc4.ensure((gn.size() + gd.size()) * sizeof(GramGroup) + 64));
     GramGroup* d_gn = (GramGroup*)ctx->misc4.p;
     GramGroup* d_gd = d_gn + gn.size();
@@ -1063,12 +1040,11 @@ int pg_k2t_pairs(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const in
         gp.cps = nullptr;
         gp.out = d_n;
         const unsigned grid = (unsigned)std::min<int64_t>((int64_t)nb * gp.ngroups, ctx->sm_count);
-        const int ti = pg_time_begin(ctx, "k2t_gram_n");
-        if (ch_n == 4) k2t_gram<1, 4><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
-        else if (ch_n == 2) k2t_gram<1, 2><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
-        else k2t_gram<1, 1><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
+        PG_TRY(pg_timed(ctx, "k2t_gram_n", [&] {
+            if (ch_n == 4) k2t_gram<1, 4><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
+            else if (ch_n == 2) k2t_gram<1, 2><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
+            else k2t_gram<1, 1><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
+        }));
     }
     {
         gp.R = ps.R;
@@ -1084,29 +1060,22 @@ int pg_k2t_pairs(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const in
         gp.cps = ps.cps;
         gp.out = d_diff;
         const unsigned grid = (unsigned)std::min<int64_t>((int64_t)nb * gp.ngroups, ctx->sm_count);
-        const int ti = pg_time_begin(ctx, "k2t_gram_diff");
-        k2t_gram<2, 1><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp);
-        pg_time_end(ctx, ti);
-        PG_CUDA(cudaGetLastError());
+        PG_TRY(pg_timed(ctx, "k2t_gram_diff", [&] { k2t_gram<2, 1><<<grid, GRAM_THREADS, smem, ctx->stream>>>(gp); }));
     }
     return PG_OK;
 }
 
 int pg_k2t_seq_nonnan(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const int64_t* d_hi, int nb, long long* d_out) {
-    const int ti = pg_time_begin(ctx, "k2_seq_nonnan");
-    k2t_seq_nonnan<<<dim3((unsigned)((ps.Hk + 127) / 128), (unsigned)nb), 128, 0, ctx->stream>>>(ps.vplane, ps.R, ps.Hk,
-                                                                                                ps.site_base, d_lo, d_hi, d_out);
-    pg_time_end(ctx, ti);
-    PG_CUDA(cudaGetLastError());
-    return PG_OK;
+    return pg_timed(ctx, "k2_seq_nonnan", [&] {
+        k2t_seq_nonnan<<<dim3((unsigned)((ps.Hk + 127) / 128), (unsigned)nb), 128, 0, ctx->stream>>>(ps.vplane, ps.R, ps.Hk,
+                                                                                                    ps.site_base, d_lo, d_hi, d_out);
+    });
 }
 
 int pg_k2t_het(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const int64_t* d_hi, int nb, const int32_t* d_ind_start,
                int n_ind, int min_sites, double* d_out) {
-    const int ti = pg_time_begin(ctx, "k2_het");
-    k2t_het<<<dim3((unsigned)((n_ind + 127) / 128), (unsigned)nb), 128, 0, ctx->stream>>>(
-        ps.vplane, ps.pq, ps.cps, ps.R, ps.site_base, d_lo, d_hi, d_ind_start, n_ind, min_sites, d_out);
-    pg_time_end(ctx, ti);
-    PG_CUDA(cudaGetLastError());
-    return PG_OK;
+    return pg_timed(ctx, "k2_het", [&] {
+        k2t_het<<<dim3((unsigned)((n_ind + 127) / 128), (unsigned)nb), 128, 0, ctx->stream>>>(
+            ps.vplane, ps.pq, ps.cps, ps.R, ps.site_base, d_lo, d_hi, d_ind_start, n_ind, min_sites, d_out);
+    });
 }

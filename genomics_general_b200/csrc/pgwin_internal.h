@@ -178,6 +178,28 @@ int pg_d2h_staged(pg_ctx* ctx, void* dst, const void* src, size_t bytes);   // l
 int pg_build_segments(pg_ctx* ctx);
 int pg_pack_rows(pg_ctx* ctx, int64_t s0, int64_t n);   // rows [s0, s0 + n) of the packed companion from d_geno (ctx stream)
 
+// launch() (one launch, or a few that share the label) bracketed by the timing label `name`, then the launch error check
+template <class Launch>
+int pg_timed(pg_ctx* ctx, const char* name, Launch&& launch) {
+    const int ti = pg_time_begin(ctx, name);
+    launch();
+    pg_time_end(ctx, ti);
+    PG_CUDA(cudaGetLastError());
+    return PG_OK;
+}
+
+// Kernels that take more dynamic shared memory than the default limit need an attribute, which is per device: set it once per
+// kernel and per device.  Only for a fixed `bytes` per kernel.
+template <auto Kern>
+int pg_smem_limit(const pg_ctx* ctx, int bytes) {
+    static bool set[64] = {};
+    if (!set[ctx->device & 63]) {
+        PG_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        set[ctx->device & 63] = true;
+    }
+    return PG_OK;
+}
+
 // tensor-core pairwise path (k2t.cu): bit-packed operand planes of one site span
 struct K2TPlanes {
     int Hk = 0, R = 0;                 // plane rows (haplotypes in `order`), rows allocated (multiple of 16, pad rows zero)
@@ -187,7 +209,6 @@ struct K2TPlanes {
     const int32_t* cps = nullptr;      // [64 nchunk_v + 1]: pseudo-sites before each site of the span
     int64_t npseudo = 0;
     const uint64_t* pq = nullptr;      // [ceil(npseudo / 64)][2][R]: P and Q planes of the pseudo-sites
-    const int32_t* d_iota = nullptr;   // [Hk] 0..Hk-1
     // n_ij is computed over "mask rows": one per plane row, or — when rows 2k and 2k+1 have identical valid planes (the two
     // haplotypes of a sample with per-genotype missingness) — one per pair of rows
     int Hm = 0, R2 = 0;
@@ -195,6 +216,9 @@ struct K2TPlanes {
     const int32_t* d_mid = nullptr;    // [Hk] mask row of each plane row
 };
 bool pg_k2_use_tensor();               // false when PG_K2_POPC is set (the bit-plane POPC kernels, kept as a checker)
+// can the tensor path's plane builders take Hk plane rows of `pitch`-byte site rows?  They stage 16 bytes per column and 8 per
+// plane row in 96 KiB of shared memory: beyond about 4000 haplotype columns only the POPC kernels (any width) build planes
+inline bool pg_k2t_fits(int pitch, int Hk) { return (size_t)16 * pitch + (size_t)((Hk + 15) / 16 * 16) * 8 <= 96 * 1024; }
 int pg_k2t_build(pg_ctx* ctx, const std::vector<int32_t>& order, int64_t lo, int64_t hi, K2TPlanes& ps);
 int pg_k2t_pairs(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const int64_t* d_hi, int nb, int32_t* d_diff,
                  int32_t* d_n);

@@ -1,8 +1,9 @@
 """The pairwise path (csrc/k2.cu, csrc/k2t.cu) at the boundaries where its behaviour changes, against plain float64 / int64
 definitions of the same quantities:
 
-  1. window batching: every caller cuts its windows into batches that fit pair_budget_bytes() (PG_PAIR_SCRATCH_MB); the
-     batch rows are mapped back to the windows' own rows (routed subsets, duplicates, empty windows in between)
+  1. window batching: every caller of the pair matrices cuts its windows into batches that fit pair_batch_size()
+     (PG_PAIR_SCRATCH_MB), pg_ind_het and pg_seq_nonnan into batches of 65535 windows; the batch rows are mapped back to the
+     windows' own rows (routed subsets, duplicates, empty windows in between)
   2. the tile groups of the wgmma Gram kernels (gram_groups): widths around 16, 64, 128 and 256 rows, per-sample (R2 rows)
      and per-haplotype (R rows) co-valid Grams, odd widths (scalar stores), both stage widths of the co-valid Gram
   3. the switch from the tensor path to the POPC kernels at 16 * pitch + 8 * R > 96 KiB
@@ -10,10 +11,12 @@ definitions of the same quantities:
   5. the plane span: site_base > 0, four alleles, allele sets {0,3} / {1,3}, pseudo-site prefixes on 64-multiples, the
      last partial chunk, and a span without any variable site
   6. the largest population the H12 clustering kernel accepts
+  7. the order of the entry points' argument checks and early returns
 
 Every case also asserts which branch it reached (kernel names and launch counts of eng.last_timings(), popgen's path), so
 that a later change of a threshold cannot silently turn it into a copy of another case."""
 import math
+import re
 import warnings
 
 import numpy as np
@@ -51,7 +54,7 @@ def pitch_for(H):
 
 
 def tensor_fits(H, Hk):
-    """k2.cu build_planes: the tensor path's plane builders stage 16 bytes per column and 8 per plane row (96 KiB)"""
+    """pgwin_internal.h pg_k2t_fits: the tensor path's plane builders stage 16 bytes per column and 8 per plane row (96 KiB)"""
     return 16 * pitch_for(H) + (Hk + 15) // 16 * 16 * 8 <= 96 * 1024
 
 
@@ -274,8 +277,8 @@ def test_popgen_window_batches(eng, batch_data, Hk, monkeypatch):
 
 @BATCH_SELECTIONS
 def test_pairdist_and_hapstats_window_batches(eng, batch_data, Hk, monkeypatch):
-    """pg_pairdist (run-wise copies of consecutive windows) and pg_hapstats (copy_rows_back) across batch boundaries, with
-    empty windows between non-empty ones"""
+    """pg_pairdist (staged copies, run by run of consecutive windows) and pg_hapstats (copy_rows_back) across batch
+    boundaries, with empty windows between non-empty ones"""
     g, lo, hi = batch_data
     eng.upload(g, np.arange(1, BATCH_S + 1, dtype=np.int32))
     eng.set_windows(lo, hi)
@@ -339,6 +342,47 @@ def test_pairdist_cat_chunk_batches(eng, Hk, monkeypatch):
     assert np.array_equal(dist, ref, equal_nan=True)
     d, n = ref_counts(g[:, :Hk])
     assert_close(dist, ind_dists_ref(d, n, hap_ind[:Hk], n_ind), "pairdist_cat", rtol=1e-11, atol=1e-14)
+
+
+def test_het_and_seq_nonnan_window_batches(eng, monkeypatch):
+    """pg_ind_het and pg_seq_nonnan take 65 535 windows per batch: 70 000 windows of 3 sites, every 997th one empty (the
+    copies back break there), are two batches, on the tensor path and on the POPC kernels"""
+    W, H = 70_000, 8
+    S = W + 2
+    rng = np.random.default_rng(65535)
+    g = random_geno(rng, S, H, 0.1)
+    lo = np.arange(W, dtype=np.int64)
+    hi = lo + 3
+    hi[::997] = lo[::997]
+    eng.upload(g, np.arange(1, S + 1, dtype=np.int32))
+    eng.set_windows(lo, hi)
+    nonempty = np.flatnonzero(hi > lo)
+    assert 65535 < len(nonempty) <= 2 * 65535
+    cum = np.concatenate([np.zeros((1, H), dtype=np.int64), np.cumsum(g >= 0, axis=0)])
+    want_nn = cum[hi] - cum[lo]
+    # het against the oracle at both ends, around the batch boundary and at random windows
+    check = set(range(12)) | set(range(W - 12, W)) | set(nonempty[65525:65545].tolist())
+    check |= set(rng.choice(W, 300, replace=False).tolist())
+    hap_ind = (np.arange(H) // 2).astype(np.int32)
+    for env in ({}, {"PG_K2_POPC": "1"}):
+        for k, v in env.items():
+            monkeypatch.setenv(k, v)
+        nn = eng.seq_nonnan()
+        t = kernels(eng)
+        assert_tensor_path(t, not env, gram=False)
+        assert t["k2_seq_nonnan"] == 2, t
+        assert np.array_equal(nn, want_nn), env
+        for min_sites in (0, 3):
+            het = eng.ind_het(hap_ind, H // 2, min_sites)
+            t = kernels(eng)
+            assert_tensor_path(t, not env, gram=False)
+            assert t["k2_het"] == 2, t
+            for w in sorted(w for w in check if hi[w] > lo[w]):
+                assert_close(het[w], do.sample_het(g[lo[w]:hi[w]], hap_ind, H // 2, min_sites),
+                             "het window %d min_sites %d %s" % (w, min_sites, env), rtol=1e-12)
+            assert np.all(np.isnan(het[hi == lo]))
+        for k in env:
+            monkeypatch.delenv(k)
 
 
 # ======================================================================================================================
@@ -699,3 +743,54 @@ def test_hapstats_clustering_width_limit(eng):
     with pytest.raises(PgError, match="too large"):
         eng.hapstats(0.0)
     assert eng.last_timings() == {}
+
+
+# ======================================================================================================================
+# 7. argument checks and early returns
+# ======================================================================================================================
+def test_checks_and_early_returns(eng):
+    """the order of the entry points' checks and early returns, messages included: with no windows pg_pairdist and
+    pg_ind_het return before they read hap_ind and pg_hapstats before its population check; with only empty windows nothing
+    needs a haplotype; pg_pairdist_cat (one window over every site) checks its selection at once"""
+    from genomics_general_b200._lib import PgError
+
+    def raises(msg, fn):
+        with pytest.raises(PgError, match=re.escape(msg)):
+            fn()
+
+    S, H = 100, 6
+    g = random_geno(np.random.default_rng(11), S, H, 0.05)
+    eng.upload(g, np.arange(1, S + 1, dtype=np.int32))
+    bad = np.array([0, 0, 1, 1, 3, 2], dtype=np.int32)     # n_ind = 3: haplotype 4 is out of range
+    none = np.full(H, -1, dtype=np.int32)
+    raises("pg_pairdist: n_ind must be >= 1", lambda: eng.pairdist(bad, 0))
+    raises("pg_ind_het: n_ind must be >= 1", lambda: eng.ind_het(bad, 0))
+    raises("pg_pairdist_cat: n_ind must be >= 1", lambda: eng.pairdist_cat(bad, 0))
+    raises("pg_pairdist_cat: hap_ind[4]=3 out of range", lambda: eng.pairdist_cat(bad, 3))
+    raises("pg_pairdist_cat: no haplotypes selected", lambda: eng.pairdist_cat(none, 3))
+
+    eng.set_windows(np.zeros(0, dtype=np.int64), np.zeros(0, dtype=np.int64))
+    assert eng.pairdist(bad, 3)["dist"].shape == (0, 3, 3)
+    assert eng.ind_het(bad, 3).shape == (0, 3)
+    eng.set_pops(np.zeros(H, dtype=np.int32), 2)           # population 1 has no haplotypes
+    assert eng.hapstats(0.0).shape == (0, 2, 3)
+    assert eng.seq_nonnan().shape == (0, H)
+    assert eng.last_timings() == {}
+
+    eng.set_windows([0, 50], [0, 50])
+    raises("pg_pairdist: hap_ind[4]=3 out of range", lambda: eng.pairdist(bad, 3))
+    raises("pg_ind_het: hap_ind[4]=3 out of range", lambda: eng.ind_het(bad, 3))
+    raises("pg_hapstats: population 1 has no haplotypes", lambda: eng.hapstats(0.0))
+    r = eng.pairdist(none, 3)
+    assert np.all(np.isnan(r["dist"])) and not r["sites"].any() and not r["pos_sum"].any()
+    assert np.all(np.isnan(eng.ind_het(none, 3)))
+    assert not eng.seq_nonnan().any()
+    d, n = eng.pair_counts(1)
+    assert not d.any() and not n.any() and eng.last_timings() == {}
+    raises("pg_pair_counts: window 2 out of range", lambda: eng.pair_counts(2))
+    raises("pg_pair_counts: window -1 out of range", lambda: eng.pair_counts(-1))
+
+    eng.set_windows([0, 50], [0, 60])
+    raises("pairwise path: no haplotypes selected", lambda: eng.pairdist(none, 3))
+    het = eng.ind_het(none, 3)                              # no haplotype selected: all nan, nothing launched
+    assert het.shape == (2, 3) and np.all(np.isnan(het)) and eng.last_timings() == {}
