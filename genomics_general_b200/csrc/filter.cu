@@ -433,10 +433,12 @@ __global__ void __launch_bounds__(256) k_filter_emit(const __grid_constant__ Emi
             for (int a = 0; a < 4; ++a)
                 if (rank[a] == nr - 1) count_allele = a;
         }
-        // prefix: the scaffold and position fields as they are in the text (filterGenotypes.py:53 objects[:2])
+        // prefix: the scaffold and position fields as they are in the text (filterGenotypes.py:53 objects[:2]); a data line
+        // may start with blanks (ingest.cu line_start_at), which line.split() drops
         long long l0 = 0, e0 = 0, b1 = 0, e1 = 0;
         if (lane == 0) {
             l0 = ep.starts[site];
+            while (ep.text[l0] != '\n' && ws_or_nl(ep.text[l0])) ++l0;
             e0 = l0;
             while (!ws_or_nl(ep.text[e0])) ++e0;
             b1 = e0;
