@@ -27,9 +27,7 @@ namespace {
 // consumer warps per CTA (+ one TMA producer warp): 8, or 12 where the register budget allows (65536 / 13 / 32 = 157)
 constexpr int K1_MAX_WARPS = 12;
 
-enum { MODE_POPGEN = 0, MODE_ABBA = 1, MODE_COUNTS = 2, MODE_POPGEN_FREQ = 3, MODE_FOURPOP = 4,   // FREQ = POPGEN + popFreq counters
-       MODE_FOURPOP_Q = 5 };   // FOURPOP with the informative sites of a warp queued and evaluated 32 at a time (site pass only;
-                               // experimental, PG_K1_FOURPOP_QUEUE: see the comment in k1_site_pass)
+enum { MODE_POPGEN = 0, MODE_ABBA = 1, MODE_COUNTS = 2, MODE_POPGEN_FREQ = 3, MODE_FOURPOP = 4 };   // FREQ = POPGEN + popFreq counters
 
 struct K1Params {
     const uint8_t* geno;
@@ -230,6 +228,31 @@ __device__ __forceinline__ int find_seg(const int64_t* __restrict__ brk, int nse
     return lo;
 }
 
+// This lane's site lies in segment sg (cur_seg when it has not moved on).  Before any lane of the warp moves, the warp
+// flushes the sums it holds into the segments they belong to.  Warp-uniform control flow.  sg is taken by reference:
+// passed by value, it changes the instruction schedule ptxas (sm_90a) picks for 36 of the site-pass kernels.
+template <class Flush>
+__device__ __forceinline__ void seg_step(const int& sg, int& cur_seg, int64_t& seg_end, int& since_flush, const int64_t* brk,
+                                         Flush&& flush) {
+    if (__any_sync(0xffffffffu, sg != cur_seg)) {
+        flush();
+        since_flush = 0;
+        if (sg != cur_seg) {
+            cur_seg = sg;
+            seg_end = __ldg(brk + sg + 1);
+        }
+    }
+}
+
+// the 32-bit sums must not overflow: flush them every acc_limit sites (never taken for N < ~900)
+template <class Flush>
+__device__ __forceinline__ void acc_limit_step(int& since_flush, int acc_limit, Flush&& flush) {
+    if (++since_flush > acc_limit) {
+        flush();
+        since_flush = 1;
+    }
+}
+
 template <int MODE, int P>
 struct ModeTraits;
 template <int P>
@@ -250,10 +273,6 @@ struct ModeTraits<MODE_COUNTS, P> {
 };
 template <int P>
 struct ModeTraits<MODE_FOURPOP, P> {
-    static constexpr int QI = 3, QU = 0, QD = 16;
-};
-template <int P>
-struct ModeTraits<MODE_FOURPOP_Q, P> {
     static constexpr int QI = 3, QU = 0, QD = 16;
 };
 
@@ -451,11 +470,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass(const __grid_co
     int64_t seg_end = -1;
     const int seg_first = (MODE == MODE_COUNTS) ? 0 : prm.cta_seg_first[b];
     const int64_t slot_base = (MODE == MODE_COUNTS) ? 0 : prm.cta_slot_off[b];
-    // MODE_FOURPOP_Q: one queued informative site per lane (k | n << 16 of P1..P4).  Sites are queued only while every lane
-    // of the warp is in the same segment, and the queue is emptied before any lane changes segment, so whichever lane
-    // evaluates a queued site adds it to the sums of the right segment.
-    uint32_t q1 = 0u, q2 = 0u, q3 = 0u, q4 = 0u;
-    bool qpend = false;
+    auto flush = [&] { warp_flush<QI, QU, QD>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW); };
 
     for (int it = team; it < ntiles; it += nteams) {
         const int stage = it % prm.stages;
@@ -535,18 +550,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass(const __grid_co
             // ---- segment bookkeeping (warp-uniform control flow) ----
             int sg = cur_seg;
             if (owner && site >= seg_end) sg = find_seg(prm.brk, prm.nseg, cur_seg + 1, site);
-            if (__any_sync(0xffffffffu, sg != cur_seg)) {
-                if (MODE == MODE_FOURPOP_Q) {
-                    if (qpend) fourpop_add(acc, q1, q2, q3, q4);
-                    qpend = false;
-                }
-                warp_flush<QI, QU, QD>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
-                since_flush = 0;
-                if (sg != cur_seg) {
-                    cur_seg = sg;
-                    seg_end = __ldg(prm.brk + sg + 1);
-                }
-            }
+            seg_step(sg, cur_seg, seg_end, since_flush, prm.brk, flush);
 
             if (MODE == MODE_POPGEN || MODE == MODE_POPGEN_FREQ) {
                 bool allpres = true, allmiss = true;
@@ -557,10 +561,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass(const __grid_co
                 }
                 const bool pres = owner && allpres;
                 const bool ragged = owner && !allpres && !allmiss;
-                if (++since_flush > prm.acc_limit) {      // the 32-bit sums must not overflow (never taken for N < ~900)
-                    warp_flush<QI, QU, QD>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
-                    since_flush = 1;
-                }
+                acc_limit_step(since_flush, prm.acc_limit, flush);
                 acc.i[0] += pres ? 1 : 0;
                 acc.i[1] += ragged ? 1 : 0;
                 acc.i[2] += (long long)posv;
@@ -659,7 +660,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass(const __grid_co
                 }
             }
 
-            if (MODE == MODE_FOURPOP || MODE == MODE_FOURPOP_Q) {
+            if (MODE == MODE_FOURPOP) {
                 // genomics.py:1595-1603: biallelic over P1+P2+P3+P4 and enough data in each population
                 uint32_t tot[4];
                 int nall = 0;
@@ -701,55 +702,14 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass(const __grid_co
                           (k3 == 0 || k3 == n[2]);
                 const uint32_t e1 = k1 | (n[0] << 16), e2 = k2 | (n[1] << 16), e3 = k3 | (n[2] << 16), e4 = k4 | (n[3] << 16);
                 acc.i[0] += hit ? 1 : 0;
-                if (MODE == MODE_FOURPOP) {
-                    if (hit) fourpop_add(acc, e1, e2, e3, e4);
-                } else {
-                    // About a third of the lanes hold an informative site, and the ~1000 instructions of the evaluation
-                    // run for the whole warp whenever one does.  Here the informative sites move into free queue slots of
-                    // the warp (one per lane) and are evaluated when the next ones no longer fit, i.e. with (nearly) all
-                    // 32 lanes at work.  The sums are identical, but the ballot / rank / __fns / four shuffles of every
-                    // iteration can cost more than the evaluations they save, so it stays an experiment
-                    // (PG_K1_FOURPOP_QUEUE; tools/fourpop_time.py times both).
-                    const unsigned full_m = 0xffffffffu;
-                    const int seg0 = __shfl_sync(full_m, cur_seg, 0);
-                    if (!__all_sync(full_m, cur_seg == seg0)) {
-                        // lanes in two segments (the iteration that crosses a window boundary, the tail of the data): the
-                        // queue is empty — a segment change empties it — and every lane evaluates its own site
-                        if (hit) fourpop_add(acc, e1, e2, e3, e4);
-                    } else {
-                        const unsigned hits = __ballot_sync(full_m, hit);
-                        if (hits) {
-                            unsigned pm = __ballot_sync(full_m, qpend);
-                            const int nh = __popc(hits);
-                            if (nh > 32 - __popc(pm)) {         // no room for the new sites: evaluate the queued ones
-                                if (qpend) fourpop_add(acc, q1, q2, q3, q4);
-                                qpend = false;
-                                pm = 0u;
-                            }
-                            const unsigned fr = ~pm;
-                            const int r = __popc(fr & ((1u << lane) - 1u));          // rank of this lane among the free ones
-                            const bool take = ((fr >> lane) & 1u) && r < nh;
-                            const int src = take ? (int)__fns(hits, 0, r + 1) : lane;  // lane of the (r+1)-th new site
-                            const uint32_t t1 = __shfl_sync(full_m, e1, src), t2 = __shfl_sync(full_m, e2, src);
-                            const uint32_t t3 = __shfl_sync(full_m, e3, src), t4 = __shfl_sync(full_m, e4, src);
-                            if (take) {
-                                q1 = t1;
-                                q2 = t2;
-                                q3 = t3;
-                                q4 = t4;
-                                qpend = true;
-                            }
-                        }
-                    }
-                }
+                if (hit) fourpop_add(acc, e1, e2, e3, e4);
             }
         }
 
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[stage]);   // this warp is done with the stage's bytes
     }
-    if (MODE == MODE_FOURPOP_Q && qpend) fourpop_add(acc, q1, q2, q3, q4);
-    if (MODE != MODE_COUNTS) warp_flush<QI, QU, QD>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+    if (MODE != MODE_COUNTS) flush();
 }
 
 
@@ -874,6 +834,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
     int64_t seg_end = -1;
     const int seg_first = (MODE == MODE_COUNTS) ? 0 : prm.cta_seg_first[b];
     const int64_t slot_base = (MODE == MODE_COUNTS) ? 0 : prm.cta_slot_off[b];
+    auto flush = [&] { warp_flush_lp<3, QU>(ai, au, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW, Q, spw, X, s_q); };
 
     for (int it = team; it < ntiles; it += nteams) {
         const int stage = it % prm.stages;
@@ -923,18 +884,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
             if (owner && site >= seg_end) sg = find_seg(prm.brk, prm.nseg, cur_seg + 1, site);
             sg = __shfl_sync(0xffffffffu, sg, sl);                   // lane sl is population 0 of this site
             if (!valid) sg = cur_seg;
-            if (__any_sync(0xffffffffu, sg != cur_seg)) {
-                warp_flush_lp<3, QU>(ai, au, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW, Q, spw, X, s_q);
-                since_flush = 0;
-                if (sg != cur_seg) {
-                    cur_seg = sg;
-                    seg_end = __ldg(prm.brk + sg + 1);
-                }
-            }
-            if (++since_flush > prm.acc_limit) {
-                warp_flush_lp<3, QU>(ai, au, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW, Q, spw, X, s_q);
-                since_flush = 1;
-            }
+            seg_step(sg, cur_seg, seg_end, since_flush, prm.brk, flush);
+            acc_limit_step(since_flush, prm.acc_limit, flush);
 
             const unsigned bf = __ballot_sync(0xffffffffu, valid && n == myN);
             const unsigned bz = __ballot_sync(0xffffffffu, valid && n == 0u);
@@ -963,7 +914,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[stage]);
     }
-    if (MODE != MODE_COUNTS) warp_flush_lp<3, QU>(ai, au, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW, Q, spw, X, s_q);
+    if (MODE != MODE_COUNTS) flush();
 }
 
 // ---- bit-sliced popgen pass on the packed companion (ctx.cu pg_pack_rows) ------------------------------------------
@@ -1245,7 +1196,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
                 ArrCounts<P> ct;
                 packed_counts<P>(prm, s_ent, row, walk, G, spw, ct);
 
-                // ---- segment bookkeeping (warp-uniform control flow), as in k1_site_pass ----
+                // ---- segment bookkeeping: seg_step and acc_limit_step written out.  Calling them (flush as a lambda) here
+                // changes the instruction schedule ptxas (sm_90a) picks for six of the packed kernels ----
                 int sg = cur_seg;
                 if (owner && site >= seg_end) sg = find_seg(prm.brk, prm.nseg, cur_seg + 1, site);
                 if (__any_sync(0xffffffffu, sg != cur_seg)) {
@@ -2765,7 +2717,6 @@ int pg_fourpop_enqueue(pg_ctx* ctx, const int* sel, double min_data, int mode, v
     PG_CHECK(mode >= 0 && mode <= 2, "pg_fourpop: mode must be 0 (default), 1 (polarize) or 2 (fixed)");
     // sitesUsed of a record without sites is 0.0, not NaN
     return fourpop_enqueue<MODE_FOURPOP>(ctx, "pg_fourpop", 2, 19, 17, 16, sel, min_data, mode, d_rec, [&](const K1Launch& L) {
-        if (getenv("PG_K1_FOURPOP_QUEUE")) return launch_site_pass<MODE_FOURPOP_Q, 4>(ctx, L, "k1_fourpop");
         return launch_site_pass<MODE_FOURPOP, 4>(ctx, L, "k1_fourpop");
     });
 }

@@ -358,8 +358,22 @@ K1_KNOBS = [{}, {"PG_K1_NO_BYTES": "1"}, {"PG_K1_NW": "8"}, {"PG_K1_NO_BYTES": "
             {"PG_K1_LANEPOP": "1", "PG_K1_ACC_LIMIT": "2"}, {"PG_K1_LANEPOP": "1", "PG_K1_WPT": "1"}]
 
 
+def _popgen_fields(eng, pops):
+    """Every record field of popgen with the popFreq counters on, then the closed-form fields again with them off."""
+    eng.set_freqstats(True)
+    r = eng.popgen(*pops)
+    fq = eng.popgen_freqstats()
+    eng.set_freqstats(False)
+    r2 = eng.popgen(*pops)
+    for k in ("pi", "dxy", "fst"):
+        assert np.array_equal(r2[k], r[k], equal_nan=True), k
+    return [r[k] for k in sorted(r)] + [fq[k] for k in sorted(fq)]
+
+
 @pytest.mark.parametrize("shape", [(2, 9), (3, 20), (5, 7), (8, 13), (2, 150), (8, 100), (4, 127)], ids=lambda s: "%dx%d" % s)
 def test_k1_variants_are_bit_identical_and_match_the_oracle(eng, shape, monkeypatch):
+    """The byte pass's popgen and counts instantiations (PG_K1_BYTE_PASS: popgen otherwise takes the packed companion) agree
+    bit for bit across the knobs that pick them, with the oracle, and with the default packed pass."""
     from genomics_general_b200 import synth
     from oracle import dense_oracle as do
     P, spp = shape
@@ -373,8 +387,9 @@ def test_k1_variants_are_bit_identical_and_match_the_oracle(eng, shape, monkeypa
     hi = np.array([10, 4000, 4001, 9000, 15000, 20000], dtype=np.int64)
     base = None
     for knobs in K1_KNOBS:
-        for k in ("PG_K1_NO_BYTES", "PG_K1_NW", "PG_K1_ACC_LIMIT", "PG_K1_G", "PG_K1_LANEPOP", "PG_K1_WPT"):
+        for k in ("PG_K1_NO_BYTES", "PG_K1_NW", "PG_K1_ACC_LIMIT", "PG_K1_G", "PG_K1_LANEPOP", "PG_K1_WPT", "PG_K1_BYTE_PASS"):
             monkeypatch.delenv(k, raising=False)
+        monkeypatch.setenv("PG_K1_BYTE_PASS", "1")
         for k, v in knobs.items():
             monkeypatch.setenv(k, v)
         eng.upload(g, pos)
@@ -405,6 +420,13 @@ def test_k1_variants_are_bit_identical_and_match_the_oracle(eng, shape, monkeypa
         else:
             for a, b in zip(cur, base):
                 assert np.array_equal(a, b, equal_nan=True), knobs
+    byte_fields = _popgen_fields(eng, (1, 0.01))
+    monkeypatch.delenv("PG_K1_BYTE_PASS")
+    for k in ("PG_K1_NO_BYTES", "PG_K1_NW", "PG_K1_ACC_LIMIT", "PG_K1_G", "PG_K1_LANEPOP", "PG_K1_WPT"):
+        monkeypatch.delenv(k, raising=False)
+    assert eng.packed_rows(0, 1) is not None           # the companion exists: without PG_K1_BYTE_PASS, the packed pass runs
+    for a, b in zip(_popgen_fields(eng, (1, 0.01)), byte_fields):
+        assert np.array_equal(a, b, equal_nan=True), "packed pass"
 
 
 def test_seq_nonnan_bit_exact(eng):
@@ -525,7 +547,8 @@ def test_many_small_populations_counts_and_target_freqs(eng, monkeypatch):
 @pytest.mark.parametrize("P", [3, 4, 6, 8])
 def test_lane_per_population_with_interleaved_columns(eng, P, monkeypatch):
     """k1_site_pass_lp forced on a layout it is not tuned for: populations interleaved column by column, unused
-    haplotypes, unequal sizes (masked chunks only, P padded to 4 / 8)."""
+    haplotypes, unequal sizes (masked chunks only, P padded to 4 / 8).  Popgen runs on the byte pass (PG_K1_BYTE_PASS), and
+    the default packed pass must give the same record fields bit for bit."""
     from genomics_general_b200 import synth
     from oracle import dense_oracle as do
     rng = np.random.default_rng(50 + P)
@@ -542,6 +565,7 @@ def test_lane_per_population_with_interleaved_columns(eng, P, monkeypatch):
     lo = np.arange(0, S, 750, dtype=np.int64)
     hi = np.minimum(lo + 1000, S)                       # overlapping windows
     res = []
+    monkeypatch.setenv("PG_K1_BYTE_PASS", "1")
     for lp in ("0", "1"):
         monkeypatch.setenv("PG_K1_LANEPOP", lp)
         eng.upload(g, pos)
@@ -552,9 +576,14 @@ def test_lane_per_population_with_interleaved_columns(eng, P, monkeypatch):
         fq = eng.popgen_freqstats()
         eng.set_freqstats(False)
         res.append([r["pi"], r["dxy"], r["fst"], r["sites"], r["pos_sum"], r["path"], fq["S"], fq["thetaPi"], eng.site_counts()])
+    byte_fields = _popgen_fields(eng, (10, 0.01))
     monkeypatch.delenv("PG_K1_LANEPOP")
+    monkeypatch.delenv("PG_K1_BYTE_PASS")
     for a, b in zip(*res):
         assert np.array_equal(a, b, equal_nan=True)
+    assert eng.packed_rows(0, 1) is not None           # the companion exists: without PG_K1_BYTE_PASS, the packed pass runs
+    for a, b in zip(_popgen_fields(eng, (10, 0.01)), byte_fields):
+        assert np.array_equal(a, b, equal_nan=True), "packed pass"
     assert np.all(res[0][5] == 1)
     assert np.array_equal(res[1][8].astype(np.int64), do.site_counts(g, hp, P))
     for w in (0, 5, len(lo) - 1):

@@ -2,8 +2,8 @@
 
   1. forced launch geometries (lanes per site, warps per team, sites per lane, ring depth, tile size) for ABBA-BABA, fourPop
      (all three modes) and per-site counts, on interleaved populations, unused columns and a population of > 255 haplotypes
-  2. the queued fourPop evaluation (PG_K1_FOURPOP_QUEUE): tiny windows, windows ending inside a warp's sites, 1 and 4 lanes per
-     site, a last partial tile
+  2. fourPop (all three modes) on tiny windows, windows ending inside a warp's sites and a last partial tile, at 1 and 4
+     lanes per site
   3. window bounds on tile and CTA seams, S % T != 0, S < T
   4. the natural flush of the 32-bit popgen sums (acc_limit = (2^32 - 1) / maxN^2) with the large population not first
   5. wide rows (8, 16 and 32 lanes per site) up to the longest row the plan accepts, and the first row it refuses
@@ -25,7 +25,7 @@ from oracle import dense_oracle as do
 pytestmark = pytest.mark.gpu
 
 KNOBS = ("PG_K1_G", "PG_K1_NW", "PG_K1_WPT", "PG_K1_I", "PG_K1_STAGES", "PG_K1_TILE_KB", "PG_K1_ACC_LIMIT", "PG_K1_LANEPOP",
-         "PG_K1_NO_BYTES", "PG_K1_FOURPOP_QUEUE", "PG_COUNTS_NO_GATHER")
+         "PG_K1_NO_BYTES", "PG_COUNTS_NO_GATHER")
 TOL = dict(rtol=1e-9, atol=1e-12)
 FP_KEYS = do.FOURPOP_KEYS[:14]
 FP_F4 = ("fhom", "D", "fd", "fdm")                         # numerator: sum of f4
@@ -298,10 +298,10 @@ def test_geometry_matrix_abba_fourpop_counts(eng, shape, monkeypatch):
 
 
 # ======================================================================================================================
-# 2. the queued fourPop evaluation
+# 2. fourPop windows inside a warp's sites
 # ======================================================================================================================
 @pytest.mark.parametrize("lanes", [1, 4])
-def test_fourpop_queue_matches_default_and_oracle(eng, lanes, monkeypatch):
+def test_fourpop_windows_inside_a_warp_match_the_oracle(eng, lanes, monkeypatch):
     rng = np.random.default_rng(20 + lanes)
     hp = contiguous_pops((11, 13, 9, 12), gap=2)
     P = 4
@@ -313,24 +313,14 @@ def test_fourpop_queue_matches_default_and_oracle(eng, lanes, monkeypatch):
     hi = np.concatenate([tiny_lo + 2, [3653, 3685, 8000, S, S]]).astype(np.int64)      # ends inside a warp's 32 sites
     wins = list(range(0, len(tiny_lo), 7)) + list(range(len(tiny_lo), len(lo)))
     sel, md = (2, 0, 1, 3), 0.3
-    res, cache = {}, {}
-    for q in (False, True):
-        knobs = {"PG_K1_G": str(lanes)} if lanes > 1 else {}
-        if q:
-            knobs["PG_K1_FOURPOP_QUEUE"] = "1"
-        set_knobs(monkeypatch, knobs)
-        assert plan(S, hp, P)["lanes_per_site"] == lanes
-        load(eng, g, pos, hp, P, lo, hi)
-        for mode, kw in FP_MODES:
-            r = eng.fourpop(*sel, md, **kw)
-            assert launches(eng, "k1_fourpop") == 1
-            check_fourpop(r, g, hp, sel, md, kw, lo, hi, pos, wins, "queue=%s" % q, cache)
-            res[q, mode] = r
-    for mode, _ in FP_MODES:
-        a, b = res[False, mode], res[True, mode]
-        assert np.array_equal(a["sitesUsed"], b["sitesUsed"]) and np.array_equal(a["pos_sum"], b["pos_sum"])
-        for k in ("ABBA", "BABA", "ABAA", "BAAA"):
-            assert_close(b[k], a[k], mode + " " + k, **TOL)
+    set_knobs(monkeypatch, {"PG_K1_G": str(lanes)} if lanes > 1 else {})
+    assert plan(S, hp, P)["lanes_per_site"] == lanes
+    load(eng, g, pos, hp, P, lo, hi)
+    cache = {}
+    for mode, kw in FP_MODES:
+        r = eng.fourpop(*sel, md, **kw)
+        assert launches(eng, "k1_fourpop") == 1
+        check_fourpop(r, g, hp, sel, md, kw, lo, hi, pos, wins, "lanes=%d" % lanes, cache)
 
 
 # ======================================================================================================================

@@ -1,5 +1,5 @@
-"""Kernel time of genomics.fourPop per window on the C2 shape (10 M sites x 400 haplotypes, 2 % missing, 2000 windows) — for the
-PG_K1_FOURPOP_QUEUE knob.  Prints one JSON line (ms of the site pass, HBM GB/s of the algorithmic bytes, a checksum)."""
+"""Kernel time of genomics.fourPop per window on the C2 shape (10 M sites x 400 haplotypes, 2 % missing, 2000 windows).  Prints
+one JSON line (ms of the site pass, HBM GB/s of the algorithmic bytes, a checksum)."""
 import json
 import os
 import sys
@@ -24,4 +24,4 @@ with Engine(0) as eng:
         ms = eng.last_timings()["k1_fourpop"]["ms"]
         out[name] = dict(ms=round(ms, 4), GBps=round(S * 404 / ms / 1e6, 1),
                          check=float(sum(np.nansum(r[k]) for k in eng.FOURPOP_KEYS)), used=float(np.nansum(r["sitesUsed"])))
-    print(json.dumps(dict(queue=bool(os.environ.get("PG_K1_FOURPOP_QUEUE")), **out)))
+    print(json.dumps(out))
