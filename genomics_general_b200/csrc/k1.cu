@@ -228,6 +228,18 @@ __device__ __forceinline__ int find_seg(const int64_t* __restrict__ brk, int nse
     return lo;
 }
 
+// find_seg for a site at or past segment `from`'s start, galloping from there: brk[from + 1], brk[from + 3], brk[from + 7], ...
+// until one lies past the site, then a binary search inside that bracket.  One load when the site lies in segment from, the
+// common case of a pass that moves through its segments in order; the same result as find_seg for any jump.
+__device__ __forceinline__ int next_seg(const int64_t* __restrict__ brk, int nseg, int from, int64_t site) {
+    int lo = from, step = 1;
+    while (lo + step < nseg && __ldg(brk + lo + step) <= site) {
+        lo += step;
+        step <<= 1;
+    }
+    return find_seg(brk, min(lo + step, nseg), lo, site);
+}
+
 // This lane's site lies in segment sg (cur_seg when it has not moved on).  Before any lane of the warp moves, the warp
 // flushes the sums it holds into the segments they belong to.  Warp-uniform control flow.  sg is taken by reference:
 // passed by value, it changes the instruction schedule ptxas (sm_90a) picks for 36 of the site-pass kernels.
@@ -361,12 +373,13 @@ __device__ __forceinline__ void k1_producer(const K1Params& prm, uint8_t* tiles,
 // [row0[t], row0[t + 1]) (room for row_cap of them), then the positions of its sites [site_lo[t], site_lo[t + 1]) from the first
 // one rounded down to a multiple of 4 (bulk copies take 16-byte-aligned sources; the consumers apply the offset), then its
 // codes (code_pitch of them) and the slots of its varied rows.  The
-// count of varied rows goes to s_nvar[stage] before the stage is armed, so the mbarrier's phase publishes it.  A tile is
+// tile's first site goes to s_site0[stage], and its varied rows and sites to s_nvar[stage] (nvar | nsites << 16; R < 2^15,
+// Tmax <= 2^15), before the stage is armed, so the mbarrier's phase publishes them.  A tile is
 // about a microsecond of HBM time, as long as a dependent load of row0, so the 32 lanes load the offsets of the next 32 tiles
 // while the current 32 are issued.
 __device__ __forceinline__ void k1_producer_uniform(const K1Params& prm, uint8_t* tiles, uint64_t* full, uint64_t* empty,
-                                                    volatile int* s_issued, volatile int* s_nvar, int ntiles, int64_t t0,
-                                                    int lane) {
+                                                    volatile int* s_issued, volatile uint32_t* s_nvar,
+                                                    volatile long long* s_site0, int ntiles, int64_t t0, int lane) {
     auto ld_row0 = [&](int64_t t) { return t <= prm.num_tiles ? __ldg(prm.row0 + t) : (int64_t)0; };
     auto ld_site = [&](int64_t t) { return t <= prm.num_tiles ? __ldg(prm.site_lo + t) : (int64_t)0; };
     int64_t cur = ld_row0(t0 + lane), cur_s = ld_site(t0 + lane);       // lane l: row0 and site_lo of tile t0 + g + l
@@ -389,7 +402,8 @@ __device__ __forceinline__ void k1_producer_uniform(const K1Params& prm, uint8_t
                 const uint32_t bytes = (uint32_t)(nvar * prm.pitch);
                 const uint32_t pbytes = (uint32_t)(((rows * 4 + 15) / 16) * 16);
                 const uint32_t cbytes = (uint32_t)(prm.code_pitch * 2 + ((nvar * 2 + 15) / 16) * 16);
-                s_nvar[stage] = nvar;
+                s_nvar[stage] = (uint32_t)nvar | (uint32_t)(s1 - s0) << 16;
+                s_site0[stage] = s0;
                 mbar_expect_tx(&full[stage], bytes + pbytes + cbytes);
                 const uint8_t* src = prm.geno + r0 * prm.pitch;
                 uint8_t* dst = tiles + (size_t)stage * prm.tile_bytes;
@@ -928,7 +942,9 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
 // population's entries at an offset taken from its site index, which spreads the reads over the banks.
 // UNI: the tiles hold only the varied rows (k1_producer_uniform), a code per site (UNI_CODE | PG_CLS_* for a site whose H
 // haplotypes all carry one allele or are all missing, else its rank among the tile's varied sites) and the slot of each varied
-// row (its site's index in the tile; T <= 2048).  A team then makes two passes over a tile.  Pass V packs the varied rows onto
+// row (its site's index in the tile; T <= 2048).  A tile's varied rows are stored word-major: word x of its row j at word
+// x * nvar + j of the tile, so that the lanes reading the same word of consecutive rows read consecutive words, in
+// distinct banks whatever the pitch.  A team then makes two passes over a tile.  Pass V packs the varied rows onto
 // the team's lanes, Gv lanes per row: the plan's lanes per site (1 at C2 and C5, where more measured slower; 2 for rows of
 // 1 KiB and more; PG_K1_UNI_GV forces 1 .. 32 for the tests), so that a warp walks only when it holds varied rows, and those
 // fill its lanes.  Pass U runs one lane per slot:
@@ -950,17 +966,6 @@ __device__ __forceinline__ void packed_walk(const K1Params& prm, int G, int gsub
         walk[X] = (uint32_t)first | ((uint32_t)cnt << 16);
     }
 }
-
-// this lane's walk[] of the varied-row pass, in shared memory ([X][lane]) or in registers (RegWalk)
-struct SmemWalk {
-    const uint32_t* p;     // the table + lane
-    __device__ __forceinline__ uint32_t operator[](int X) const { return p[X * 32]; }
-};
-template <int P>
-struct RegWalk {
-    uint32_t w[P];
-    __device__ __forceinline__ uint32_t operator[](int X) const { return w[X]; }
-};
 
 // the allele counts of one packed row, combined over the 32 / spw lanes that share it; walk[X] as packed_walk sets it
 // A row's counts per population: n(X) haplotypes present and c(X, a) of allele a.  ArrCounts holds the five numbers;
@@ -1025,6 +1030,37 @@ __device__ __forceinline__ void packed_counts(const K1Params& prm, const uint2* 
     }
 }
 
+// packed_counts for a varied row stored word-major (word x at row[x * nvar]).  Lane gsub of the row's Gv lanes takes entries
+// gsub, gsub + Gv, ... of each population.  ONE (Gv = 1): every lane walks all the entries in the same order, so the entry
+// index is warp-uniform, an entry's load is a broadcast and the lanes' row words are consecutive words.
+template <int P, bool ONE, class CT>
+__device__ __forceinline__ void varied_counts(const K1Params& prm, const uint2* s_ent, const uint32_t* row, int nvar, int Gv,
+                                              int gsub, int spv, CT& ct) {
+    const int pn = prm.wd * nvar;     // words from one plane to the next
+#pragma unroll
+    for (int X = 0; X < P; ++X) {
+        uint32_t a = 0u, a1 = 0u, a2 = 0u, a3 = 0u;
+        // not unrolled: unrolled, the walks of the two variants made the kernel four times longer and slower at C2
+#pragma unroll 1
+        for (int e = prm.ent_lo[X] + (ONE ? 0 : gsub); e < prm.ent_hi[X]; e += (ONE ? 1 : Gv)) {
+            const uint2 em = s_ent[e];
+            const uint32_t* w = row + em.x * nvar;
+            const uint32_t m = w[0] & em.y;
+            const uint32_t b0 = w[pn], b1 = w[2 * pn];
+            a += __popc(m);
+            a1 += __popc(m & b0);
+            a2 += __popc(m & b1);
+            a3 += __popc(m & b0 & b1);
+        }
+        uint32_t p0 = a | (a1 << 16), p1 = a2 | (a3 << 16);
+        for (int d = spv; !ONE && d < 32; d <<= 1) {
+            p0 += __shfl_xor_sync(0xffffffffu, p0, d);
+            p1 += __shfl_xor_sync(0xffffffffu, p1, d);
+        }
+        ct.set(X, p0, p1);
+    }
+}
+
 // whether the site (of the lane that owns it) has every haplotype of every population, or some but not all of them
 template <int P, class CT>
 __device__ __forceinline__ void packed_class(const K1Params& prm, bool owner, const CT& ct, bool& pres, bool& ragged) {
@@ -1063,14 +1099,14 @@ __device__ __forceinline__ void packed_add(ACC& acc, bool pres, bool ragged, con
 
 // Pass U's state, one per consumer warp in shared memory behind the entry table, so that it holds no register while pass V
 // walks: its segment (warp-uniform) and the segment's end, and the positions and the uniform non-missing sites it has added
-// since its last flush.  Behind the records: pass V's walk table (SmemWalk).
+// since its last flush.
 struct UniRec {
     long long pos;
     long long seg_end;
     int seg;
     uint32_t npres;
 };
-constexpr int UNI_SMEM_BYTES = K1_MAX_WARPS * (int)sizeof(UniRec) + PG_MAX_K1_POPS * 32 * 4;
+constexpr int UNI_SMEM_BYTES = K1_MAX_WARPS * (int)sizeof(UniRec);
 
 // the exact sum of the 32 lanes' v, from 32-bit reductions of its 16-bit halves
 __device__ __forceinline__ long long warp_sum_i32(int v) {
@@ -1115,7 +1151,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)prm.stages * prm.tile_bytes);   // [stages]
     uint64_t* empty = full + 8;                                                                  // [stages]
     volatile int* s_issued = reinterpret_cast<volatile int*>(empty + 8);
-    volatile int* s_nvar = s_issued + 8;     // UNI: varied rows of the tile in each stage [stages]
+    volatile uint32_t* s_nvar = reinterpret_cast<volatile uint32_t*>(s_issued + 8);   // UNI: nvar | nsites << 16 [stages]
+    volatile long long* s_site0 = reinterpret_cast<volatile long long*>(s_issued + 16);   // UNI: first site [stages]
     uint2* s_ent = reinterpret_cast<uint2*>(smem + (size_t)prm.stages * prm.tile_bytes + 256);
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1124,18 +1161,9 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     const int ntiles = (int)(t1 - t0);
 
     for (int e = tid; e < prm.n_ent; e += K1_THREADS) s_ent[e] = prm.word_ent[e];
-    UniRec* s_urec = reinterpret_cast<UniRec*>(s_ent + prm.n_ent);          // UNI: [NW] pass U records, then the walk table
-    uint32_t* s_walk = reinterpret_cast<uint32_t*>(s_urec + K1_MAX_WARPS);
+    UniRec* s_urec = reinterpret_cast<UniRec*>(s_ent + prm.n_ent);          // UNI: [NW] pass U records
     const int Gv = prm.uni_gv > 0 ? prm.uni_gv : prm.G;                    // UNI: lanes per varied row, the plan's per site
-    if (UNI && warp < NW) {
-        if (warp == 0) {
-            uint32_t w[P];
-            packed_walk<P>(prm, Gv, lane / (32 / Gv), lane % (32 / Gv), w);
-#pragma unroll
-            for (int X = 0; X < P; ++X) s_walk[X * 32 + lane] = w[X];
-        }
-        if (lane == 0) s_urec[warp] = UniRec{0ll, -1ll, -1, 0u};
-    }
+    if (UNI && warp < NW && lane == 0) s_urec[warp] = UniRec{0ll, -1ll, -1, 0u};
     if (tid == 0) {
         for (int s = 0; s < prm.stages; ++s) {
             mbar_init(&full[s], 1);
@@ -1148,7 +1176,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     __syncthreads();
 
     if (warp == NW) {
-        if (UNI) k1_producer_uniform(prm, tiles, full, empty, s_issued, s_nvar, ntiles, t0, lane);
+        if (UNI) k1_producer_uniform(prm, tiles, full, empty, s_issued, s_nvar, s_site0, ntiles, t0, lane);
         else if (lane == 0) k1_producer<MODE>(prm, tiles, full, empty, s_issued, ntiles, t0);
         return;
     }
@@ -1224,11 +1252,6 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     } else {
         const size_t pos_off = (size_t)prm.row_cap * prm.pitch, codes_off = pos_off + (size_t)(prm.T + 4) * 4;
         const int spv = 32 / Gv, gsub = lane / spv, sl = lane % spv;
-        // Register budget: with 8 populations walk[] lives in shared memory and the counts are expanded once; with fewer, walk[]
-        // stays in registers and the counts stay two words per population (the choices with the fewest spills, ptxas sm_90a)
-        std::conditional_t<P == 8, SmemWalk, RegWalk<P>> walk;
-        if constexpr (P == 8) walk.p = s_walk + lane;
-        else packed_walk<P>(prm, Gv, gsub, sl, walk.w);
 
         for (int it = team; it < ntiles; it += nteams) {
             const int stage = it % prm.stages;
@@ -1237,10 +1260,10 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             __syncwarp();
             mbar_wait(&full[stage], (uint32_t)((it / prm.stages) & 1));
             const uint8_t* tile = tiles + (size_t)stage * prm.tile_bytes;
-            const int64_t tile_site0 = __ldg(prm.site_lo + t0 + it);
-            const int nsites = (int)(__ldg(prm.site_lo + t0 + it + 1) - tile_site0);
+            const int64_t tile_site0 = s_site0[stage];
+            const uint32_t sizes = s_nvar[stage];
+            const int nvar = (int)(sizes & 0xffffu), nsites = (int)(sizes >> 16);
             const int32_t* s_pos = reinterpret_cast<const int32_t*>(tile + pos_off) + (tile_site0 & 3);
-            const int nvar = s_nvar[stage];
             const uint16_t* s_slot = reinterpret_cast<const uint16_t*>(tile + codes_off) + prm.code_pitch;
 
             // ---- pass V: blocks of spv varied rows, block k to warp k % wpt, so a lane's rows stay in site order ----
@@ -1248,13 +1271,16 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
                 const int rw = r + sl;
                 const bool valid = rw < nvar;
                 const bool owner = valid && (gsub == 0);
-                const uint32_t* row = reinterpret_cast<const uint32_t*>(tile + (size_t)(valid ? rw : r) * prm.pitch);
+                const uint32_t* row = reinterpret_cast<const uint32_t*>(tile) + (valid ? rw : r);
+                // with 8 populations the counts are expanded once; with fewer they stay two words per population (the
+                // choices with the fewest spills, ptxas sm_90a)
                 std::conditional_t<P == 8, ArrCounts<P>, PkCounts<P>> ct;
-                packed_counts<P>(prm, s_ent, row, walk, Gv, spv, ct);
+                if (P < 8 && Gv == 1) varied_counts<P, true>(prm, s_ent, row, nvar, 1, 0, 32, ct);
+                else varied_counts<P, false>(prm, s_ent, row, nvar, Gv, gsub, spv, ct);
 
                 const int64_t site = tile_site0 + (valid ? s_slot[rw] : 0);
                 int sg = cur_seg;
-                if (owner && site >= seg_end) sg = find_seg(prm.brk, prm.nseg, cur_seg + 1, site);
+                if (owner && site >= seg_end) sg = next_seg(prm.brk, prm.nseg, cur_seg + 1, site);
                 if (__any_sync(0xffffffffu, sg != cur_seg)) {
                     warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
                     since_flush = 0;
@@ -1312,7 +1338,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
                         upres = 0u;
                         upos = 0ll;
                     }
-                    useg = find_seg(prm.brk, prm.nseg, useg + 1, __shfl_sync(0xffffffffu, site, __ffs(left) - 1));
+                    useg = next_seg(prm.brk, prm.nseg, useg + 1, __shfl_sync(0xffffffffu, site, __ffs(left) - 1));
                     useg_end = __ldg(prm.brk + useg + 1);
                 }
             }
@@ -1709,7 +1735,7 @@ int push(pg_ctx* ctx, uint8_t* base, size_t& off, const T* src, size_t n, T** ou
 // tile has at most R varied rows and at most Tmax sites, and tile t covers the sites [site_lo[t], site_lo[t + 1]).  Per tile:
 // the index of its first varied row (row0, int64 [tiles + 1]), a 16-bit code per site (UNI_CODE | class, or the rank among the
 // tile's varied sites; tile t's codes at t * 2 * code_pitch, code_pitch = Tmax), the slot (index in the tile) of each of its
-// varied rows, behind its codes; and the varied rows, contiguous.  bound holds the first site of each CTA's tiles (B + 1).
+// varied rows, behind its codes; and the varied rows, each tile's contiguous and word-major (k1_uni_codes).  bound holds the first site of each CTA's tiles (B + 1).
 struct UniformStream {
     uint64_t gen = 0;         // ctx->data_gen it describes (0: none)
     uint64_t serial = 0;      // counts the builds (the slot tables follow it)
@@ -1745,10 +1771,14 @@ __global__ void __launch_bounds__(256) k1_uni_count(const uint8_t* __restrict__ 
 }
 
 // codes of tile blockIdx.x (tiles as in k1_uni_count; none when codes is null), and the slot and the source site of each of its
-// varied rows
+// varied rows.  With rows, the block then copies its nvar varied rows from the companion (chunks of 16 bytes per row) into
+// the stream, word-major: word x of its row j to word row0[t] * 4 * chunks + x * nvar + j.  A warp reads one chunk of 32
+// rows and writes each of its words as 32 consecutive words.
 __global__ void __launch_bounds__(256) k1_uni_codes(const uint8_t* __restrict__ cls, int64_t S, const int64_t* __restrict__ site_lo,
                                                     int T, int code_pitch, const int64_t* __restrict__ row0,
-                                                    uint16_t* __restrict__ codes, int64_t* __restrict__ src) {
+                                                    uint16_t* __restrict__ codes, int64_t* __restrict__ src,
+                                                    const uint4* __restrict__ packed = nullptr, int chunks = 0,
+                                                    uint32_t* __restrict__ rows = nullptr) {
     typedef cub::BlockScan<int, 256> Scan;
     __shared__ typename Scan::TempStorage tmp;
     const int64_t t = blockIdx.x, r0 = row0[t];
@@ -1770,6 +1800,19 @@ __global__ void __launch_bounds__(256) k1_uni_codes(const uint8_t* __restrict__ 
         }
         base += total;
     }
+    if (!rows) return;
+    __syncthreads();                          // the block's src entries, read back below
+    const int nvar = base, lane = threadIdx.x & 31;
+    uint32_t* dst = rows + r0 * 4 * chunks;
+    for (int c = threadIdx.x >> 5; c < chunks; c += blockDim.x >> 5)
+        for (int j = lane; j < nvar; j += 32) {
+            const uint4 v = packed[src[r0 + j] * chunks + c];
+            uint32_t* d = dst + (int64_t)4 * c * nvar + j;
+            d[0] = v.x;
+            d[nvar] = v.y;
+            d[2 * nvar] = v.z;
+            d[3 * nvar] = v.w;
+        }
 }
 
 // group k's first site (the site of varied rank k R; 0 for k = 0) and end (the next group's first site; S for the last)
@@ -1812,16 +1855,6 @@ __global__ void __launch_bounds__(256) k1_uni_bounds(const int64_t* __restrict__
     const int64_t B = nt < sm ? (nt > 1 ? nt : 1) : sm;
     for (int64_t b = threadIdx.x; b <= B; b += blockDim.x) info[1 + b] = site_lo[b * nt / B];
     if (threadIdx.x == 0) info[0] = nt;
-}
-
-// varied row r <- companion row src[r], 16 bytes per thread
-__global__ void __launch_bounds__(256) k1_uni_gather(const uint4* __restrict__ packed, const int64_t* __restrict__ src,
-                                                     int64_t nrows, int chunks, uint4* __restrict__ rows) {
-    const int64_t total = nrows * chunks;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t r = i / chunks;
-        rows[i] = packed[src[r] * chunks + (i - r * chunks)];
-    }
 }
 
 // The packed popgen pass over the varied rows only: the stream, its geometry, the slot tables of its CTA ranges and the
@@ -2173,7 +2206,8 @@ int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
     int64_t* d_site_lo = (int64_t*)us.site_lo.p;
     int64_t* d_info = (int64_t*)us.info.p;
     ti = pg_time_begin(ctx, "k1_uniform");
-    // each varied row's site, then the groups of R rows, their pieces, the tiles' first sites and first rows, their codes
+    // each varied row's site, then the groups of R rows, their pieces, the tiles' first sites and first rows, their codes and
+    // varied rows
     k1_uni_codes<<<(unsigned)nc, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, nullptr, CH, CH, d_row0, nullptr, d_src);
     PG_CUDA(cudaGetLastError());
     PG_CUDA(cudaMemsetAsync(d_pieces + ng, 0, 8, ctx->stream));
@@ -2189,13 +2223,9 @@ int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
     PG_CUDA(cudaGetLastError());
     PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, scan_bytes, d_cnt, d_row0, nt_max + 1, ctx->stream));
     k1_uni_codes<<<(unsigned)nt_max, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, d_site_lo, Tmax, us.code_pitch, d_row0,
-                                                           (uint16_t*)us.codes.p, d_src);
+                                                           (uint16_t*)us.codes.p, d_src, (const uint4*)ctx->d_packed, chunks,
+                                                           (uint32_t*)us.rows.p);
     PG_CUDA(cudaGetLastError());
-    if (varied > 0) {
-        const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((varied * chunks + 255) / 256, (int64_t)ctx->sm_count * 16));
-        k1_uni_gather<<<blocks, 256, 0, ctx->stream>>>((const uint4*)ctx->d_packed, d_src, varied, chunks, (uint4*)us.rows.p);
-        PG_CUDA(cudaGetLastError());
-    }
     k1_uni_bounds<<<1, 256, 0, ctx->stream>>>(d_base, ng, d_site_lo, ctx->sm_count, d_info);
     PG_CUDA(cudaGetLastError());
     pg_time_end(ctx, ti);

@@ -1,8 +1,8 @@
 """The popgen site pass three ways, timed alternately in one process: on the one-hot bytes (PG_K1_BYTE_PASS), on every row of
 the packed companion (PG_K1_NO_UNIFORM), and on the packed rows of the varied sites only ("varied_rows", the default where
 enough sites are uniform: a walk over the varied rows on all the team's lanes, then a pass over every slot without a walk),
-at the C2 shape (4 x 50 diploid samples, H = 400, 10 M sites) and the C5 shape (8 x 100 diploid samples, H = 1600, 12.5 M
-sites).  Per pass and shape: median / min / max of the k1_popgen kernel time (CUDA events) over the rounds, the bytes the
+at the C2 shape (4 x 50 diploid samples, H = 400, 10 M sites) with 50,000-site windows and with the benchmark's 5,000-site
+windows (C2_w5000), and the C5 shape (8 x 100 diploid samples, H = 1600, 12.5 M sites).  Per pass and shape: median / min / max of the k1_popgen kernel time (CUDA events) over the rounds, the bytes the
 pass reads per site, the achieved GB/s, the time of the varied-row build (k1_uniform, once per data change), the varied-row
 stream's geometry (row budget R, tile bound Tmax, ring stages and bytes, tiles, mean rows and sites per tile), and whether the
 records of the three passes are bit-identical.
@@ -98,7 +98,8 @@ def main():
     args = ap.parse_args()
     out = {"card": card(), "shapes": {}}
     with Engine(0) as eng:
-        for name, P, spp, S, w in (("C2", 4, 50, args.c2_sites, 50_000), ("C5", 8, 100, args.c5_sites, 5000)):
+        for name, P, spp, S, w in (("C2", 4, 50, args.c2_sites, 50_000), ("C2_w5000", 4, 50, args.c2_sites, 5000),
+                                   ("C5", 8, 100, args.c5_sites, 5000)):
             H = load(eng, P, spp, S, w)
             one_hot, packed = row_bytes(H)
             ms = {k: [] for k in PASS_ENV}
