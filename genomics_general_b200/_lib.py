@@ -88,8 +88,10 @@ _SIGS = {
     "pg_debug_k1_plan": (C.c_int, [C.c_int64, C.c_int32] + [C.POINTER(C.c_int32)] * 5),
     "pg_debug_k1_plan_ex": (C.c_int, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32)]),
     "pg_debug_packed": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int32), C.c_void_p]),
+    "pg_debug_site_cls": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_int32), C.c_void_p]),
     "pg_debug_uniform": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
     "pg_debug_uniform_tile": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
+    "pg_debug_uniform_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "pg_debug_uniform_ring": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "pg_debug_uniform_tiles": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int32)]),

@@ -290,7 +290,7 @@ int pg_k1_ring_stages(int tile_bytes, int table_bytes) {
     return std::min(stages, std::max(2, env_int("PG_K1_STAGES", stages)));
 }
 
-K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G, int code_bytes) {
+K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G) {
     K1Plan p;
     memset(&p, 0, sizeof(p));
     p.pitch = pitch;
@@ -321,9 +321,8 @@ K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes,
     p.wpt = wpt;
     p.nw = nw;
     p.T = (32 * wpt / G) * I;
-    // genotype rows + the tile's positions (+ code_bytes per site for its codes, in arrays of 2 bytes per site padded to
-    // 16-byte pieces)
-    p.tile_bytes = ((p.T * p.pitch + p.T * 4 + code_bytes * ((p.T + 7) / 8 * 8) + 127) / 128) * 128;
+    // genotype rows + the tile's positions
+    p.tile_bytes = ((p.T * p.pitch + p.T * 4 + 127) / 128) * 128;
     p.stages = pg_k1_ring_stages(p.tile_bytes, table_bytes);   // < 2 means the row is too long for this kernel
     p.smem_bytes = p.stages * p.tile_bytes + 256 + table_bytes;
     p.num_tiles = (S + p.T - 1) / p.T;
@@ -593,8 +592,9 @@ __global__ void __launch_bounds__(256) k_pack_rows(const uint8_t* __restrict__ g
     for (int64_t r = row0 + (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5); r < row0 + n; r += nwarps) {
         const uint8_t* src = geno + r * pitch;
         uint32_t* dst = packed + r * ppw;
-        // warp-uniform: some haplotype valid / missing, some valid code bit 0 (1) set / clear
+        // warp-uniform: some haplotype valid / missing, some valid code bit 0 (1) set / clear; alleles present (bit a: code a)
         bool any_v = false, any_m = false, any_b0 = false, any_nb0 = false, any_b1 = false, any_nb1 = false;
+        uint32_t present = 0u;
         for (int w0 = 0; w0 < wd; w0 += 32) {
             const int ng = min(8, (wd - w0 + 3) / 4);       // 128-haplotype groups in this stretch (warp-uniform)
             uint32_t v[8];
@@ -623,6 +623,8 @@ __global__ void __launch_bounds__(256) k_pack_rows(const uint8_t* __restrict__ g
                     any_nb0 |= (bv & ~b0) != 0u;
                     any_b1 |= b1 != 0u;
                     any_nb1 |= (bv & ~b1) != 0u;
+                    present |= ((bv & ~b0 & ~b1) != 0u ? 1u : 0u) | ((bv & b0 & ~b1) != 0u ? 2u : 0u) |
+                               ((bv & ~b0 & b1) != 0u ? 4u : 0u) | ((bv & b0 & b1) != 0u ? 8u : 0u);
                     if (lane == 4 * j + k) {
                         V = bv;
                         B0 = b0;
@@ -642,6 +644,8 @@ __global__ void __launch_bounds__(256) k_pack_rows(const uint8_t* __restrict__ g
             if (!any_v) c = PG_CLS_MISSING;
             else if (!any_m && !(any_b0 && any_nb0) && !(any_b1 && any_nb1))
                 c = (uint8_t)(PG_CLS_A + (any_b0 ? 1 : 0) + (any_b1 ? 2 : 0));
+            else if (!any_m && __popc(present) == 2)
+                c = (any_b1 && any_nb1) ? PG_CLS_VARIED2_B1 : PG_CLS_VARIED2;
             cls[r] = c;
         }
     }
@@ -666,6 +670,18 @@ extern "C" int pg_debug_packed(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* r
     PG_CUDA(cudaSetDevice(ctx->device));
     PG_CUDA(cudaMemcpyAsync(out, (const uint8_t*)ctx->d_packed + site0 * ctx->packed_pitch, (size_t)n * ctx->packed_pitch,
                             cudaMemcpyDeviceToHost, ctx->stream));
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    return PG_OK;
+}
+
+// the class bytes (PG_CLS_*) of sites [site0, site0 + n); *avail = 0 when the context keeps none
+extern "C" int pg_debug_site_cls(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* avail, uint8_t* out) {
+    PG_CHECK(ctx && avail, "pg_debug_site_cls: null argument");
+    PG_CHECK(site0 >= 0 && n >= 0 && site0 + n <= ctx->S, "pg_debug_site_cls: range outside S");
+    *avail = ctx->d_site_cls ? 1 : 0;
+    if (!ctx->d_site_cls || !out || n == 0) return PG_OK;
+    PG_CUDA(cudaSetDevice(ctx->device));
+    PG_CUDA(cudaMemcpyAsync(out, ctx->d_site_cls + site0, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
     return PG_OK;
 }

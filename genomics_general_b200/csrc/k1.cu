@@ -44,16 +44,16 @@ struct K1Params {
     // packed popgen pass: (word, mask) entries of the populations (ent_lo / ent_hi index them), words per plane
     const uint2* word_ent;
     int wd;
-    // packed pass with uniform sites elided (UniformStream): geno holds only the varied rows, tile t's being rows
-    // [row0[t], row0[t + 1]); codes holds tile t's 16-bit codes, one per site, at t * 2 * code_pitch, and code_pitch further
-    // the site index in the tile (slot) of each of its varied rows; uni_gv > 0 forces the lanes per varied row (PG_K1_UNI_GV).
-    // Tile t covers the sites [site_lo[t], site_lo[t + 1]): at most T (Tmax) of them and at most row_cap (R) varied rows.  A
-    // stage holds row_cap rows, then the positions from the tile's first site rounded down to 4 (T + 4 of them), then its
-    // codes and slots.
+    // packed pass with uniform sites elided (UniformStream): geno holds only the varied rows.  Tile t covers the sites
+    // [site_lo[t], site_lo[t + 1]) (at most T = Tmax of them), holds the varied rows [row0[t], row0[t + 1]) (at most row_cap = R)
+    // of which n1[t] are one-plane rows, and its rows are the words [woff[t], woff[t + 1]) of geno; slots holds, at t * T,
+    // the site index in the tile (slot) of each of its rows.  A stage holds the tile's rows (room for row_cap three-plane
+    // rows), then their slots.  uni_gv > 0 forces the lanes per varied row (PG_K1_UNI_GV).
     const int64_t* row0;
     const int64_t* site_lo;
-    const uint16_t* codes;
-    int code_pitch;
+    const int64_t* woff;
+    const int32_t* n1;
+    const uint16_t* slots;
     int uni_gv;
     int row_cap;
     // segments / slots
@@ -369,58 +369,58 @@ __device__ __forceinline__ void k1_producer(const K1Params& prm, uint8_t* tiles,
     }
 }
 
-// Producer of the packed pass over the varied rows only (the whole producer warp): a tile is its varied rows
-// [row0[t], row0[t + 1]) (room for row_cap of them), then the positions of its sites [site_lo[t], site_lo[t + 1]) from the first
-// one rounded down to a multiple of 4 (bulk copies take 16-byte-aligned sources; the consumers apply the offset), then its
-// codes (code_pitch of them) and the slots of its varied rows.  The
-// tile's first site goes to s_site0[stage], and its varied rows and sites to s_nvar[stage] (nvar | nsites << 16; R < 2^15,
-// Tmax <= 2^15), before the stage is armed, so the mbarrier's phase publishes them.  A tile is
-// about a microsecond of HBM time, as long as a dependent load of row0, so the 32 lanes load the offsets of the next 32 tiles
-// while the current 32 are issued.
+// Producer of the packed pass over the varied rows only (the whole producer warp): a stage is the tile's rows, the words
+// [woff[t], woff[t + 1]) of the stream (room for row_cap three-plane rows), then the slots of its rows.  The tile's first site
+// goes to s_site0[stage], and its one-plane and three-plane row counts to s_nvar[stage] (n1 | n3 << 16; R < 2^15), before the
+// stage is armed, so the mbarrier's phase publishes them.  A tile is about a microsecond of HBM time, as long as a dependent
+// load of its offsets, so the 32 lanes load the offsets of the next 32 tiles while the current 32 are issued.
 __device__ __forceinline__ void k1_producer_uniform(const K1Params& prm, uint8_t* tiles, uint64_t* full, uint64_t* empty,
                                                     volatile int* s_issued, volatile uint32_t* s_nvar,
                                                     volatile long long* s_site0, int ntiles, int64_t t0, int lane) {
-    auto ld_row0 = [&](int64_t t) { return t <= prm.num_tiles ? __ldg(prm.row0 + t) : (int64_t)0; };
-    auto ld_site = [&](int64_t t) { return t <= prm.num_tiles ? __ldg(prm.site_lo + t) : (int64_t)0; };
-    int64_t cur = ld_row0(t0 + lane), cur_s = ld_site(t0 + lane);       // lane l: row0 and site_lo of tile t0 + g + l
+    auto ld = [&](const int64_t* a, int64_t t) { return t <= prm.num_tiles ? __ldg(a + t) : (int64_t)0; };
+    auto ld_n1 = [&](int64_t t) { return t < prm.num_tiles ? __ldg(prm.n1 + t) : 0; };
+    // lane l: row0, woff, site_lo and n1 of tile t0 + g + l
+    int64_t cur = ld(prm.row0, t0 + lane), cur_w = ld(prm.woff, t0 + lane), cur_s = ld(prm.site_lo, t0 + lane);
+    int cur_n1 = ld_n1(t0 + lane);
     for (int g = 0; g < ntiles; g += 32) {
-        const int64_t nxt = ld_row0(t0 + g + 32 + lane), nxt_s = ld_site(t0 + g + 32 + lane);
+        const int64_t nt = t0 + g + 32 + lane;
+        const int64_t nxt = ld(prm.row0, nt), nxt_w = ld(prm.woff, nt), nxt_s = ld(prm.site_lo, nt);
+        const int nxt_n1 = ld_n1(nt);
         const int kn = min(32, ntiles - g);
         for (int k = 0; k < kn; ++k) {
             const int64_t r0 = __shfl_sync(0xffffffffu, cur, k);
             const int64_t r1 = k < 31 ? __shfl_sync(0xffffffffu, cur, k + 1) : __shfl_sync(0xffffffffu, nxt, 0);
+            const int64_t w0 = __shfl_sync(0xffffffffu, cur_w, k);
+            const int64_t w1 = k < 31 ? __shfl_sync(0xffffffffu, cur_w, k + 1) : __shfl_sync(0xffffffffu, nxt_w, 0);
             const int64_t s0 = __shfl_sync(0xffffffffu, cur_s, k);
-            const int64_t s1 = k < 31 ? __shfl_sync(0xffffffffu, cur_s, k + 1) : __shfl_sync(0xffffffffu, nxt_s, 0);
+            const int n1 = __shfl_sync(0xffffffffu, cur_n1, k);
             if (lane == 0) {
                 const int it = g + k;
                 const int stage = it % prm.stages;
                 if (it >= prm.stages) mbar_wait(&empty[stage], (uint32_t)(((it / prm.stages) - 1) & 1));
                 const int64_t tile = t0 + it;
-                const int64_t s_lo = s0 & ~(int64_t)3;
-                const int64_t rows = s1 - s_lo;
                 const int nvar = (int)(r1 - r0);
-                const uint32_t bytes = (uint32_t)(nvar * prm.pitch);
-                const uint32_t pbytes = (uint32_t)(((rows * 4 + 15) / 16) * 16);
-                const uint32_t cbytes = (uint32_t)(prm.code_pitch * 2 + ((nvar * 2 + 15) / 16) * 16);
-                s_nvar[stage] = (uint32_t)nvar | (uint32_t)(s1 - s0) << 16;
+                const uint32_t bytes = (uint32_t)((w1 - w0) * 4);
+                const uint32_t sbytes = (uint32_t)(((nvar * 2 + 15) / 16) * 16);
+                s_nvar[stage] = (uint32_t)n1 | (uint32_t)(nvar - n1) << 16;
                 s_site0[stage] = s0;
-                mbar_expect_tx(&full[stage], bytes + pbytes + cbytes);
-                const uint8_t* src = prm.geno + r0 * prm.pitch;
+                mbar_expect_tx(&full[stage], bytes + sbytes);
+                const uint8_t* src = prm.geno + w0 * 4;
                 uint8_t* dst = tiles + (size_t)stage * prm.tile_bytes;
                 for (uint32_t off = 0; off < bytes; off += 32768u) {
                     const uint32_t n = (bytes - off) < 32768u ? (bytes - off) : 32768u;
                     bulk_g2s(dst + off, src + off, n, &full[stage]);
                 }
-                const size_t pos_off = (size_t)prm.row_cap * prm.pitch;
-                bulk_g2s(dst + pos_off, prm.pos + s_lo, pbytes, &full[stage]);
-                bulk_g2s(dst + pos_off + (size_t)(prm.T + 4) * 4, prm.codes + tile * 2 * prm.code_pitch, cbytes, &full[stage]);
+                if (sbytes) bulk_g2s(dst + (size_t)prm.row_cap * prm.pitch, prm.slots + tile * prm.T, sbytes, &full[stage]);
                 __threadfence_block();
                 atomicExch(const_cast<int*>(s_issued), it + 1);
             }
             __syncwarp();
         }
         cur = nxt;
+        cur_w = nxt_w;
         cur_s = nxt_s;
+        cur_n1 = nxt_n1;
     }
 }
 
@@ -940,18 +940,15 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
 // Tiles and the ring are k1_site_pass's too, over rows of prm.pitch = packed bytes.  Rows start on 16-byte boundaries, so
 // the 32 lanes of a warp reading the same word of their own rows meet in at most 8 banks: each lane starts its walk over a
 // population's entries at an offset taken from its site index, which spreads the reads over the banks.
-// UNI: the tiles hold only the varied rows (k1_producer_uniform), a code per site (UNI_CODE | PG_CLS_* for a site whose H
-// haplotypes all carry one allele or are all missing, else its rank among the tile's varied sites) and the slot of each varied
-// row (its site's index in the tile; T <= 2048).  A tile's varied rows are stored word-major: word x of its row j at word
-// x * nvar + j of the tile, so that the lanes reading the same word of consecutive rows read consecutive words, in
-// distinct banks whatever the pitch.  A team then makes two passes over a tile.  Pass V packs the varied rows onto
-// the team's lanes, Gv lanes per row: the plan's lanes per site (1 at C2 and C5, where more measured slower; 2 for rows of
-// 1 KiB and more; PG_K1_UNI_GV forces 1 .. 32 for the tests), so that a warp walks only when it holds varied rows, and those
-// fill its lanes.  Pass U runs one lane per slot:
-// it adds every site's position, and counts the uniform sites that are not missing, whose sums follow from the population
-// sizes (n_X = c_Xa = N_X: N_X^2 and N_X N_Y per site) and are added at its flush (uniform_flush).  Either pass keeps its own
-// segment and flushes into the warp's slots, which add, so the slots end with the same integers.
-constexpr uint32_t UNI_CODE = 0x8000u;
+// UNI: the tiles hold only the varied rows (k1_producer_uniform) and the slot of each (its site's index in the tile;
+// Tmax <= 32768).  A complete biallelic row (PG_CLS_VARIED2*: every haplotype called, two alleles) is one plane of wd words,
+// "carries the higher of the two codes"; any other varied row is the three planes.  A tile stores its one-plane rows, then its
+// three-plane rows, each kind word-major: word x of its row j at word x * n + j of the kind's run (n rows of the kind), so
+// that the lanes reading the same word of consecutive rows read consecutive words, in distinct banks whatever the pitch.  A
+// team packs the rows onto its lanes, Gv lanes per row: the plan's lanes per site (1 at C2 and C5, where more measured
+// slower; 2 for rows of 1 KiB and more; PG_K1_UNI_GV forces 1 .. 32 for the tests), in blocks of 32 / Gv rows, the
+// one-plane rows' blocks, then the three-plane rows', block k to warp (k + tile) % wpt.  The uniform sites and every site's
+// position are not streamed: k1_finalize adds them from per-site prefix sums (UniformStream::pre).
 
 // this lane's entries of population X: the first one, then steps of G (wrapping inside the population), as many as
 // walk[X] >> 16 (first | count << 16: the table holds < 6144 entries).  The G lanes of a site (gsub = 0 .. G - 1) share the
@@ -1061,6 +1058,33 @@ __device__ __forceinline__ void varied_counts(const K1Params& prm, const uint2* 
     }
 }
 
+// A complete biallelic row's counts: every haplotype of population X is present, k(X) of them carry the higher code.
+template <int P>
+struct BitCounts {
+    uint32_t k[P];
+    const int* N;
+    __device__ __forceinline__ void set(int X, uint32_t kx) { k[X] = kx; }
+    __device__ __forceinline__ uint32_t n(int X) const { return (uint32_t)N[X]; }
+    __device__ __forceinline__ uint32_t c(int X, int a) const { return a == 0 ? (uint32_t)N[X] - k[X] : (a == 1 ? k[X] : 0u); }
+};
+
+// varied_counts for a one-plane row (word x at row[x * nvar]): one load, one AND, one POPC per entry
+template <int P, bool ONE>
+__device__ __forceinline__ void varied_bits(const K1Params& prm, const uint2* s_ent, const uint32_t* row, int nvar, int Gv,
+                                            int gsub, int spv, BitCounts<P>& ct) {
+#pragma unroll
+    for (int X = 0; X < P; ++X) {
+        uint32_t a = 0u;
+#pragma unroll 1
+        for (int e = prm.ent_lo[X] + (ONE ? 0 : gsub); e < prm.ent_hi[X]; e += (ONE ? 1 : Gv)) {
+            const uint2 em = s_ent[e];
+            a += __popc(row[em.x * nvar] & em.y);
+        }
+        for (int d = spv; !ONE && d < 32; d <<= 1) a += __shfl_xor_sync(0xffffffffu, a, d);
+        ct.set(X, a);
+    }
+}
+
 // whether the site (of the lane that owns it) has every haplotype of every population, or some but not all of them
 template <int P, class CT>
 __device__ __forceinline__ void packed_class(const K1Params& prm, bool owner, const CT& ct, bool& pres, bool& ragged) {
@@ -1097,50 +1121,6 @@ __device__ __forceinline__ void packed_add(ACC& acc, bool pres, bool ragged, con
         }
 }
 
-// Pass U's state, one per consumer warp in shared memory behind the entry table, so that it holds no register while pass V
-// walks: its segment (warp-uniform) and the segment's end, and the positions and the uniform non-missing sites it has added
-// since its last flush.
-struct UniRec {
-    long long pos;
-    long long seg_end;
-    int seg;
-    uint32_t npres;
-};
-constexpr int UNI_SMEM_BYTES = K1_MAX_WARPS * (int)sizeof(UniRec);
-
-// the exact sum of the 32 lanes' v, from 32-bit reductions of its 16-bit halves
-__device__ __forceinline__ long long warp_sum_i32(int v) {
-    const uint32_t u = (uint32_t)v;
-    const long long lo = __reduce_add_sync(0xffffffffu, u & 0xffffu), hi = __reduce_add_sync(0xffffffffu, u >> 16);
-    const int neg = __popc(__ballot_sync(0xffffffffu, v < 0));
-    return lo + (hi << 16) - ((long long)neg << 32);
-}
-
-// Pass U's flush (the whole warp, the same values in every lane): into this warp's slot of segment seg, the positions, the
-// uniform non-missing sites, and the sums those sites add (N_X^2 per population, N_X N_Y per pair), in 64 bits; lane q adds
-// word q, so the read-modify-writes go out together.
-template <int MODE, int P>
-__device__ __forceinline__ void uniform_flush(const K1Params& prm, int seg, long long np, long long pos, int64_t slot_base,
-                                              int seg_first, int warp, int lane, int nw) {
-    constexpr int QI = ModeTraits<MODE, P>::QI, Q = QI + ModeTraits<MODE, P>::QU, NQ = QI + P + P * (P - 1) / 2;
-    unsigned long long* dst = prm.part + slot_base + ((int64_t)(seg - seg_first) * nw + warp) * Q;
-#pragma unroll
-    for (int q0 = 0; q0 < NQ; q0 += 32) {
-        const int q = q0 + lane;
-        long long v = q == 0 ? np : (q == 2 ? pos : 0ll);
-        if (q >= QI && q < NQ) {       // population X = Y, then the pairs (X, Y > X) in order
-            int X = q - QI, Y = X;
-            if (X >= P) {
-                int k = X - P, left = P - 1;
-                for (X = 0; k >= left; ++X, --left) k -= left;
-                Y = X + 1 + k;
-            }
-            v = np * (long long)prm.popN[X] * (long long)prm.popN[Y];
-        }
-        if (q < NQ && q != 1) dst[q] += (unsigned long long)v;
-    }
-}
-
 template <int MODE, int P, int NW, bool UNI = false>
 __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __grid_constant__ K1Params prm) {
     static_assert(MODE == MODE_POPGEN || MODE == MODE_POPGEN_FREQ, "packed site pass: popgen modes");
@@ -1151,7 +1131,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)prm.stages * prm.tile_bytes);   // [stages]
     uint64_t* empty = full + 8;                                                                  // [stages]
     volatile int* s_issued = reinterpret_cast<volatile int*>(empty + 8);
-    volatile uint32_t* s_nvar = reinterpret_cast<volatile uint32_t*>(s_issued + 8);   // UNI: nvar | nsites << 16 [stages]
+    volatile uint32_t* s_nvar = reinterpret_cast<volatile uint32_t*>(s_issued + 8);   // UNI: n1 | n3 << 16 [stages]
     volatile long long* s_site0 = reinterpret_cast<volatile long long*>(s_issued + 16);   // UNI: first site [stages]
     uint2* s_ent = reinterpret_cast<uint2*>(smem + (size_t)prm.stages * prm.tile_bytes + 256);
 
@@ -1161,9 +1141,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     const int ntiles = (int)(t1 - t0);
 
     for (int e = tid; e < prm.n_ent; e += K1_THREADS) s_ent[e] = prm.word_ent[e];
-    UniRec* s_urec = reinterpret_cast<UniRec*>(s_ent + prm.n_ent);          // UNI: [NW] pass U records
     const int Gv = prm.uni_gv > 0 ? prm.uni_gv : prm.G;                    // UNI: lanes per varied row, the plan's per site
-    if (UNI && warp < NW && lane == 0) s_urec[warp] = UniRec{0ll, -1ll, -1, 0u};
     if (tid == 0) {
         for (int s = 0; s < prm.stages; ++s) {
             mbar_init(&full[s], 1);
@@ -1250,8 +1228,34 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             if (lane == 0) mbar_arrive(&empty[stage]);
         }
     } else {
-        const size_t pos_off = (size_t)prm.row_cap * prm.pitch, codes_off = pos_off + (size_t)(prm.T + 4) * 4;
-        const int spv = 32 / Gv, gsub = lane / spv, sl = lane % spv;
+        const int spv = 32 / Gv, gsub = lane / spv, sl = lane % spv, wpt = prm.wpt;
+        // One row's sums, its segment first.  A lane's rows come in site order within each kind, so only the three-plane
+        // rows (back) may lie before the lane's segment: the one-plane rows of the same tile may have moved it on.
+        auto add_row = [&](int64_t site, bool owner, const auto& ct, bool back) {
+            int sg = cur_seg;
+            if (owner && site >= seg_end) sg = next_seg(prm.brk, prm.nseg, cur_seg + 1, site);
+            else if (back && owner && site < __ldg(prm.brk + cur_seg)) sg = find_seg(prm.brk, cur_seg, 0, site);
+            if (__any_sync(0xffffffffu, sg != cur_seg)) {
+                warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+                since_flush = 0;
+                // A lane that owns no row here (a row's other lanes, lanes past the block) would keep an old segment
+                // and flush the warp once more when it next owns one.  Its sums are zero now, so it takes the warp's last
+                // segment, which no later row of it lies before but for a three-plane row, which searches back.
+                const int last = __reduce_max_sync(0xffffffffu, sg);
+                const int to = owner ? sg : last;
+                if (to != cur_seg) {
+                    cur_seg = to;
+                    seg_end = __ldg(prm.brk + to + 1);
+                }
+            }
+            bool pres, ragged;
+            packed_class<P>(prm, owner, ct, pres, ragged);
+            if (++since_flush > prm.acc_limit) {      // the 32-bit sums must not overflow
+                warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
+                since_flush = 1;
+            }
+            packed_add<MODE, P>(acc, pres, ragged, ct);
+        };
 
         for (int it = team; it < ntiles; it += nteams) {
             const int stage = it % prm.stages;
@@ -1262,95 +1266,42 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             const uint8_t* tile = tiles + (size_t)stage * prm.tile_bytes;
             const int64_t tile_site0 = s_site0[stage];
             const uint32_t sizes = s_nvar[stage];
-            const int nvar = (int)(sizes & 0xffffu), nsites = (int)(sizes >> 16);
-            const int32_t* s_pos = reinterpret_cast<const int32_t*>(tile + pos_off) + (tile_site0 & 3);
-            const uint16_t* s_slot = reinterpret_cast<const uint16_t*>(tile + codes_off) + prm.code_pitch;
+            const int n1 = (int)(sizes & 0xffffu), n3 = (int)(sizes >> 16);
+            const uint16_t* s_slot = reinterpret_cast<const uint16_t*>(tile + (size_t)prm.row_cap * prm.pitch);
+            // block k of the tile goes to warp (k + rot) % wpt: the one-plane rows' blocks first, then the three-plane rows'
+            const int rot = (int)((t0 + it) % wpt), nb1 = (n1 + spv - 1) / spv;
 
-            // ---- pass V: blocks of spv varied rows, block k to warp k % wpt, so a lane's rows stay in site order ----
-            for (int r = lw * spv; r < nvar; r += prm.wpt * spv) {
+            // ---- one-plane rows (none at 8 populations: uniform_prepare streams three planes there) ----
+            for (int r = ((lw - rot + wpt) % wpt) * spv; P < 8 && r < n1; r += wpt * spv) {
                 const int rw = r + sl;
-                const bool valid = rw < nvar;
+                const bool valid = rw < n1;
                 const bool owner = valid && (gsub == 0);
                 const uint32_t* row = reinterpret_cast<const uint32_t*>(tile) + (valid ? rw : r);
+                BitCounts<P> ct;
+                ct.N = prm.popN;
+                if (Gv == 1) varied_bits<P, true>(prm, s_ent, row, n1, 1, 0, 32, ct);
+                else varied_bits<P, false>(prm, s_ent, row, n1, Gv, gsub, spv, ct);
+                add_row(tile_site0 + (valid ? s_slot[rw] : 0), owner, ct, false);
+            }
+
+            // ---- three-plane rows, behind the one-plane rows' words rounded up to 16 bytes ----
+            const uint32_t* rows3 = reinterpret_cast<const uint32_t*>(tile) + ((n1 * prm.wd + 3) & ~3);
+            for (int r = ((lw - rot - nb1 % wpt + 2 * wpt) % wpt) * spv; r < n3; r += wpt * spv) {
+                const int rw = r + sl;
+                const bool valid = rw < n3;
+                const bool owner = valid && (gsub == 0);
+                const uint32_t* row = rows3 + (valid ? rw : r);
                 // with 8 populations the counts are expanded once; with fewer they stay two words per population (the
                 // choices with the fewest spills, ptxas sm_90a)
                 std::conditional_t<P == 8, ArrCounts<P>, PkCounts<P>> ct;
-                if (P < 8 && Gv == 1) varied_counts<P, true>(prm, s_ent, row, nvar, 1, 0, 32, ct);
-                else varied_counts<P, false>(prm, s_ent, row, nvar, Gv, gsub, spv, ct);
-
-                const int64_t site = tile_site0 + (valid ? s_slot[rw] : 0);
-                int sg = cur_seg;
-                if (owner && site >= seg_end) sg = next_seg(prm.brk, prm.nseg, cur_seg + 1, site);
-                if (__any_sync(0xffffffffu, sg != cur_seg)) {
-                    warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
-                    since_flush = 0;
-                    // A lane that owns no row here (a row's other lanes, lanes past the block) would keep an old segment
-                    // and flush the warp once more when it next owns one.  Its sums are zero now and none of its later
-                    // sites comes before the warp's sites here, so it takes the warp's last segment.
-                    const int last = __reduce_max_sync(0xffffffffu, sg);
-                    const int to = owner ? sg : last;
-                    if (to != cur_seg) {
-                        cur_seg = to;
-                        seg_end = __ldg(prm.brk + to + 1);
-                    }
-                }
-                bool pres, ragged;
-                packed_class<P>(prm, owner, ct, pres, ragged);
-                if (++since_flush > prm.acc_limit) {      // the 32-bit sums must not overflow
-                    warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
-                    since_flush = 1;
-                }
-                packed_add<MODE, P>(acc, pres, ragged, ct);
+                if (P < 8 && Gv == 1) varied_counts<P, true>(prm, s_ent, row, n3, 1, 0, 32, ct);
+                else varied_counts<P, false>(prm, s_ent, row, n3, Gv, gsub, spv, ct);
+                add_row(tile_site0 + (valid ? s_slot[n1 + rw] : 0), owner, ct, true);
             }
 
-            // ---- pass U: every slot of the tile, 32 per iteration, one lane each, no walk.  The warps that walked no row take
-            // the iterations when they are at most two each, the whole team otherwise.  The lanes of an iteration hold
-            // increasing sites, so those before the warp's segment end are a prefix of them ----
-            const int vw = min(prm.wpt, (nvar + spv - 1) / spv), nit = (nsites + 31) / 32;
-            const bool idle_only = vw < prm.wpt && nit <= 2 * (prm.wpt - vw);
-            const uint16_t* s_code = reinterpret_cast<const uint16_t*>(tile + codes_off);
-            const int uw = idle_only ? prm.wpt - vw : prm.wpt, ul = idle_only ? lw - vw : lw;
-            UniRec& ur = s_urec[warp];
-            int useg = ur.seg;
-            int64_t useg_end = ur.seg_end;
-            long long upos = ur.pos;
-            uint32_t upres = ur.npres;
-            for (int j0 = ul * 32; ul >= 0 && j0 < nsites; j0 += uw * 32) {
-                const int j = j0 + lane;
-                const int64_t site = tile_site0 + j;
-                const bool valid = j < nsites;
-                uint32_t code = UNI_CODE | PG_CLS_MISSING;
-                int posv = 0;
-                if (valid) {
-                    code = s_code[j];
-                    posv = s_pos[j];
-                }
-                const unsigned up = __ballot_sync(0xffffffffu, (code & UNI_CODE) && (code & 7u) != PG_CLS_MISSING);
-                unsigned left = __ballot_sync(0xffffffffu, valid);
-                while (true) {
-                    const unsigned in = __ballot_sync(0xffffffffu, site < useg_end) & left;
-                    upres += __popc(up & in);
-                    upos += warp_sum_i32((in >> lane) & 1u ? posv : 0);
-                    left &= ~in;
-                    if (!left) break;
-                    if (useg >= 0) {
-                        uniform_flush<MODE, P>(prm, useg, upres, upos, slot_base, seg_first, warp, lane, NW);
-                        upres = 0u;
-                        upos = 0ll;
-                    }
-                    useg = next_seg(prm.brk, prm.nseg, useg + 1, __shfl_sync(0xffffffffu, site, __ffs(left) - 1));
-                    useg_end = __ldg(prm.brk + useg + 1);
-                }
-            }
             __syncwarp();
-            if (lane == 0) {
-                ur = UniRec{upos, useg_end, useg, upres};
-                mbar_arrive(&empty[stage]);
-            }
+            if (lane == 0) mbar_arrive(&empty[stage]);
         }
-        __syncwarp();
-        const UniRec ur = s_urec[warp];
-        if (ur.seg >= 0) uniform_flush<MODE, P>(prm, ur.seg, ur.npres, ur.pos, slot_base, seg_first, warp, lane, NW);
     }
     warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
 }
@@ -1377,6 +1328,11 @@ struct FinParams {
     int force_path;
     int with_freq;                 // the site pass carried the popFreq counters
     int bookkeeping_only;          // P > 8: the site pass saw one collapsed population; statistics come from K2
+    // popgen over the varied-row stream: exclusive per-site prefixes of the positions and of the uniform non-missing sites
+    // (nullptr: the site pass added every site itself), S sites
+    const int64_t* pre_pos;
+    const int64_t* pre_uni;
+    int64_t S;
     // outputs: fixed-width 8-byte records per window
     //   popgen: [sites(i64) pos_sum(i64) path(i64) pi[P] dxy[npairs] fst[npairs]]
     //   abba  : [sites(i64) pos_sum(i64) ABBA BABA D fd fdM sitesUsed]
@@ -1419,6 +1375,24 @@ __global__ void __launch_bounds__(64) k1_finalize(const __grid_constant__ FinPar
                         const unsigned long long v = src[wp * fp.Q + q];
                         if (q < fp.QI) si += (long long)v; else sd += __longlong_as_double((long long)v);
                     }
+                }
+            }
+            if (MODE == MODE_POPGEN && fp.pre_uni) {
+                // the window's positions, and what its uniform non-missing sites add: 1 to the complete sites, and per
+                // site N_X^2 to sum c_Xa^2 and N_X N_Y to sum c_Xa c_Ya (population X = Y, then the pairs X < Y in order)
+                const int64_t lo = min(max(fp.win_lo[w], (int64_t)0), fp.S), hi = min(max(fp.win_hi[w], lo), fp.S);
+                const long long u = fp.pre_uni[hi] - fp.pre_uni[lo];
+                const int Pp = fp.Ppad;
+                if (q == 0) si += u;
+                else if (q == 2) si += fp.pre_pos[hi] - fp.pre_pos[lo];
+                else if (q >= 3 && q < 3 + Pp + Pp * (Pp - 1) / 2) {
+                    int X = q - 3, Y = X;
+                    if (X >= Pp) {
+                        int k = X - Pp, left = Pp - 1;
+                        for (X = 0; k >= left; ++X, --left) k -= left;
+                        Y = X + 1 + k;
+                    }
+                    si += u * (long long)fp.popN[X] * (long long)fp.popN[Y];
                 }
             }
             sums[q] = (q < fp.QI) ? (unsigned long long)si : (unsigned long long)__double_as_longlong(sd);
@@ -1729,105 +1703,165 @@ int push(pg_ctx* ctx, uint8_t* base, size_t& off, const T* src, size_t n, T** ou
 }
 
 // ---- the packed rows of the varied sites only (DESIGN.md "Uniform sites") -------------------------------------------
-// Derived from the companion and its site classes (ctx->d_site_cls) for one data generation, row budget R and tile bound
-// Tmax.  Tiles are cut by a budget of varied rows: group k holds the varied rows of ranks [k R, (k + 1) R) and runs from the
-// site of rank k R (site 0 for k = 0) to the next group's; a group of more than Tmax sites is split into pieces of Tmax.  So a
-// tile has at most R varied rows and at most Tmax sites, and tile t covers the sites [site_lo[t], site_lo[t + 1]).  Per tile:
-// the index of its first varied row (row0, int64 [tiles + 1]), a 16-bit code per site (UNI_CODE | class, or the rank among the
-// tile's varied sites; tile t's codes at t * 2 * code_pitch, code_pitch = Tmax), the slot (index in the tile) of each of its
-// varied rows, behind its codes; and the varied rows, each tile's contiguous and word-major (k1_uni_codes).  bound holds the first site of each CTA's tiles (B + 1).
+// Derived from the companion and its site classes (ctx->d_site_cls) for one data generation, row budget R, tile bound Tmax
+// and row kinds (bits: complete biallelic rows as one plane).  Tiles are cut by a budget of varied rows: group k holds the
+// varied rows of ranks [k R, (k + 1) R) and runs from the site of rank k R (site 0 for k = 0) to the next group's; a group of
+// more than Tmax sites is split into pieces of Tmax (the slots are 16 bits).  So a tile has at most R varied rows and at most
+// Tmax sites, and tile t covers the sites [site_lo[t], site_lo[t + 1]).  Per tile: the index of its first varied row (row0,
+// int64 [tiles + 1]), its one-plane rows (n1, int32 [tiles]), its first word in the stream (woff, int64 [tiles + 1]: a tile's
+// one-plane rows take n1 wd words rounded up to 4, its three-plane rows a packed row's words each), the slot (index in the
+// tile) of each of its rows at t * Tmax; and the rows (k1_uni_rows).  bound holds the first site of each CTA's tiles (B + 1).
+// pre holds the exclusive prefixes, over the S + 1 site bounds, of the positions and of the uniform non-missing sites, which
+// k1_finalize adds to each window in place of walking those sites.
 struct UniformStream {
     uint64_t gen = 0;         // ctx->data_gen it describes (0: none)
     uint64_t serial = 0;      // counts the builds (the slot tables follow it)
     int R = 0, Tmax = 0;
-    bool forced = false;
+    bool forced = false, bits = false, wb = false;
     bool in_use = false;      // false: too few uniform sites to pay off, or no memory; the packed pass streams every row
     int64_t varied = 0;
     int64_t nt = 0;           // tiles
-    int code_pitch = 0;
+    const int64_t* woff = nullptr;   // in words
     std::vector<int64_t> bound;
-    PgBuf cnt, row0, codes, src, rows, scan, site_lo, groups, info;
+    PgBuf cnt, row0, slots, src, rows, scan, site_lo, groups, info, words, n1, pre, wts, scan2;
     void release() {
-        for (PgBuf* b : {&cnt, &row0, &codes, &src, &rows, &scan, &site_lo, &groups, &info}) b->release();
+        for (PgBuf* b : {&cnt, &row0, &slots, &src, &rows, &scan, &site_lo, &groups, &info, &words, &n1, &pre, &wts, &scan2})
+            b->release();
         gen = 0;
     }
 };
 
-// varied sites per tile: tile t is [site_lo[t], site_lo[t + 1]), or the T sites from t * T when site_lo is null
+// whether a site of class c is streamed as one plane (bits: complete biallelic rows are)
+__device__ __forceinline__ bool uni_one_plane(uint32_t c, bool bits) { return bits && pg_cls_biallelic(c); }
+
+// varied sites per tile: tile t is [site_lo[t], site_lo[t + 1]), or the T sites from t * T when site_lo is null.  With wcnt,
+// also the tile's one-plane rows (n1) and the stream words of its rows (wcnt): wd words per one-plane row, rounded up to 4,
+// and pw per three-plane row.
 __global__ void __launch_bounds__(256) k1_uni_count(const uint8_t* __restrict__ cls, int64_t S, const int64_t* __restrict__ site_lo,
-                                                    int T, int64_t* __restrict__ cnt) {
-    __shared__ int s_n;
-    if (threadIdx.x == 0) s_n = 0;
+                                                    int T, int64_t* __restrict__ cnt, int64_t* __restrict__ wcnt = nullptr,
+                                                    int32_t* __restrict__ n1 = nullptr, int wd = 0, int pw = 0, bool bits = false) {
+    __shared__ int s_n, s_n1;
+    if (threadIdx.x == 0) s_n = s_n1 = 0;
     __syncthreads();
     const int64_t s0 = site_lo ? site_lo[blockIdx.x] : (int64_t)blockIdx.x * T;
     const int64_t len = site_lo ? site_lo[blockIdx.x + 1] - s0 : (S - s0 < T ? S - s0 : (int64_t)T);
-    int n = 0;
-    for (int j = threadIdx.x; j < len; j += blockDim.x)
-        if (cls[s0 + j] == PG_CLS_VARIED) ++n;
+    int n = 0, m = 0;
+    for (int j = threadIdx.x; j < len; j += blockDim.x) {
+        const uint32_t c = cls[s0 + j];
+        if (pg_cls_varied(c)) ++n;
+        if (uni_one_plane(c, bits)) ++m;
+    }
     n = __reduce_add_sync(0xffffffffu, n);
-    if ((threadIdx.x & 31) == 0) atomicAdd(&s_n, n);
+    m = __reduce_add_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0) {
+        atomicAdd(&s_n, n);
+        atomicAdd(&s_n1, m);
+    }
     __syncthreads();
-    if (threadIdx.x == 0) cnt[blockIdx.x] = s_n;
+    if (threadIdx.x == 0) {
+        cnt[blockIdx.x] = s_n;
+        if (wcnt) {
+            n1[blockIdx.x] = s_n1;
+            wcnt[blockIdx.x] = (int64_t)((s_n1 * wd + 3) & ~3) + (int64_t)(s_n - s_n1) * pw;
+        }
+    }
 }
 
-// codes of tile blockIdx.x (tiles as in k1_uni_count; none when codes is null), and the slot and the source site of each of its
-// varied rows.  With rows, the block then copies its nvar varied rows from the companion (chunks of 16 bytes per row) into
-// the stream, word-major: word x of its row j to word row0[t] * 4 * chunks + x * nvar + j.  A warp reads one chunk of 32
-// rows and writes each of its words as 32 consecutive words.
-__global__ void __launch_bounds__(256) k1_uni_codes(const uint8_t* __restrict__ cls, int64_t S, const int64_t* __restrict__ site_lo,
-                                                    int T, int code_pitch, const int64_t* __restrict__ row0,
-                                                    uint16_t* __restrict__ codes, int64_t* __restrict__ src,
-                                                    const uint4* __restrict__ packed = nullptr, int chunks = 0,
-                                                    uint32_t* __restrict__ rows = nullptr) {
+// The source site of each varied row of tile blockIdx.x (tiles as in k1_uni_count), in site order.  With slots (tiles of
+// site_lo), in the tile's row order instead: its one-plane rows, then its three-plane rows, each kind in site order, with
+// the slot of each; the block then copies the rows from the companion (ppw words per row) into the stream from word
+// woff[t], word-major: word x of one-plane row j (its plane B0 or B1, as the class says) to word x * n1 + j, then word x of
+// three-plane row j to word x * n3 + j of the run that starts at the one-plane rows' words rounded up to 4.
+__global__ void __launch_bounds__(256) k1_uni_rows(const uint8_t* __restrict__ cls, int64_t S, const int64_t* __restrict__ site_lo,
+                                                   int T, const int64_t* __restrict__ row0, int64_t* __restrict__ src,
+                                                   uint16_t* __restrict__ slots = nullptr, const int32_t* __restrict__ n1 = nullptr,
+                                                   const int64_t* __restrict__ woff = nullptr, const uint32_t* __restrict__ packed = nullptr,
+                                                   int ppw = 0, int wd = 0, bool bits = false, uint32_t* __restrict__ rows = nullptr) {
     typedef cub::BlockScan<int, 256> Scan;
     __shared__ typename Scan::TempStorage tmp;
     const int64_t t = blockIdx.x, r0 = row0[t];
     const int64_t s0 = site_lo ? site_lo[t] : t * T;
     const int64_t len = site_lo ? site_lo[t + 1] - s0 : (S - s0 < T ? S - s0 : (int64_t)T);
-    int base = 0;
-    for (int j0 = 0; j0 < code_pitch; j0 += 256) {
+    const int m1 = slots ? n1[t] : 0;
+    int base1 = 0, base3 = 0;
+    for (int j0 = 0; j0 < len; j0 += 256) {
         const int j = j0 + threadIdx.x;
         const int64_t s = s0 + j;
         const uint32_t k = j < len ? cls[s] : (uint32_t)PG_CLS_MISSING;
-        const int v = k == PG_CLS_VARIED ? 1 : 0;
+        // a row of either kind counts in the low half, a three-plane row in the high half too (< 256 each)
+        const int one = slots && uni_one_plane(k, bits) ? 1 : 0, var = pg_cls_varied(k) ? 1 : 0;
         int rank, total;
-        Scan(tmp).ExclusiveSum(v, rank, total);
+        Scan(tmp).ExclusiveSum(var | (var - one) << 16, rank, total);
         __syncthreads();
-        if (codes && j < code_pitch) codes[t * 2 * code_pitch + j] = (uint16_t)(v ? (uint32_t)(base + rank) : (UNI_CODE | k));
-        if (v) {
-            if (codes) codes[(t * 2 + 1) * code_pitch + base + rank] = (uint16_t)j;
-            src[r0 + base + rank] = s;
+        if (var) {
+            const int r3 = rank >> 16, r1 = (rank & 0xffff) - r3;
+            const int idx = !slots ? base1 + (rank & 0xffff) : (one ? base1 + r1 : m1 + base3 + r3);
+            if (slots) slots[t * T + idx] = (uint16_t)j;
+            src[r0 + idx] = s;
         }
-        base += total;
+        base1 += slots ? (total & 0xffff) - (total >> 16) : (total & 0xffff);
+        base3 += total >> 16;
     }
     if (!rows) return;
     __syncthreads();                          // the block's src entries, read back below
-    const int nvar = base, lane = threadIdx.x & 31;
-    uint32_t* dst = rows + r0 * 4 * chunks;
+    const int nvar = (int)(row0[t + 1] - r0), m3 = nvar - m1;
+    uint32_t* dst = rows + woff[t];
+    // a thread per row: the words a warp writes are consecutive, and each thread's reads stay in its row's sectors (a warp
+    // per row, its lanes over the words, took the C2 rebuild from 0.68 to 1.03 ms and C5's from 1.6 to 4.3, H100)
+    for (int j = threadIdx.x; j < m1; j += blockDim.x) {
+        const int64_t site = src[r0 + j];
+        const uint32_t* w = packed + site * ppw + (cls[site] == PG_CLS_VARIED2_B1 ? 2 : 1) * wd;
+        for (int x = 0; x < wd; ++x) dst[(int64_t)x * m1 + j] = w[x];
+    }
+    dst += (m1 * wd + 3) & ~3;
+    const int lane = threadIdx.x & 31, chunks = ppw / 4;
     for (int c = threadIdx.x >> 5; c < chunks; c += blockDim.x >> 5)
-        for (int j = lane; j < nvar; j += 32) {
-            const uint4 v = packed[src[r0 + j] * chunks + c];
-            uint32_t* d = dst + (int64_t)4 * c * nvar + j;
+        for (int j = lane; j < m3; j += 32) {
+            const uint4 v = reinterpret_cast<const uint4*>(packed)[src[r0 + m1 + j] * chunks + c];
+            uint32_t* d = dst + (int64_t)4 * c * m3 + j;
             d[0] = v.x;
-            d[nvar] = v.y;
-            d[2 * nvar] = v.z;
-            d[3 * nvar] = v.w;
+            d[m3] = v.y;
+            d[2 * m3] = v.z;
+            d[3 * m3] = v.w;
         }
 }
 
-// group k's first site (the site of varied rank k R; 0 for k = 0) and end (the next group's first site; S for the last)
-__device__ __forceinline__ void uni_group(const int64_t* src, int R, int64_t S, int64_t ng, int64_t k, int64_t& lo, int64_t& hi) {
-    lo = k == 0 ? 0 : src[k * R];
-    hi = k + 1 < ng ? src[(k + 1) * R] : S;
+// the uniform non-missing sites, as 0 / 1 per site for the prefix scan
+struct UniformSite {
+    __host__ __device__ int64_t operator()(uint8_t c) const { return c >= PG_CLS_A && c <= PG_CLS_T ? 1 : 0; }
+};
+struct Widen {
+    __host__ __device__ int64_t operator()(int32_t v) const { return v; }
+};
+
+// group k's first site (the site of varied rank k R, or of rank first[k] for a budget of words; 0 for k = 0) and end (the next
+// group's first site; S for the last)
+__device__ __forceinline__ void uni_group(const int64_t* src, int R, int64_t S, int64_t ng, int64_t k, int64_t& lo, int64_t& hi,
+                                          const int64_t* first) {
+    lo = k == 0 ? 0 : src[first ? first[k] : k * R];
+    hi = k + 1 < ng ? src[first ? first[k + 1] : (k + 1) * R] : S;
+}
+// the words of each varied row (src: its site, in site order), and 0 behind the last, for the scan of their first words
+__global__ void k1_uni_w(const uint8_t* cls, const int64_t* src, int64_t varied, int wd, int pw, bool bits, int64_t* w) {
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r <= varied; r += (int64_t)gridDim.x * blockDim.x)
+        w[r] = r < varied ? (uni_one_plane(cls[src[r]], bits) ? wd : pw) : 0;
+}
+// group g of a budget of Bw words: the rows whose first word cw lies in [g Bw, (g + 1) Bw) (consecutive, as no row exceeds Bw
+// words); first[g] = its first row's rank
+__global__ void k1_uni_first(const int64_t* cw, int64_t varied, int64_t Bw, int64_t* first) {
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < varied; r += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t g = cw[r] / Bw;
+        if (r == 0 || cw[r - 1] / Bw != g) first[g] = r;
+    }
 }
 
 // pieces of at most tmax sites per group
 __global__ void __launch_bounds__(256) k1_uni_groups(const int64_t* __restrict__ src, int R, int64_t S, int tmax, int64_t ng,
-                                                     int64_t* __restrict__ pieces) {
+                                                     int64_t* __restrict__ pieces, const int64_t* first) {
     const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= ng) return;
     int64_t lo, hi;
-    uni_group(src, R, S, ng, k, lo, hi);
+    uni_group(src, R, S, ng, k, lo, hi, first);
     const int64_t n = (hi - lo + tmax - 1) / tmax;
     pieces[k] = n > 1 ? n : 1;
 }
@@ -1835,13 +1869,14 @@ __global__ void __launch_bounds__(256) k1_uni_groups(const int64_t* __restrict__
 // site_lo of every tile from the groups' first pieces (base, the exclusive scan of the pieces: base[ng] = tiles); the entries
 // from the last tile on up to nt_max hold S (empty tiles)
 __global__ void __launch_bounds__(256) k1_uni_tiles(const int64_t* __restrict__ src, int R, int64_t S, int tmax, int64_t ng,
-                                                    const int64_t* __restrict__ base, int64_t nt_max, int64_t* __restrict__ site_lo) {
+                                                    const int64_t* __restrict__ base, int64_t nt_max, int64_t* __restrict__ site_lo,
+                                                    const int64_t* first) {
     const int64_t nt = base[ng];
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= (ng > nt_max ? ng : nt_max);
          i += (int64_t)gridDim.x * blockDim.x) {
         if (i < ng) {
             int64_t lo, hi;
-            uni_group(src, R, S, ng, i, lo, hi);
+            uni_group(src, R, S, ng, i, lo, hi, first);
             for (int64_t b = base[i], j = 0; b + j < base[i + 1]; ++j) site_lo[b + j] = lo + j * tmax;
         }
         if (i >= nt && i <= nt_max) site_lo[i] = S;
@@ -1862,9 +1897,16 @@ __global__ void __launch_bounds__(256) k1_uni_bounds(const int64_t* __restrict__
 // uniform_prepare rebuilds the stream when the data or the geometry changed; uniform_slots rebuilds the slot tables and the
 // launch when the windows (epoch), the stream (serial), the slot width or the ring changed.
 struct UniformPass {
-    K1Plan plan;              // the cache's plan with room for the codes in each stage (its G, wpt and warps serve the stream)
+    K1Plan plan;              // the cache's plan (its G, wpt and warps serve the stream)
     int table_bytes = 0;      // shared-memory bytes of plan's tables
     int R = 0, Tmax = 0, stages = 0, stage_bytes = 0;   // row budget, tile bound, and ring (uni_geometry)
+    // complete biallelic rows as one plane: below 8 (padded) populations.  At 8 the one-plane walk was slower than the
+    // three-plane one (C5, H100 80GB HBM3, 700 W: 0.963 against 0.884 ms) and spilled more, so there every varied row is
+    // streamed as three planes and the kernel has no one-plane walk
+    bool one_plane = true;
+    int wd = 0;                     // words per plane
+    bool bits = false, words = false;   // this call: one-plane rows; tiles by a budget of row words (uni_geometry)
+    int row_cap = 0, cap_rows = 0;      // three-plane rows a stage has room for; rows a tile may hold
     UniformStream us;
     PgBuf slot_buf;
     uint64_t slots_epoch = 0, slots_serial = 0;
@@ -2109,16 +2151,20 @@ int with_popgen_mode(bool with_freq, int Pp, F&& f) {
     });
 }
 
-// Streaming only the varied rows costs 6 + (1 - u) * (pitch + 2) bytes per site (position, code; row, slot) against
-// 4 + pitch, for a uniform fraction u, plus a rebuild whenever the data change.  tools/packed_site_pass.py --sweep times the
-// two passes across u at the C2 shape (H100 80GB HBM3, 700 W): 0.48 against 0.55 ms at u = 20 %, 0.52 against 0.55 at 10 %,
-// 0.553 against 0.555 at 5 %, 0.57 against 0.555 at 1 %.  The stream is kept from u >= 1/8 on, where its gain is clear of the
+// Streaming only the varied rows costs (1 - u) * (pitch + 2) bytes per site (row, slot; a third of the row for a complete
+// biallelic site) against 4 + pitch, for a uniform fraction u, plus a rebuild whenever the data change.
+// tools/packed_site_pass.py --sweep timed the two passes across u at the C2 shape when the stream still carried 6 bytes of
+// position and code per site (H100 80GB HBM3, 700 W): 0.48 against 0.55 ms at u = 20 %, 0.52 against 0.55 at 10 %, 0.553
+// against 0.555 at 5 %, 0.57 against 0.555 at 1 %.  The stream is kept from u >= 1/8 on, where its gain is clear of the
 // run-to-run spread.
 constexpr double UNI_MIN_FRACTION = 0.125;
 
-// Bytes of a stage of the stream's ring: R varied rows, the positions of Tmax sites from a 4-site boundary, Tmax codes, R slots.
-int uni_stage_bytes(int R, int Tmax, int pitch) {
-    return (int)align_up((size_t)R * pitch + (size_t)(Tmax + 4) * 4 + (size_t)Tmax * 2 + align_up((size_t)R * 2, 16), 128);
+// One-plane rows of wd words a budget of R three-plane rows (of pitch bytes) holds, less 3 words of padding
+int uni_word_rows(int R, int pitch, int wd) { return (R * (pitch / 4) - 3) / wd; }
+
+// Bytes of a stage of the stream's ring: row_cap three-plane rows, then a slot per row (cap_rows of them).
+int uni_stage_bytes(int row_cap, int cap_rows, int pitch) {
+    return (int)align_up((size_t)row_cap * pitch + align_up((size_t)cap_rows * 2, 16), 128);
 }
 
 // The stream's geometry for the plan u.plan: a tile bound of Tmax = 512 sites (PG_K1_UNI_TMAX, a multiple of 8 up to 32768), and a
@@ -2128,37 +2174,57 @@ int uni_stage_bytes(int R, int Tmax, int pitch) {
 // R = 32 / 64 / 128 / 256 0.50 / 0.30 / 0.22 / 0.23 ms; C5 (2 warps, 608-byte rows) R = 32 / 64 / 128 1.40 / 1.09 / 1.62 ms
 // (8, 5 and 2 stages): rows that fill the lanes matter more than stages beyond the teams' count.  Tmax = 256 / 512 / 2048:
 // C2 0.30 / 0.22 / 0.24 ms.
+// With one-plane rows (bits) and R not set, tiles are cut by a budget of row words instead: the words of R three-plane rows,
+// so a tile holds up to about 3R one-plane rows (cap_rows).  A row belongs to the tile its first word falls in, so the last
+// one may run past the budget by a row: the stage has room for R + 1 rows (row_cap).  H100 80GB HBM3, 700 W,
+// tools/packed_site_pass.py: C2 0.120 ms against 0.156 with R rows (5,000-site windows 0.145 against 0.176), with Tmax 2048 (the
+// R-row budget at Tmax 2048: 0.156, 0.176).  PG_K1_UNI_R sets a budget of R rows of either kind, as before.
 void uni_geometry(UniformPass& u) {
     const K1Plan& pl = u.plan;
-    int Tmax = 512;
+    const char* eb = getenv("PG_K1_UNI_BITS");
+    u.bits = u.one_plane && !(eb && *eb && atoi(eb) == 0);
+    const char* er = getenv("PG_K1_UNI_R");
+    u.words = u.bits && !(er && *er);
+    int Tmax = u.words ? 2048 : 512;
     if (const char* e = getenv("PG_K1_UNI_TMAX")) Tmax = std::max(8, std::min(32768, (atoi(e) + 7) / 8 * 8));
     const int lanes = 32 / std::max(1, pl.G);
     int R = lanes * pl.wpt;
-    const char* er = getenv("PG_K1_UNI_R");
+    auto stage = [&](int r) {
+        const bool w = u.words && r >= 2;     // from 2 rows on the budget holds a three-plane row whole
+        u.row_cap = w ? r + 1 : r;
+        u.cap_rows = w ? uni_word_rows(r, pl.pitch, u.wd) : r;
+        return uni_stage_bytes(u.row_cap, u.cap_rows, pl.pitch);
+    };
     if (er && *er) {
         R = std::max(1, std::min(0x7fff, atoi(er)));
     } else {
-        while (R > lanes && pg_k1_ring_stages(uni_stage_bytes(R, Tmax, pl.pitch), u.table_bytes) < 2) R /= 2;
+        while (R > lanes && pg_k1_ring_stages(stage(R), u.table_bytes) < 2) R /= 2;
     }
+    u.words = u.words && R >= 2;
     u.R = R;
     u.Tmax = Tmax;
-    u.stage_bytes = uni_stage_bytes(R, Tmax, pl.pitch);
+    u.stage_bytes = stage(R);
     u.stages = pl.stages >= 2 ? pg_k1_ring_stages(u.stage_bytes, u.table_bytes) : 0;
 }
 
 // (Re)builds u.us for the current data and geometry when they changed: two host synchronisations per rebuild (the count of
 // varied rows, which sizes the buffers; the count of tiles with the CTAs' first sites, which size the launch and its slots),
 // nothing on a call over unchanged data.  PG_K1_UNIFORM_FORCE keeps the stream whatever the uniform fraction (tests on missing
-// data).
+// data); PG_K1_UNI_BITS=0 streams every varied row as three planes (the tests and tools/packed_site_pass.py compare the two),
+// as the stream does at 8 populations (UniformPass::one_plane).
 int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
     UniformStream& us = u.us;
     const bool forced = getenv("PG_K1_UNIFORM_FORCE") != nullptr;
+    const bool bits = u.bits, wb = u.words;
     const int R = u.R, Tmax = u.Tmax;
-    if (us.gen == ctx->data_gen && us.R == R && us.Tmax == Tmax && us.forced == forced) return PG_OK;
+    if (us.gen == ctx->data_gen && us.R == R && us.Tmax == Tmax && us.forced == forced && us.bits == bits && us.wb == wb)
+        return PG_OK;
+    us.wb = wb;
     us.gen = ctx->data_gen;
     us.R = R;
     us.Tmax = Tmax;
     us.forced = forced;
+    us.bits = bits;
     us.in_use = false;
     us.varied = ctx->S;
     us.serial += 1;
@@ -2166,15 +2232,21 @@ int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
     const int64_t S = ctx->S;
     constexpr int CH = 2048;                  // the chunks of the first pass (varied counts, then each varied row's site)
     const int64_t nc = (S + CH - 1) / CH;
-    const int64_t nt_max = S / Tmax + 1 + (S + R - 1) / R + 1;   // groups + S / Tmax bound the pieces
+    const int ppw = ctx->packed_pitch / 4, wd = u.wd;
+    const int64_t Bw = (int64_t)u.cap_rows * wd;   // words budget: a multiple of the one-plane rows' words
+    // groups + S / Tmax bound the pieces
+    const int64_t nt_max = S / Tmax + 1 + (wb ? S * ppw / Bw + 2 : (S + R - 1) / R) + 1;
     const int64_t nscan = std::max(nc, nt_max) + 1;
     PG_TRY(us.cnt.ensure((size_t)nscan * 8));
     PG_TRY(us.row0.ensure((size_t)nscan * 8));
     int64_t* d_cnt = (int64_t*)us.cnt.p;
     int64_t* d_row0 = (int64_t*)us.row0.p;
-    size_t scan_bytes = 0;
+    size_t scan_bytes = 0, pre_bytes = 0;
     PG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_cnt, d_row0, nscan, ctx->stream));
-    PG_TRY(us.scan.ensure(scan_bytes));
+    const auto uni_in = cub::TransformInputIterator<int64_t, UniformSite, const uint8_t*>(ctx->d_site_cls, UniformSite());
+    const auto pos_in = cub::TransformInputIterator<int64_t, Widen, const int32_t*>(ctx->d_pos, Widen());
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, pre_bytes, uni_in, d_row0, S + 1, ctx->stream));
+    PG_TRY(us.scan.ensure(std::max(scan_bytes, pre_bytes)));
     int ti = pg_time_begin(ctx, "k1_uniform");
     PG_CUDA(cudaMemsetAsync(d_cnt + nc, 0, 8, ctx->stream));
     k1_uni_count<<<(unsigned)nc, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, nullptr, CH, d_cnt);
@@ -2186,18 +2258,16 @@ int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
     us.varied = varied;
     if (!forced && (double)(S - varied) < UNI_MIN_FRACTION * (double)S) return PG_OK;
-    us.code_pitch = Tmax;
-    const int64_t ng = varied > 0 ? (varied + R - 1) / R : 1;
-    const int chunks = ctx->packed_pitch / 16;
-    if (us.codes.ensure((size_t)nt_max * us.code_pitch * 4) != PG_OK ||
-        us.src.ensure((size_t)std::max<int64_t>(varied, 1) * 8) != PG_OK ||
-        us.rows.ensure((size_t)std::max<int64_t>(varied, 1) * ctx->packed_pitch) != PG_OK ||
+    // the group count, exact for a budget of rows, a bound for a budget of words (set below)
+    int64_t ng = varied > 0 ? (wb ? varied * ppw / Bw + 2 : (varied + R - 1) / R) : 1;
+    if (us.slots.ensure((size_t)nt_max * Tmax * 2) != PG_OK || us.src.ensure((size_t)std::max<int64_t>(varied, 1) * 8) != PG_OK ||
+        us.rows.ensure((size_t)std::max<int64_t>(varied, 1) * ctx->packed_pitch + (size_t)nt_max * 16) != PG_OK ||
         us.site_lo.ensure((size_t)(nt_max + 1) * 8) != PG_OK || us.groups.ensure((size_t)(ng + 1) * 8 * 2) != PG_OK ||
-        us.info.ensure((size_t)(ctx->sm_count + 2) * 8) != PG_OK) {
+        us.info.ensure((size_t)(ctx->sm_count + 2) * 8) != PG_OK || us.words.ensure((size_t)(nt_max + 1) * 8 * 2) != PG_OK ||
+        us.n1.ensure((size_t)(nt_max + 1) * 4) != PG_OK || us.pre.ensure((size_t)(S + 1) * 8 * 2) != PG_OK ||
+        (wb && us.wts.ensure((size_t)(varied + 1) * 8 * 2 + (size_t)(ng + 1) * 8) != PG_OK)) {
         cudaGetLastError();                   // no memory for the stream: the packed pass streams every row
-        us.rows.release();
-        us.src.release();
-        us.codes.release();
+        for (PgBuf* b : {&us.rows, &us.src, &us.slots, &us.pre}) b->release();
         return PG_OK;
     }
     int64_t* d_src = (int64_t*)us.src.p;
@@ -2205,29 +2275,60 @@ int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
     int64_t* d_base = d_pieces + ng + 1;
     int64_t* d_site_lo = (int64_t*)us.site_lo.p;
     int64_t* d_info = (int64_t*)us.info.p;
+    int64_t* d_wcnt = (int64_t*)us.words.p;
+    int64_t* d_woff = d_wcnt + nt_max + 1;
+    us.woff = d_woff;
+    int32_t* d_n1 = (int32_t*)us.n1.p;
+    int64_t* d_pre = (int64_t*)us.pre.p;
     ti = pg_time_begin(ctx, "k1_uniform");
-    // each varied row's site, then the groups of R rows, their pieces, the tiles' first sites and first rows, their codes and
-    // varied rows
-    k1_uni_codes<<<(unsigned)nc, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, nullptr, CH, CH, d_row0, nullptr, d_src);
+    // each varied row's site, then the groups of R rows, their pieces, the tiles' first sites, first rows, one-plane rows and
+    // first words, their slots and rows; the per-site prefixes
+    k1_uni_rows<<<(unsigned)nc, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, nullptr, CH, d_row0, d_src);
     PG_CUDA(cudaGetLastError());
+    // a budget of words: each row's first word (cw), the first row of each group, and (a third synchronisation) the count
+    int64_t* d_first = nullptr;
+    if (wb && varied > 0) {
+        int64_t* w = (int64_t*)us.wts.p;
+        int64_t* cw = w + varied + 1;
+        d_first = cw + varied + 1;
+        k1_uni_w<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(ctx->d_site_cls, d_src, varied, wd, ppw, bits, w);
+        PG_CUDA(cudaGetLastError());
+        size_t tb = 0;
+        PG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, w, cw, varied + 1, ctx->stream));
+        PG_TRY(us.scan2.ensure(tb));
+        PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan2.p, tb, w, cw, varied + 1, ctx->stream));
+        k1_uni_first<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(cw, varied, Bw, d_first);
+        PG_CUDA(cudaGetLastError());
+        int64_t last = 0;
+        PG_CUDA(cudaMemcpyAsync(&last, cw + varied - 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        PG_CUDA(cudaStreamSynchronize(ctx->stream));
+        ng = last / Bw + 1;
+    } else if (wb) {
+        ng = 1;
+    }
     PG_CUDA(cudaMemsetAsync(d_pieces + ng, 0, 8, ctx->stream));
-    k1_uni_groups<<<(unsigned)((ng + 255) / 256), 256, 0, ctx->stream>>>(d_src, R, S, Tmax, ng, d_pieces);
+    k1_uni_groups<<<(unsigned)((ng + 255) / 256), 256, 0, ctx->stream>>>(d_src, R, S, Tmax, ng, d_pieces, d_first);
     PG_CUDA(cudaGetLastError());
     PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, scan_bytes, d_pieces, d_base, ng + 1, ctx->stream));
     const int64_t nfill = std::max(ng, nt_max) + 1;
     k1_uni_tiles<<<(unsigned)std::min<int64_t>((nfill + 255) / 256, (int64_t)ctx->sm_count * 16), 256, 0, ctx->stream>>>(
-        d_src, R, S, Tmax, ng, d_base, nt_max, d_site_lo);
+        d_src, R, S, Tmax, ng, d_base, nt_max, d_site_lo, d_first);
     PG_CUDA(cudaGetLastError());
     PG_CUDA(cudaMemsetAsync(d_cnt + nt_max, 0, 8, ctx->stream));
-    k1_uni_count<<<(unsigned)nt_max, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, d_site_lo, Tmax, d_cnt);
+    PG_CUDA(cudaMemsetAsync(d_wcnt + nt_max, 0, 8, ctx->stream));
+    k1_uni_count<<<(unsigned)nt_max, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, d_site_lo, Tmax, d_cnt, d_wcnt, d_n1, wd, ppw,
+                                                           bits);
     PG_CUDA(cudaGetLastError());
     PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, scan_bytes, d_cnt, d_row0, nt_max + 1, ctx->stream));
-    k1_uni_codes<<<(unsigned)nt_max, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, d_site_lo, Tmax, us.code_pitch, d_row0,
-                                                           (uint16_t*)us.codes.p, d_src, (const uint4*)ctx->d_packed, chunks,
-                                                           (uint32_t*)us.rows.p);
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, scan_bytes, d_wcnt, d_woff, nt_max + 1, ctx->stream));
+    k1_uni_rows<<<(unsigned)nt_max, 256, 0, ctx->stream>>>(ctx->d_site_cls, S, d_site_lo, Tmax, d_row0, d_src,
+                                                          (uint16_t*)us.slots.p, d_n1, d_woff, ctx->d_packed, ppw, wd, bits,
+                                                          (uint32_t*)us.rows.p);
     PG_CUDA(cudaGetLastError());
     k1_uni_bounds<<<1, 256, 0, ctx->stream>>>(d_base, ng, d_site_lo, ctx->sm_count, d_info);
     PG_CUDA(cudaGetLastError());
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, pre_bytes, uni_in, d_pre, S + 1, ctx->stream));
+    PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, pre_bytes, pos_in, d_pre + S + 1, S + 1, ctx->stream));
     pg_time_end(ctx, ti);
     std::vector<int64_t> info(ctx->sm_count + 2);
     PG_CUDA(cudaMemcpyAsync(info.data(), d_info, info.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2268,13 +2369,14 @@ int uniform_slots(pg_ctx* ctx, UniformPass& u, const K1Launch& L, int Q) {
     p.num_tiles = pl.num_tiles;
     p.stages = pl.stages;
     p.tile_bytes = pl.tile_bytes;
-    p.row_cap = u.R;
+    p.row_cap = u.row_cap;
     p.cta_seg_first = u.L.slots.cta_seg_first;
     p.cta_slot_off = u.L.slots.cta_slot_off;
     p.row0 = (const int64_t*)u.us.row0.p;
     p.site_lo = (const int64_t*)u.us.site_lo.p;
-    p.codes = (const uint16_t*)u.us.codes.p;
-    p.code_pitch = u.us.code_pitch;
+    p.woff = u.us.woff;
+    p.n1 = (const int32_t*)u.us.n1.p;
+    p.slots = (const uint16_t*)u.us.slots.p;
     u.slots_epoch = ctx->epoch;
     u.slots_serial = u.us.serial;
     u.slots_Q = Q;
@@ -2494,9 +2596,10 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
             c.lanepop = false;
             const int nw = k1_nw_for(ctx->packed_pitch, false);
             PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, /*force_G=*/0, /*packed=*/true));
-            u.table_bytes = table_bytes_of(c.pt) + UNI_SMEM_BYTES;
-            u.plan = pg_make_k1_plan_rows(ctx->S, ctx->packed_pitch, ctx->sm_count, u.table_bytes, nw, 0, 4);
-            if (!pg_k1_plan_ok(u.plan)) u.plan.stages = 0;    // no room for the codes: every row is streamed
+            u.table_bytes = table_bytes_of(c.pt);
+            u.plan = c.L.plan;
+            u.one_plane = Pp < 8;
+            u.wd = (ctx->H + 31) / 32;
             u.slots_epoch = 0;                                  // u.L follows c.L
         } else {
             // long rows, 4 or 8 real populations of <= 255 haplotypes: one lane per population (k1_site_pass_lp)
@@ -2550,6 +2653,11 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     fp.force_path = many ? 2 : force_path;
     fp.bookkeeping_only = many ? 1 : 0;
     fp.with_freq = wf ? 1 : 0;
+    if (u.last) {
+        fp.pre_uni = (const int64_t*)u.us.pre.p;
+        fp.pre_pos = fp.pre_uni + ctx->S + 1;
+        fp.S = ctx->S;
+    }
     fp.rec = (unsigned long long*)d_rec;
     fp.RC = RC;
     fp.path = d_path;
@@ -2586,7 +2694,7 @@ extern "C" int pg_debug_uniform_ring(pg_ctx* ctx, int32_t* out) {
     PG_CHECK(ctx && out, "pg_debug_uniform_ring: null argument");
     const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
     const bool read = c && c->up.last;
-    out[0] = read ? c->up.R : 0;
+    out[0] = read ? c->up.cap_rows : 0;
     out[1] = read ? c->up.stages : 0;
     out[2] = read ? c->up.stage_bytes : 0;
     return PG_OK;
@@ -2599,7 +2707,7 @@ extern "C" int pg_debug_uniform_tiles(pg_ctx* ctx, int64_t cap, int64_t* site_lo
     const bool read = c && c->up.last;
     const UniformStream* us = read ? &c->up.us : nullptr;
     *ntiles = read ? us->nt : 0;
-    geometry[0] = read ? c->up.R : 0;
+    geometry[0] = read ? c->up.cap_rows : 0;
     geometry[1] = read ? c->up.Tmax : 0;
     if (!read || cap < us->nt + 1) return PG_OK;
     PG_CHECK(site_lo && row0, "pg_debug_uniform_tiles: null table");
@@ -2607,6 +2715,22 @@ extern "C" int pg_debug_uniform_tiles(pg_ctx* ctx, int64_t cap, int64_t* site_lo
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
     PG_CUDA(cudaMemcpy(site_lo, us->site_lo.p, (size_t)(us->nt + 1) * 8, cudaMemcpyDeviceToHost));
     PG_CUDA(cudaMemcpy(row0, us->row0.p, (size_t)(us->nt + 1) * 8, cudaMemcpyDeviceToHost));
+    return PG_OK;
+}
+
+extern "C" int pg_debug_uniform_rows(pg_ctx* ctx, int64_t* one_plane_rows, int64_t* words) {
+    PG_CHECK(ctx && one_plane_rows && words, "pg_debug_uniform_rows: null argument");
+    const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
+    const bool read = c && c->up.last;
+    *one_plane_rows = *words = 0;
+    if (!read) return PG_OK;
+    const UniformStream& us = c->up.us;
+    PG_CUDA(cudaSetDevice(ctx->device));
+    PG_CUDA(cudaStreamSynchronize(ctx->stream));
+    std::vector<int32_t> n1((size_t)us.nt);
+    PG_CUDA(cudaMemcpy(n1.data(), us.n1.p, n1.size() * 4, cudaMemcpyDeviceToHost));
+    PG_CUDA(cudaMemcpy(words, us.woff + us.nt, 8, cudaMemcpyDeviceToHost));
+    for (int32_t v : n1) *one_plane_rows += v;
     return PG_OK;
 }
 

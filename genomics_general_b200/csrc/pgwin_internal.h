@@ -72,17 +72,22 @@ struct K1Plan {
     int ctas;         // persistent CTAs, each owning a contiguous tile range
 };
 K1Plan pg_make_k1_plan(int64_t S, int H, int sm_count, int table_bytes, int nw = 8, int force_G = 0);
-// rows of `pitch` bytes; code_bytes: bytes per site that a tile carries behind its positions (the uniform-site codes and
-// varied-row slots), an even number
-K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G, int code_bytes = 0);
+// rows of `pitch` bytes
+K1Plan pg_make_k1_plan_rows(int64_t S, int pitch, int sm_count, int table_bytes, int nw, int force_G);
 int pg_k1_ring_stages(int tile_bytes, int table_bytes);   // ring depth for stages of tile_bytes (< 2: does not fit)
 int pg_k1_plan_ok(const K1Plan& p);   // 1 if the site-pass kernels can run this plan
 int pg_pitch_for(int H);
 int pg_packed_pitch_for(int H);       // bytes per row of the packed companion
 
 // Site class of a packed row over its H haplotypes: every haplotype carries allele A / C / G / T, every haplotype is missing,
-// or anything else.  Zeroed memory reads as "varied", which is always safe to walk.
-enum { PG_CLS_VARIED = 0, PG_CLS_A = 1, PG_CLS_C = 2, PG_CLS_G = 3, PG_CLS_T = 4, PG_CLS_MISSING = 5 };
+// every haplotype is called and exactly two alleles are present ("complete biallelic": VARIED2 when the two codes differ in
+// their low bit only, so that plane B0 tells them apart; VARIED2_B1 when they differ in the high bit, so that plane B1 does,
+// the higher code carrying the set bit either way), or anything else.  Zeroed memory reads as "varied", which is always safe
+// to walk.
+enum { PG_CLS_VARIED = 0, PG_CLS_A = 1, PG_CLS_C = 2, PG_CLS_G = 3, PG_CLS_T = 4, PG_CLS_MISSING = 5, PG_CLS_VARIED2 = 6,
+       PG_CLS_VARIED2_B1 = 7 };
+__host__ __device__ inline bool pg_cls_varied(unsigned c) { return c == PG_CLS_VARIED || c >= PG_CLS_VARIED2; }
+__host__ __device__ inline bool pg_cls_biallelic(unsigned c) { return c >= PG_CLS_VARIED2; }
 
 struct pg_ctx {
     int device = 0;

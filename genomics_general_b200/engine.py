@@ -635,12 +635,26 @@ class Engine:
         wd = (self.H + 31) // 32
         return out[:, :3 * wd].reshape(n, 3, wd)
 
+    def site_classes(self, site0: int, n: int):
+        """uint8 [n] class bytes of the packed companion's rows (0 varied, 1..4 all A / C / G / T, 5 all missing, 6 / 7 every
+        haplotype called and exactly two alleles, differing in the low / high allele-code bit), or None when it keeps none."""
+        avail = C.c_int32(0)
+        out = np.empty(int(n), dtype=np.uint8)
+        check(self._lib.pg_debug_site_cls(self._ctx, int(site0), int(n), C.byref(avail), _ptr(out)), "pg_debug_site_cls")
+        return out if avail.value else None
+
     def uniform_stream(self):
         """(in_use, varied_sites): whether the last popgen call's site pass streamed only the packed rows of the sites whose
         haplotypes are not all the same, and how many such sites it counted (S when it did not count them)."""
         in_use, varied = C.c_int32(0), C.c_int64(0)
         check(self._lib.pg_debug_uniform(self._ctx, C.byref(in_use), C.byref(varied)), "pg_debug_uniform")
         return bool(in_use.value), int(varied.value)
+
+    def uniform_rows(self):
+        """(one-plane rows, words of all rows) of the varied-row stream the last popgen call read ((0, 0) when it did not)."""
+        n1, words = C.c_int64(0), C.c_int64(0)
+        check(self._lib.pg_debug_uniform_rows(self._ctx, C.byref(n1), C.byref(words)), "pg_debug_uniform_rows")
+        return int(n1.value), int(words.value)
 
     def uniform_tile(self):
         """(sites per tile, warps per tile) of the varied-row stream's launch plan, as the last popgen call on the packed

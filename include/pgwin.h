@@ -355,6 +355,10 @@ int pg_debug_k1_plan_ex(int64_t S, int32_t H, int32_t nw, int32_t force_G, int32
  * (three planes of ceil(H / 32) words — valid bits, low and high bit of the allele code A0 C1 G2 T3 — then padding), 0 when
  * the context has no companion.  out (may be NULL) receives rows [site0, site0 + n). */
 int pg_debug_packed(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* row_words, uint32_t* out);
+/* The class byte of each site of the packed companion, sites [site0, site0 + n) into out (may be NULL): 0 varied, 1..4 every
+ * haplotype carries A / C / G / T, 5 every haplotype missing, 6 / 7 every haplotype called and exactly two alleles present,
+ * told apart by the low / high allele-code bit.  *avail = 0 when the context keeps no classes. */
+int pg_debug_site_cls(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* avail, uint8_t* out);
 /* The popgen pass's stream of varied rows as the last popgen call left it: *in_use = 1 when that call streamed only the
  * rows of sites whose haplotypes are not all the same (0: every packed row), *varied_sites = the varied sites it counted
  * (S when it did not count them). */
@@ -369,6 +373,9 @@ int pg_debug_uniform_ring(pg_ctx* ctx, int32_t* out);
  * geometry[1] = Tmax (sites per tile at most); when cap >= *ntiles + 1, site_lo / row0 get each tile's first site / first
  * varied row and the totals (S, varied rows) at [ntiles].  All 0 when the last call did not read the stream. */
 int pg_debug_uniform_tiles(pg_ctx* ctx, int64_t cap, int64_t* site_lo, int64_t* row0, int64_t* ntiles, int32_t* geometry);
+/* Rows of the varied-row stream the last popgen call read: *one_plane_rows = complete biallelic rows streamed as one plane,
+ * *words = 32-bit words of all its rows (both 0 when the last call did not read the stream). */
+int pg_debug_uniform_rows(pg_ctx* ctx, int64_t* one_plane_rows, int64_t* words);
 
 #ifdef __cplusplus
 }

@@ -1,11 +1,12 @@
-"""The popgen site pass three ways, timed alternately in one process: on the one-hot bytes (PG_K1_BYTE_PASS), on every row of
-the packed companion (PG_K1_NO_UNIFORM), and on the packed rows of the varied sites only ("varied_rows", the default where
-enough sites are uniform: a walk over the varied rows on all the team's lanes, then a pass over every slot without a walk),
-at the C2 shape (4 x 50 diploid samples, H = 400, 10 M sites) with 50,000-site windows and with the benchmark's 5,000-site
+"""The popgen site pass four ways, timed alternately in one process: on the one-hot bytes (PG_K1_BYTE_PASS), on every row of
+the packed companion (PG_K1_NO_UNIFORM), on the packed rows of the varied sites only ("varied_rows", the default where
+enough sites are uniform: complete biallelic rows as one allele bit per haplotype, the others as three planes, walked on all
+the team's lanes; the uniform sites and positions come from per-site prefixes), and on that stream with every varied row in
+three planes ("varied_planes", PG_K1_UNI_BITS=0), at the C2 shape (4 x 50 diploid samples, H = 400, 10 M sites) with 50,000-site windows and with the benchmark's 5,000-site
 windows (C2_w5000), and the C5 shape (8 x 100 diploid samples, H = 1600, 12.5 M sites).  Per pass and shape: median / min / max of the k1_popgen kernel time (CUDA events) over the rounds, the bytes the
 pass reads per site, the achieved GB/s, the time of the varied-row build (k1_uniform, once per data change), the varied-row
 stream's geometry (row budget R, tile bound Tmax, ring stages and bytes, tiles, mean rows and sites per tile), and whether the
-records of the three passes are bit-identical.
+records of the four passes are bit-identical.
 
 --sweep adds, at C2 and C5: the elided pass under PG_K1_UNI_R / PG_K1_UNI_TMAX / PG_K1_STAGES settings; at C2: and the packed pass against the elided one
 (forced on) at small uniform fractions, the measurement behind the fraction from which the stream is kept.
@@ -25,8 +26,10 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from genomics_general_b200 import synth  # noqa: E402
 from genomics_general_b200.engine import Engine  # noqa: E402
 
-PASS_ENV = {"byte": {"PG_K1_BYTE_PASS": "1"}, "packed": {"PG_K1_NO_UNIFORM": "1"}, "varied_rows": {}}
-KNOBS = ("PG_K1_BYTE_PASS", "PG_K1_NO_UNIFORM", "PG_K1_UNIFORM_FORCE", "PG_K1_TILE_KB", "PG_K1_STAGES")
+PASS_ENV = {"byte": {"PG_K1_BYTE_PASS": "1"}, "packed": {"PG_K1_NO_UNIFORM": "1"}, "varied_rows": {},
+            "varied_planes": {"PG_K1_UNI_BITS": "0"}}
+STREAMS = ("varied_rows", "varied_planes")
+KNOBS = ("PG_K1_BYTE_PASS", "PG_K1_NO_UNIFORM", "PG_K1_UNIFORM_FORCE", "PG_K1_TILE_KB", "PG_K1_STAGES", "PG_K1_UNI_BITS")
 
 
 def card():
@@ -103,19 +106,23 @@ def main():
             H = load(eng, P, spp, S, w)
             one_hot, packed = row_bytes(H)
             ms = {k: [] for k in PASS_ENV}
-            build_ms, rec, varied = [], {}, None
+            build_ms, rec, varied = {k: [] for k in STREAMS}, {}, None
+            wd = (H + 31) // 32
+            one_plane = 0
             for rnd in range(args.rounds):
                 for kind, env in PASS_ENV.items():
-                    if kind == "varied_rows" and rnd % 2:
-                        env = {"PG_K1_UNIFORM_FORCE": "1"}      # a different key: the next call rebuilds the stream
+                    if kind in STREAMS and rnd % 2:
+                        env = dict(env, PG_K1_UNIFORM_FORCE="1")   # a different key: the next call rebuilds the stream
                     set_env(env)
                     r = eng.popgen(1, 0.01)                      # warm-up (and re-plan / rebuild after the switch)
-                    if kind == "varied_rows":
+                    if kind in STREAMS:
                         t = eng.last_timings()
-                        assert "k1_uniform" in t
-                        build_ms.append(t["k1_uniform"]["ms"])
+                        if "k1_uniform" in t:       # at 8 populations both streams are three-plane: the same stream
+                            build_ms[kind].append(t["k1_uniform"]["ms"])
                         used, varied = eng.uniform_stream()
                         assert used
+                        if kind == "varied_rows":
+                            one_plane = eng.uniform_rows()[0]     # none at 8 populations
                         R, stages, stage_bytes = eng.uniform_ring()
                         _, Tmax, site_lo, row0 = eng.uniform_tiles()
                         geometry = {"R": R, "Tmax": Tmax, "stages": stages, "stage_bytes": stage_bytes,
@@ -127,14 +134,19 @@ def main():
             res = {"H": H, "P": P, "sites": S, "varied_sites": varied, "uniform_fraction": 1 - varied / S}
             res["byte"] = stats(ms["byte"], S, one_hot + 4)
             res["packed"] = stats(ms["packed"], S, packed + 4)
-            # position + code per site; packed row + its slot per varied site
-            res["varied_rows"] = stats(ms["varied_rows"], S, 6 + varied / S * (packed + 2))
-            res["varied_rows"]["k1_uniform_build_ms_median"] = float(np.median(build_ms))
+            # per varied site its row and its slot: one plane of wd words for a complete biallelic site
+            res["one_plane_rows"] = one_plane
+            res["varied_rows"] = stats(ms["varied_rows"], S, (one_plane * (4 * wd + 2) + (varied - one_plane) * (packed + 2)) / S)
+            res["varied_planes"] = stats(ms["varied_planes"], S, varied / S * (packed + 2))
+            for k in STREAMS:
+                res[k]["k1_uniform_build_ms_median"] = float(np.median(build_ms[k])) if build_ms[k] else None
             res["varied_rows"]["geometry"] = geometry
             res["speedup_varied_rows_vs_packed"] = (res["packed"]["k1_popgen_ms_median"] /
                                                     res["varied_rows"]["k1_popgen_ms_median"])
+            res["speedup_varied_rows_vs_planes"] = (res["varied_planes"]["k1_popgen_ms_median"] /
+                                                    res["varied_rows"]["k1_popgen_ms_median"])
             res["records_bit_identical"] = all(np.array_equal(rec["byte"][k], rec[o][k])
-                                               for k in rec["byte"] for o in ("packed", "varied_rows"))
+                                               for k in rec["byte"] for o in ("packed",) + STREAMS)
             out["shapes"][name] = res
         if args.sweep:
             for name, P, spp, S, w in (("C2", 4, 50, args.c2_sites, 50_000), ("C5", 8, 100, args.c5_sites, 5000)):
