@@ -78,6 +78,8 @@ _SIGS = {
     "pg_sfs_sparse_fetch": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_pairdist": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                               C.c_void_p]),
+    "pg_distpaint": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                               C.c_double, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_pairdist_cat": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64)]),
     "pg_seq_nonnan": (C.c_int, [C.c_void_p, C.c_void_p]),
     "pg_ind_het": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),

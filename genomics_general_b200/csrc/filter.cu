@@ -520,7 +520,7 @@ void pg_filter_free(pg_ctx* ctx) {
 extern "C" int pg_filter(pg_ctx* ctx, const pg_filter_spec* sp, const uint8_t* contig_mask, const int32_t* scaf_id,
                          int64_t* n_kept, uint8_t* flags_or) {
     PG_CHECK(ctx && sp && n_kept, "pg_filter: null argument");
-    PG_CHECK(ctx->ingest_sites == ctx->S && ctx->ingest_strict,
+    PG_CHECK(ctx->ingest_sites == ctx->S && ctx->ingest_strict == 1,
              "pg_filter: the resident sites must come from a text ingest with strict tokens (pg_ingest_set_strict)");
     const int64_t S = ctx->S;
     const int P = sp->P, ns = sp->n_samp;

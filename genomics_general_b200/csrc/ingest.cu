@@ -107,9 +107,10 @@ struct ParseParams {
     int32_t* pos;
     unsigned long long* scaf_hash;
     unsigned long long* err;    // all ones = ok, else (data line << 28) | (genotype column << 4) | code, 1-based
-    // strict tokens (pg_ingest_set_strict): a token must be exactly as wide as the sample's ploidy and hold only A C G T N
+    // strict tokens (pg_ingest_set_strict): 1 = a token must be exactly as wide as the sample's ploidy and hold only A C G T N
     // (phased / pairs) or a letter of genomics.py:14 DIPLOTYPES (diplo, diploid samples only); the phase character of each
-    // sample (token[1] of a phased token of ploidy >= 2, else '/', genomics.py:335) goes to aux[line * H + first_hap]
+    // sample (token[1] of a phased token of ploidy >= 2, else '/', genomics.py:335) goes to aux[line * H + first_hap].
+    // 2 = the width test only: other characters are read as without it (missing unless A C G T)
     int strict;
     uint8_t* aux;
     int aux_stride;
@@ -255,6 +256,8 @@ __global__ void __launch_bounds__(256) k_parse_lines(const __grid_constant__ Par
                             report(pp, ERR_PLOIDY, line, col);
                             continue;
                         }
+                    }
+                    if (pp.strict == 1) {
                         bool ok = true;
                         if (pp.fmt == 1) ok = diplotype(byte_at(pp, q));
                         else
@@ -535,7 +538,7 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
     pp.strict = ctx->ingest_strict;
     pp.aux = nullptr;
     pp.aux_stride = H_out;
-    if (pp.strict) {
+    if (pp.strict == 1) {
         PG_TRY(ctx->flt_aux.ensure((size_t)S * H_out + 64));
         pp.aux = (uint8_t*)ctx->flt_aux.p;
     }
@@ -601,7 +604,8 @@ extern "C" int pg_ingest_meta(pg_ctx* ctx, int32_t* pos, int8_t* new_scaffold, i
 // Strict tokens for the next ingests of this ctx (off by default): see ParseParams::strict.
 extern "C" int pg_ingest_set_strict(pg_ctx* ctx, int32_t on) {
     PG_CHECK(ctx != nullptr, "pg_ingest_set_strict: null ctx");
-    ctx->ingest_strict = on ? 1 : 0;
+    PG_CHECK(on >= 0 && on <= 2, "pg_ingest_set_strict: level %d is not 0, 1 or 2", on);
+    ctx->ingest_strict = on;
     return PG_OK;
 }
 

@@ -888,6 +888,177 @@ __global__ void __launch_bounds__(256) k2_ind_epi64(const __grid_constant__ IndE
     }
 }
 
+// ---- distPaint.py (distPaint.py:26-44, 62-83): nearest reference population of every query haplotype -------------
+constexpr int PAINT_WARPS = 4;         // warps per CTA; each holds its query's member distances in shared memory
+constexpr int PAINT_MAX_POPS = 32;     // one lane per population
+constexpr int PAINT_MAX_M = 1024;      // member entries: 8 KB of distances per warp, 32 KB per CTA
+
+struct PaintEpiParams {
+    const int32_t* diff;        // [nb][Hk][Hk]
+    const int32_t* n;           // [nb][Hm][Hm]
+    const int32_t* mid;
+    int Hm, Hk;
+    int n_query;
+    const int32_t* query_row;   // [n_query] plane row of each query
+    int P, M;
+    const int32_t* ref_off;     // [P + 1]
+    const int32_t* ref_row;     // [M] plane row of each member entry (duplicates allowed)
+    int min_sites;              // >= 1
+    int mode;                   // 0 rank-sum rule, 1 delta rule
+    double threshold;
+    int noresult;
+    int32_t* out;               // [nb][n_query]
+    double* means;              // [nb][n_query][P] or nullptr
+    double* pvals;              // [nb][n_query][P] or nullptr
+};
+
+__device__ __forceinline__ double nan_as_zero(double v) { return v != v ? 0.0 : v; }
+
+// np.sum of n doubles, nans read as 0 (np.nanmean's _replace_nan): numpy's pairwise summation (pairwise_sum in
+// numpy/_core/src/umath/loops_utils.h.src) — sequential below 8 values, 8 strided accumulators up to 128, else split at
+// n / 2 rounded down to a multiple of 8.  DEPTH bounds the splits: 5 covers PAINT_MAX_M.
+template <int DEPTH>
+__device__ double np_pairwise_sum(const double* a, int n) {
+    if (n < 8) {
+        double res = 0.0;
+        for (int i = 0; i < n; ++i) res += nan_as_zero(a[i]);
+        return res;
+    }
+    if constexpr (DEPTH > 0) {
+        if (n > 128) {
+            int n2 = n / 2;
+            n2 -= n2 % 8;
+            return np_pairwise_sum<DEPTH - 1>(a, n2) + np_pairwise_sum<DEPTH - 1>(a + n2, n - n2);
+        }
+    }
+    double r[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) r[k] = nan_as_zero(a[k]);
+    int i = 8;
+    for (; i < n - (n % 8); i += 8)
+#pragma unroll
+        for (int k = 0; k < 8; ++k) r[k] += nan_as_zero(a[i + k]);
+    double res = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
+    for (; i < n; ++i) res += nan_as_zero(a[i]);
+    return res;
+}
+
+// One warp per (query, window).  The warp gathers the query's M member distances d = diff / n (nan when n < minSites; 0 for
+// the query itself) into shared memory; lane p takes population p's np.nanmean; every lane then runs np.argmin (the first
+// nan, else the first minimum).  Rank-sum rule: for each other population j, scipy's ranksums(x_i, x_j, "less") from
+// average-tie ranks (twice the rank is an integer: 2 #less + #equal + 1), nan when either list holds a nan; p > threshold
+// gives noresult.  Delta rule: lane 0 sorts the means as CPython's list.sort does for fewer than 64 items (count_run, then
+// binarysort, all with <) and gives noresult when sorted[1] - sorted[0] < threshold.
+__global__ void __launch_bounds__(PAINT_WARPS * 32) k2_paint_epi(const __grid_constant__ PaintEpiParams ep) {
+    extern __shared__ __align__(16) double paint_sh[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int q = blockIdx.x * PAINT_WARPS + warp;
+    if (q >= ep.n_query) return;                            // warp-uniform
+    const int wb = blockIdx.y;
+    const int P = ep.P;
+    double* x = paint_sh + (size_t)warp * ep.M;
+    const int32_t* D = ep.diff + (size_t)wb * ep.Hk * ep.Hk;
+    const int32_t* N = ep.n + (size_t)wb * ep.Hm * ep.Hm;
+    const int i = ep.query_row[q], mi = ep.mid[i];
+    for (int k = lane; k < ep.M; k += 32) {
+        const int j = ep.ref_row[k];
+        const int nij = N[upper_idx(mi, ep.mid[j], ep.Hm)];
+        double d = nan_d();
+        if (nij >= ep.min_sites) d = (i == j) ? 0.0 : (double)D[upper_idx(i, j, ep.Hk)] / (double)nij;
+        x[k] = d;
+    }
+    __syncwarp();
+    double mean = nan_d();
+    bool has_nan = false;
+    if (lane < P) {
+        const int o0 = ep.ref_off[lane], o1 = ep.ref_off[lane + 1];
+        int cnt = 0;
+        for (int k = o0; k < o1; ++k) cnt += (x[k] == x[k]) ? 1 : 0;
+        if (cnt) mean = np_pairwise_sum<5>(x + o0, o1 - o0) / (double)cnt;
+        has_nan = cnt < o1 - o0;
+    }
+    const unsigned full = 0xffffffffu;
+    int best = 0;
+    double bv = __shfl_sync(full, mean, 0);
+    for (int p = 1; p < P; ++p) {
+        const double v = __shfl_sync(full, mean, p);
+        if (bv == bv && (v != v || v < bv)) {
+            best = p;
+            bv = v;
+        }
+    }
+    int result = best;
+    double pv = nan_d();                                   // lane p: p-value of the test against population p
+    if (ep.mode == 1) {
+        double s[PAINT_MAX_POPS];
+        for (int p = 0; p < P; ++p) s[p] = __shfl_sync(full, mean, p);
+        if (lane == 0) {
+            int run = 1;                                   // count_run: a strictly descending run is reversed
+            if (P > 1) {
+                run = 2;
+                if (s[1] < s[0]) {
+                    while (run < P && s[run] < s[run - 1]) ++run;
+                    for (int a = 0, b = run - 1; a < b; ++a, --b) {
+                        const double t = s[a];
+                        s[a] = s[b];
+                        s[b] = t;
+                    }
+                } else {
+                    while (run < P && !(s[run] < s[run - 1])) ++run;
+                }
+            }
+            for (int st = run; st < P; ++st) {             // binarysort of the rest into the run
+                const double pivot = s[st];
+                int l = 0, r = st;
+                do {
+                    const int m = l + ((r - l) >> 1);
+                    if (pivot < s[m]) r = m;
+                    else l = m + 1;
+                } while (l < r);
+                for (int k = st; k > l; --k) s[k] = s[k - 1];
+                s[l] = pivot;
+            }
+            if (s[1] - s[0] < ep.threshold) result = ep.noresult;
+        }
+    } else {
+        const int i0 = ep.ref_off[best], n1 = ep.ref_off[best + 1] - i0;
+        const bool nan_i = __shfl_sync(full, has_nan, best);
+        for (int j = 0; j < P; ++j) {
+            const bool nan_j = __shfl_sync(full, has_nan, j);
+            if (j == best || nan_i || nan_j) continue;     // scipy propagates nan: p = nan, and nan > threshold is false
+            const int j0 = ep.ref_off[j], n2 = ep.ref_off[j + 1] - j0;
+            int two_s = 0;
+            for (int a = lane; a < n1; a += 32) {
+                const double v = x[i0 + a];
+                int less = 0, eq = 0;
+                for (int b = 0; b < n1; ++b) {
+                    less += (x[i0 + b] < v) ? 1 : 0;
+                    eq += (x[i0 + b] == v) ? 1 : 0;
+                }
+                for (int b = 0; b < n2; ++b) {
+                    less += (x[j0 + b] < v) ? 1 : 0;
+                    eq += (x[j0 + b] == v) ? 1 : 0;
+                }
+                two_s += 2 * less + eq + 1;
+            }
+#pragma unroll
+            for (int d = 16; d >= 1; d >>= 1) two_s += __shfl_xor_sync(full, two_s, d);
+            // ranksums: z = (s - n1 (n1 + n2 + 1) / 2.0) / sqrt(n1 n2 (n1 + n2 + 1) / 12.0), integer products as Python ints
+            const double expected = (double)((long long)n1 * (n1 + n2 + 1)) / 2.0;
+            const double z = (0.5 * (double)two_s - expected) / sqrt((double)((long long)n1 * n2 * (n1 + n2 + 1)) / 12.0);
+            const double p = normcdf(z);
+            if (p > ep.threshold) result = ep.noresult;
+            if (lane == j) pv = p;
+        }
+    }
+    const size_t row = (size_t)wb * ep.n_query + q;
+    if (lane == 0) ep.out[row] = result;
+    if (lane < P) {
+        if (ep.means) ep.means[row * P + lane] = mean;
+        if (ep.pvals) ep.pvals[row * P + lane] = pv;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
 // host orchestration
 //
@@ -1284,6 +1455,84 @@ extern "C" int pg_pairdist(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_ind, i
         }));
         // n_ind^2 doubles per window, possibly into pageable memory: staged copies
         return copy_rows_back(ctx, wins, b0, nb, ctx->out_d.p, dist, nn * 8, true);
+    });
+}
+
+extern "C" int pg_distpaint(pg_ctx* ctx, int32_t n_query, const int32_t* query_hap, int32_t P, const int32_t* ref_off,
+                            const int32_t* ref_hap, int32_t min_sites, int32_t mode, double threshold, int32_t noresult,
+                            int32_t* out, double* means, double* pvals) {
+    PG_CHECK(ctx && query_hap && ref_off && ref_hap && out, "pg_distpaint: null argument");
+    PG_CHECK(ctx->H > 0, "pg_distpaint: upload genotypes first");
+    PG_CHECK(n_query >= 1, "pg_distpaint: n_query must be >= 1");
+    PG_CHECK(P >= 1 && P <= PAINT_MAX_POPS, "pg_distpaint: P=%d populations; the epilogue takes 1 to %d (one lane each)", P,
+             PAINT_MAX_POPS);
+    PG_CHECK(mode == 0 || mode == 1, "pg_distpaint: mode %d is neither 0 (rank-sum rule) nor 1 (delta rule)", mode);
+    PG_CHECK(mode == 0 || P >= 2, "pg_distpaint: the delta rule compares the two lowest means and needs two populations");
+    PG_CHECK(min_sites >= 1, "pg_distpaint: min_sites must be >= 1");
+    PG_CHECK(ref_off[0] == 0, "pg_distpaint: ref_off[0] must be 0");
+    for (int p = 0; p < P; ++p)
+        PG_CHECK(ref_off[p + 1] > ref_off[p], "pg_distpaint: reference population %d has no member entries", p);
+    const int M = ref_off[P];
+    PG_CHECK(M <= PAINT_MAX_M, "pg_distpaint: %d member entries; at most %d fit the epilogue's shared memory (8 bytes each "
+             "per warp)", M, PAINT_MAX_M);
+    const int H = ctx->H;
+    for (int k = 0; k < M; ++k)
+        PG_CHECK(ref_hap[k] >= 0 && ref_hap[k] < H, "pg_distpaint: ref_hap[%d]=%d out of range", k, ref_hap[k]);
+    for (int k = 0; k < n_query; ++k)
+        PG_CHECK(query_hap[k] >= 0 && query_hap[k] < H, "pg_distpaint: query_hap[%d]=%d out of range", k, query_hap[k]);
+    PG_CUDA(cudaSetDevice(ctx->device));
+    pg_timings_reset(ctx);
+    if (ctx->W == 0) return PG_OK;
+    std::vector<int64_t> wins;
+    int64_t lo, hi;
+    nonempty_windows(ctx, wins, lo, hi);
+    if (wins.empty()) return PG_OK;
+    PlaneSet ps;
+    PG_TRY(build_planes(ctx, all_rows(H), lo, hi, ps));     // plane row = haplotype
+    // query rows | population offsets | member rows
+    PG_TRY(ctx->misc.ensure((size_t)(n_query + P + 1 + M) * 4 + 64));
+    int32_t* d_query = (int32_t*)ctx->misc.p;
+    int32_t* d_off = d_query + n_query;
+    int32_t* d_ref = d_off + P + 1;
+    PG_CUDA(cudaMemcpyAsync(d_query, query_hap, (size_t)n_query * 4, cudaMemcpyHostToDevice, ctx->stream));
+    PG_CUDA(cudaMemcpyAsync(d_off, ref_off, (size_t)(P + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+    PG_CUDA(cudaMemcpyAsync(d_ref, ref_hap, (size_t)M * 4, cudaMemcpyHostToDevice, ctx->stream));
+    const size_t qp = (size_t)n_query * P;
+    const int n_dbl = (means ? 1 : 0) + (pvals ? 1 : 0);
+    const size_t per_batch = pair_batch_size(ps.Hk, (size_t)n_query * 4 + qp * 8 * n_dbl);
+    PG_TRY(ctx->out_i.ensure(per_batch * n_query * 4 + 64));
+    PG_TRY(ctx->out_d.ensure(per_batch * qp * 8 * std::max(n_dbl, 1) + 64));
+    const size_t smem = (size_t)PAINT_WARPS * M * 8;
+    return for_each_batch(ctx, wins, ctx->win_lo.data(), ctx->win_hi.data(), per_batch,
+                          [&](size_t b0, size_t nb, const int64_t* d_lo, const int64_t* d_hi) {
+        int32_t *d_diff = nullptr, *d_n = nullptr;
+        PG_TRY(run_pair_batch(ctx, ps, d_lo, d_hi, (int)nb, &d_diff, &d_n));
+        PaintEpiParams ep;
+        ep.diff = d_diff;
+        ep.n = d_n;
+        ep.mid = ps.d_mid;
+        ep.Hm = ps.Hm;
+        ep.Hk = ps.Hk;
+        ep.n_query = n_query;
+        ep.query_row = d_query;
+        ep.P = P;
+        ep.M = M;
+        ep.ref_off = d_off;
+        ep.ref_row = d_ref;
+        ep.min_sites = min_sites;
+        ep.mode = mode;
+        ep.threshold = threshold;
+        ep.noresult = noresult;
+        ep.out = (int32_t*)ctx->out_i.p;
+        ep.means = means ? (double*)ctx->out_d.p : nullptr;
+        ep.pvals = pvals ? (double*)ctx->out_d.p + (means ? nb * qp : 0) : nullptr;
+        PG_TRY(pg_timed(ctx, "k2_paint_epi", [&] {
+            k2_paint_epi<<<dim3((unsigned)((n_query + PAINT_WARPS - 1) / PAINT_WARPS), (unsigned)nb), PAINT_WARPS * 32, smem,
+                           ctx->stream>>>(ep);
+        }));
+        if (means) PG_TRY(copy_rows_back(ctx, wins, b0, nb, ep.means, means, qp * 8));
+        if (pvals) PG_TRY(copy_rows_back(ctx, wins, b0, nb, ep.pvals, pvals, qp * 8));
+        return copy_rows_back(ctx, wins, b0, nb, ep.out, out, (size_t)n_query * 4);
     });
 }
 

@@ -363,9 +363,10 @@ class Engine:
     # ---- filterGenotypes.py ----
     FILTER_FORMATS = {"phased": 0, "diplo": 1, "bases": 2, "alleles": 3, "coded": 4, "count": 5}
 
-    def set_strict_ingest(self, on: bool = True):
-        """Strict genotype tokens for the next ingests (pg_ingest_set_strict)."""
-        check(self._lib.pg_ingest_set_strict(self._ctx, 1 if on else 0), "pg_ingest_set_strict")
+    def set_strict_ingest(self, on=True):
+        """Strict genotype tokens for the next ingests (pg_ingest_set_strict): True / 1 = widths and characters,
+        2 = token widths only."""
+        check(self._lib.pg_ingest_set_strict(self._ctx, int(on)), "pg_ingest_set_strict")
 
     def filter(self, spec: dict, contig_mask=None, scaf_id=None):
         """pg_filter over the sites of the last strict ingest.  spec keys: samp_hap0, samp_ploidy, pops (one list of sample
@@ -568,6 +569,28 @@ class Engine:
         check(self._lib.pg_pairdist(self._ctx, int(n_ind), _ptr(hap_ind), 1 if include_same_with_same else 0,
                                     int(min_sites or 0), _ptr(dist), _ptr(sites), _ptr(pos_sum)), "pg_pairdist")
         return dict(dist=dist, sites=sites, pos_sum=pos_sum)
+
+    def distpaint(self, query_hap, ref_off, ref_hap, min_sites: int, delta: bool = False, threshold: float = 0.05,
+                  noresult: int = -1, with_stats: bool = False):
+        """distPaint.py's assignment of every query haplotype to its nearest reference population, per window ->
+        dict(assign int32 [W, n_query]) and, with_stats, means / pvals float64 [W, n_query, P].  Populations are
+        CSR: population p's member haplotypes are ref_hap[ref_off[p]:ref_off[p + 1]] (an ordered list; duplicates count
+        twice).  delta: the delta rule with `threshold`, else the rank-sum rule with p-value threshold `threshold`.
+        Windows without sites hold noresult (and nan statistics); the caller decides what to write for them."""
+        query_hap = np.ascontiguousarray(query_hap, dtype=np.int32)
+        ref_off = np.ascontiguousarray(ref_off, dtype=np.int32)
+        ref_hap = np.ascontiguousarray(ref_hap, dtype=np.int32)
+        W, nq, P = self.W, len(query_hap), len(ref_off) - 1
+        assign = np.full((W, nq), int(noresult), dtype=np.int32)
+        means = np.full((W, nq, P), np.nan) if with_stats else None
+        pvals = np.full((W, nq, P), np.nan) if with_stats else None
+        check(self._lib.pg_distpaint(self._ctx, nq, _ptr(query_hap), P, _ptr(ref_off), _ptr(ref_hap), int(min_sites),
+                                     1 if delta else 0, float(threshold), int(noresult), _ptr(assign), _ptr(means),
+                                     _ptr(pvals)), "pg_distpaint")
+        out = dict(assign=assign)
+        if with_stats:
+            out.update(means=means, pvals=pvals)
+        return out
 
     def pairdist_cat(self, hap_ind, n_ind: int, include_same_with_same: bool = False):
         """distMat.py --windType cat: one matrix over every uploaded site (summed over the ranks of the NCCL

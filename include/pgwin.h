@@ -161,6 +161,22 @@ int pg_sfs_sparse_fetch(pg_ctx* ctx, int64_t total, int64_t* cell, int64_t* coun
 int pg_pairdist(pg_ctx* ctx, int32_t n_ind, const int32_t* hap_ind, int32_t include_same_with_same,
                 int32_t min_sites, double* dist, int64_t* n_sites, int64_t* pos_sum);
 
+/* Replaces distPaint.py's per-window loop (distPaint.py:26-44, 62-83): the nearest reference population of every query
+ * haplotype in every window, by p-distance.  Haplotypes are upload-order indices: query_hap [n_query]; population p's
+ * member entries are ref_hap[ref_off[p] .. ref_off[p+1]) (ordered, duplicates allowed; ref_off[0] = 0, every population
+ * at least one entry).  d = diff_ij / n_ij, nan when n_ij < min_sites (>= 1); a query listed as a member is at 0.0 when
+ * n_ii >= min_sites.  Population means are np.nanmean of the member distances, bit for bit; i = np.argmin of the means
+ * (the first nan, else the first minimum).  mode 0 (rank-sum rule, which_lowest_test): out = noresult when
+ * ranksums(x_i, x_j, "less").pvalue > threshold for some j != i (a list with a nan gives p = nan, which passes); mode 1
+ * (delta rule, which_lowest_delta; P >= 2): out = noresult when sorted(means)[1] - sorted(means)[0] < threshold, sorted as
+ * CPython's list.sort orders floats that may be nan.  Else out = i.  out int32 [W x n_query]; means, pvals double
+ * [W x n_query x P] (either may be NULL; pvals[.., j] = the test against population j, nan for j = i, for lists with a nan
+ * and in mode 1).  P <= 32 and ref_off[P] <= 1024 (PG_ERR before any launch).  Windows without sites are left as the
+ * caller filled them. */
+int pg_distpaint(pg_ctx* ctx, int32_t n_query, const int32_t* query_hap, int32_t P, const int32_t* ref_off,
+                 const int32_t* ref_hap, int32_t min_sites, int32_t mode, double threshold, int32_t noresult, int32_t* out,
+                 double* means, double* pvals);
+
 /* Replaces distMat.py --windType cat (distMat.py:303-314: parseGenoFile turns the WHOLE file into one window, then
  * indPairDists): dist [n_ind x n_ind] over every uploaded site.  With a communicator (pg_nccl_init, nranks > 1) the
  * uploaded sites are this rank's shard of that window: the integer pair matrices diff_ij / n_ij are added across the
@@ -278,11 +294,12 @@ int pg_ingest_meta(pg_ctx* ctx, int32_t* pos, int8_t* new_scaffold, int64_t* lin
 /* Frees the device copy of the text. */
 int pg_ingest_release(pg_ctx* ctx);
 
-/* Strict genotype tokens for the next ingests of this ctx (off by default; filterGenotypes turns it on): a token must be
+/* Strict genotype tokens for the next ingests of this ctx (off by default; filterGenotypes turns it on with on = 1): a token must be
  * exactly as wide as its sample's ploidy (2p-1 characters phased, p alleles, one letter diplo with diploid samples only), and
  * hold only A C G T N (a diplo letter of genomics.py:14 DIPLOTYPES).  The reference makes a genotype with any other character
  * missing but writes the character back out (genomics.py:351-352), which the one-hot matrix cannot do; such a line is an
- * error naming its data line.  The ingest also keeps each sample's phase character (genomics.py:335) for pg_filter_emit. */
+ * error naming its data line.  The ingest also keeps each sample's phase character (genomics.py:335) for pg_filter_emit.
+ * on = 2 keeps only the width test (distPaint.py's haploid tokens: one character; other characters read as usual). */
 int pg_ingest_set_strict(pg_ctx* ctx, int32_t on);
 
 /* ---- filterGenotypes.py ------------------------------------------------------------------------ */
