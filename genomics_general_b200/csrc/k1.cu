@@ -43,6 +43,7 @@ struct K1Params {
     int popN[PG_MAX_K1_POPS];
     // packed popgen pass: (word, mask) entries of the populations (ent_lo / ent_hi index them), words per plane
     const uint2* word_ent;
+    const uint2* bit_frag;   // varied_mma's B operand: 32 lanes per K-block of 8 words (PopTables::bit_frag)
     int wd;
     // packed pass with uniform sites elided (UniformStream): geno holds only the varied rows.  Tile t covers the sites
     // [site_lo[t], site_lo[t + 1]) (at most T = Tmax of them), holds the varied rows [row0[t], row0[t + 1]) (at most row_cap = R)
@@ -945,10 +946,11 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
 // "carries the higher of the two codes"; any other varied row is the three planes.  A tile stores its one-plane rows, then its
 // three-plane rows, each kind word-major: word x of its row j at word x * n + j of the kind's run (n rows of the kind), so
 // that the lanes reading the same word of consecutive rows read consecutive words, in distinct banks whatever the pitch.  A
-// team packs the rows onto its lanes, Gv lanes per row: the plan's lanes per site (1 at C2 and C5, where more measured
-// slower; 2 for rows of 1 KiB and more; PG_K1_UNI_GV forces 1 .. 32 for the tests), in blocks of 32 / Gv rows, the
-// one-plane rows' blocks, then the three-plane rows', block k to warp (k + tile) % wpt.  The uniform sites and every site's
-// position are not streamed: k1_finalize adds them from per-site prefix sums (UniformStream::pre).
+// team takes the one-plane rows in blocks of 32, a row per lane, counted on the tensor cores (varied_mma), then the
+// three-plane rows Gv lanes per row: the plan's lanes per site (1 at C2 and C5, where more measured slower; 2 for rows of
+// 1 KiB and more; PG_K1_UNI_GV forces 1 .. 32 for the tests), in blocks of 32 / Gv rows; block k of either kind goes to warp
+// (k + tile) % wpt, the three-plane blocks numbered on from the one-plane ones.  The uniform sites and every site's position
+// are not streamed: k1_finalize adds them from per-site prefix sums (UniformStream::pre).
 
 // this lane's entries of population X: the first one, then steps of G (wrapping inside the population), as many as
 // walk[X] >> 16 (first | count << 16: the table holds < 6144 entries).  The G lanes of a site (gsub = 0 .. G - 1) share the
@@ -1068,20 +1070,57 @@ struct BitCounts {
     __device__ __forceinline__ uint32_t c(int X, int a) const { return a == 0 ? (uint32_t)N[X] - k[X] : (a == 1 ? k[X] : 0u); }
 };
 
-// varied_counts for a one-plane row (word x at row[x * nvar]): one load, one AND, one POPC per entry
-template <int P, bool ONE>
-__device__ __forceinline__ void varied_bits(const K1Params& prm, const uint2* s_ent, const uint32_t* row, int nvar, int Gv,
-                                            int gsub, int spv, BitCounts<P>& ct) {
+// d += popc-sums of (A AND B) over 256 haplotypes, 16 rows x 8 populations (BMMA.168256.AND.POPC on sm_90a)
+__device__ __forceinline__ void bmma_and_popc(int (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint2 b) {
+    asm("mma.sync.aligned.m16n8k256.row.col.s32.b1.b1.s32.and.popc {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+        "{%0, %1, %2, %3};"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b.x), "r"(b.y));
+}
+
+// the row of its block of 32 one-plane rows whose counts a lane gets from varied_mma
+__device__ __forceinline__ int mma_row(int lane) { return (lane >> 2) + 8 * (lane & 3); }
+
+// The counts of the one-plane rows [r, r + 32) (word x of row j at rows[x * n1 + j]) on the tensor cores: k(X) is the binary
+// matrix product of the rows' bits and the populations' member bits, 16 rows x 8 populations x 256 haplotypes per mma.  The
+// block is two m16 tiles (rows r .. r + 15, r + 16 .. r + 31) over K-blocks of 8 words.  Lane (g, t) = (lane / 4, lane % 4)
+// holds words 8 kb + t and 8 kb + 4 + t of a tile's rows g and g + 8 (A) and, in s_bf[32 kb + lane], of population g's
+// members (B, build_word_tables: zero past wd words, past H, for no population and for g >= the padded populations, so that a
+// row's bits past H count for nothing).  Words past wd are not read: they lie outside the one-plane rows.  Rows past n1 read
+// row n1 - 1 instead, so every load stays in the tile's one-plane rows; their counts are dropped (add_row's owner).  Lane
+// (g, t) ends with populations 2t, 2t + 1 of the block's rows g + 8q (q = 0 .. 3), as 16-bit pairs (counts < 65536), and
+// takes those of its own row g + 8t (mma_row) in four exchanges: in exchange j it sends pair q = t ^ j to lane ^ j, and gets
+// populations 2 (t ^ j), 2 (t ^ j) + 1 of its row.
+template <int P>
+__device__ __forceinline__ void varied_mma(const uint2* s_bf, const uint32_t* rows, int n1, int wd, int r, int lane,
+                                           BitCounts<P>& ct) {
+    static_assert(P <= 4, "one-plane rows: up to 4 (padded) populations");
+    const int g = lane >> 2, t = lane & 3;
+    const int j0 = min(r + g, n1 - 1), j1 = min(r + g + 8, n1 - 1), j2 = min(r + g + 16, n1 - 1), j3 = min(r + g + 24, n1 - 1);
+    int d0[4] = {0, 0, 0, 0}, d1[4] = {0, 0, 0, 0};
+    const uint32_t* w = rows + t * n1;    // word 8 kb + t of the rows; word 8 kb + 4 + t at w + 4 n1
+    for (int kb = 0; kb * 8 < wd; ++kb, w += 8 * n1) {
+        const bool lo = kb * 8 + t < wd, hi = kb * 8 + 4 + t < wd;
+        const uint32_t* v = w + 4 * n1;
+        const uint2 b = s_bf[kb * 32 + lane];
+        bmma_and_popc(d0, lo ? w[j0] : 0u, lo ? w[j1] : 0u, hi ? v[j0] : 0u, hi ? v[j1] : 0u, b);
+        bmma_and_popc(d1, lo ? w[j2] : 0u, lo ? w[j3] : 0u, hi ? v[j2] : 0u, hi ? v[j3] : 0u, b);
+    }
+    const uint32_t pk[4] = {(uint32_t)d0[0] | (uint32_t)d0[1] << 16, (uint32_t)d0[2] | (uint32_t)d0[3] << 16,
+                            (uint32_t)d1[0] | (uint32_t)d1[1] << 16, (uint32_t)d1[2] | (uint32_t)d1[3] << 16};
+    uint32_t k01 = 0u, k23 = 0u;
 #pragma unroll
-    for (int X = 0; X < P; ++X) {
-        uint32_t a = 0u;
-#pragma unroll 1
-        for (int e = prm.ent_lo[X] + (ONE ? 0 : gsub); e < prm.ent_hi[X]; e += (ONE ? 1 : Gv)) {
-            const uint2 em = s_ent[e];
-            a += __popc(row[em.x * nvar] & em.y);
-        }
-        for (int d = spv; !ONE && d < 32; d <<= 1) a += __shfl_xor_sync(0xffffffffu, a, d);
-        ct.set(X, a);
+    for (int j = 0; j < 4; ++j) {
+        const int q = t ^ j;
+        const uint32_t v = __shfl_xor_sync(0xffffffffu, (q & 2) ? ((q & 1) ? pk[3] : pk[2]) : ((q & 1) ? pk[1] : pk[0]), j);
+        if (q == 0) k01 = v;
+        if (q == 1) k23 = v;
+    }
+    ct.set(0, k01 & 0xffffu);
+    ct.set(1, k01 >> 16);
+    if constexpr (P > 2) {
+        ct.set(2, k23 & 0xffffu);
+        ct.set(3, k23 >> 16);
     }
 }
 
@@ -1134,6 +1173,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     volatile uint32_t* s_nvar = reinterpret_cast<volatile uint32_t*>(s_issued + 8);   // UNI: n1 | n3 << 16 [stages]
     volatile long long* s_site0 = reinterpret_cast<volatile long long*>(s_issued + 16);   // UNI: first site [stages]
     uint2* s_ent = reinterpret_cast<uint2*>(smem + (size_t)prm.stages * prm.tile_bytes + 256);
+    uint2* s_bf = s_ent + prm.n_ent;                                  // UNI, P < 8: varied_mma's B operand
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.x, B = gridDim.x;
@@ -1141,6 +1181,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
     const int ntiles = (int)(t1 - t0);
 
     for (int e = tid; e < prm.n_ent; e += K1_THREADS) s_ent[e] = prm.word_ent[e];
+    if constexpr (UNI && P < 8)
+        for (int e = tid; e < (prm.wd + 7) / 8 * 32; e += K1_THREADS) s_bf[e] = prm.bit_frag[e];
     const int Gv = prm.uni_gv > 0 ? prm.uni_gv : prm.G;                    // UNI: lanes per varied row, the plan's per site
     if (tid == 0) {
         for (int s = 0; s < prm.stages; ++s) {
@@ -1268,20 +1310,19 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             const uint32_t sizes = s_nvar[stage];
             const int n1 = (int)(sizes & 0xffffu), n3 = (int)(sizes >> 16);
             const uint16_t* s_slot = reinterpret_cast<const uint16_t*>(tile + (size_t)prm.row_cap * prm.pitch);
-            // block k of the tile goes to warp (k + rot) % wpt: the one-plane rows' blocks first, then the three-plane rows'
-            const int rot = (int)((t0 + it) % wpt), nb1 = (n1 + spv - 1) / spv;
+            // block k of the tile goes to warp (k + rot) % wpt: the one-plane rows' blocks of 32 first, then the three-plane
+            // rows' blocks of spv
+            const int rot = (int)((t0 + it) % wpt), nb1 = (n1 + 31) / 32;
 
-            // ---- one-plane rows (none at 8 populations: uniform_prepare streams three planes there) ----
-            for (int r = ((lw - rot + wpt) % wpt) * spv; P < 8 && r < n1; r += wpt * spv) {
-                const int rw = r + sl;
-                const bool valid = rw < n1;
-                const bool owner = valid && (gsub == 0);
-                const uint32_t* row = reinterpret_cast<const uint32_t*>(tile) + (valid ? rw : r);
-                BitCounts<P> ct;
-                ct.N = prm.popN;
-                if (Gv == 1) varied_bits<P, true>(prm, s_ent, row, n1, 1, 0, 32, ct);
-                else varied_bits<P, false>(prm, s_ent, row, n1, Gv, gsub, spv, ct);
-                add_row(tile_site0 + (valid ? s_slot[rw] : 0), owner, ct, false);
+            // ---- one-plane rows, a row per lane (none at 8 populations: uniform_prepare streams three planes there) ----
+            if constexpr (P < 8) {
+                for (int r = ((lw - rot + wpt) % wpt) * 32; r < n1; r += wpt * 32) {
+                    const int rw = r + mma_row(lane);
+                    BitCounts<P> ct;
+                    ct.N = prm.popN;
+                    varied_mma<P>(s_bf, reinterpret_cast<const uint32_t*>(tile), n1, prm.wd, r, lane, ct);
+                    add_row(tile_site0 + (rw < n1 ? s_slot[rw] : 0), rw < n1, ct, false);
+                }
             }
 
             // ---- three-plane rows, behind the one-plane rows' words rounded up to 16 bytes ----
@@ -1542,18 +1583,22 @@ struct PopTables {
     std::vector<int32_t> ent_chunk;
     std::vector<uint32_t> ent_mask;   // 4 words per entry
     std::vector<uint32_t> word_ent;   // packed pass: (word, mask) per entry, instead of ent_chunk / ent_mask
+    std::vector<uint32_t> bit_frag;   // packed pass: varied_mma's B operand, 2 words per lane and K-block
     int ent_lo[PG_MAX_K1_POPS], ent_hi[PG_MAX_K1_POPS], full_lo[PG_MAX_K1_POPS], full_hi[PG_MAX_K1_POPS];
     int popN[PG_MAX_K1_POPS];
 };
 
 // The packed pass's form of the tables: population X is entries [ent_lo[X], ent_hi[X]) of word_ent, one per 32-haplotype
-// word it has a member in, with the mask of its members.
+// word it has a member in, with the mask of its members.  bit_frag holds the same masks in the order of an mma B operand
+// (varied_mma): for K-block kb (words 8 kb .. 8 kb + 7) and lane 4 X + t, population X's masks of words 8 kb + t and
+// 8 kb + 4 + t, zero past wd words and for lanes 4 X + t with X >= Ppad.
 void build_word_tables(const std::vector<int32_t>& hap_pop_local, int H, int Ppad, PopTables& t) {
     t.ent_chunk.clear();
     t.ent_mask.clear();
     t.word_ent.clear();
     for (int X = 0; X < PG_MAX_K1_POPS; ++X) t.ent_lo[X] = t.ent_hi[X] = t.full_lo[X] = t.full_hi[X] = t.popN[X] = 0;
     const int wd = (H + 31) / 32;
+    t.bit_frag.assign((size_t)(wd + 7) / 8 * 64, 0u);
     for (int X = 0; X < Ppad; ++X) {
         std::vector<uint32_t> m(wd, 0u);
         for (int h = 0; h < H; ++h)
@@ -1562,11 +1607,13 @@ void build_word_tables(const std::vector<int32_t>& hap_pop_local, int H, int Ppa
                 ++t.popN[X];
             }
         t.ent_lo[X] = (int)t.word_ent.size() / 2;
-        for (int w = 0; w < wd; ++w)
+        for (int w = 0; w < wd; ++w) {
             if (m[w]) {
                 t.word_ent.push_back((uint32_t)w);
                 t.word_ent.push_back(m[w]);
             }
+            t.bit_frag[((size_t)(w / 8) * 32 + 4 * X + w % 4) * 2 + (w % 8) / 4] = m[w];
+        }
         t.ent_hi[X] = (int)t.word_ent.size() / 2;
     }
 }
@@ -1678,12 +1725,13 @@ int seg_of(const std::vector<int64_t>& brk, int64_t site) {
 }
 
 // device layout of the uploaded tables inside K1Cache::tables:
-//   [ent_mask (16B each)] [ent_chunk] [word_ent (8B each)] [brk] [the launch's SlotTables] [win_seg_lo] [win_seg_hi] [win_lo]
-//   [win_hi]
+//   [ent_mask (16B each)] [ent_chunk] [word_ent (8B each)] [bit_frag (8B each)] [brk] [the launch's SlotTables] [win_seg_lo]
+//   [win_seg_hi] [win_lo] [win_hi]
 struct DevTables {
     uint4* ent_mask;
     int32_t* ent_chunk;
     uint2* word_ent;
+    uint2* bit_frag;
     int64_t* brk;
     int32_t* win_seg_lo;
     int32_t* win_seg_hi;
@@ -1898,11 +1946,11 @@ __global__ void __launch_bounds__(256) k1_uni_bounds(const int64_t* __restrict__
 // launch when the windows (epoch), the stream (serial), the slot width or the ring changed.
 struct UniformPass {
     K1Plan plan;              // the cache's plan (its G, wpt and warps serve the stream)
-    int table_bytes = 0;      // shared-memory bytes of plan's tables
+    int table_bytes = 0;      // shared-memory bytes of the stream kernel's tables (plan's, and varied_mma's B operand)
     int R = 0, Tmax = 0, stages = 0, stage_bytes = 0;   // row budget, tile bound, and ring (uni_geometry)
-    // complete biallelic rows as one plane: below 8 (padded) populations.  At 8 the one-plane walk was slower than the
-    // three-plane one (C5, H100 80GB HBM3, 700 W: 0.963 against 0.884 ms) and spilled more, so there every varied row is
-    // streamed as three planes and the kernel has no one-plane walk
+    // complete biallelic rows as one plane: below 8 (padded) populations.  At 8 the one-plane walk that preceded varied_mma
+    // was slower than the three-plane one (C5, H100 80GB HBM3, 700 W: 0.963 against 0.884 ms) and spilled more, so there
+    // every varied row is streamed as three planes and the kernel has no one-plane rows
     bool one_plane = true;
     int wd = 0;                     // words per plane
     bool bits = false, words = false;   // this call: one-plane rows; tiles by a budget of row words (uni_geometry)
@@ -2018,6 +2066,7 @@ void fill_params(K1Params& p, const pg_ctx* ctx, const K1Plan& pl, const PopTabl
     p.ent_chunk = dt.ent_chunk;
     p.ent_mask = dt.ent_mask;
     p.word_ent = dt.word_ent;
+    p.bit_frag = dt.bit_frag;
     p.wd = (ctx->H + 31) / 32;
     p.n_ent = packed ? (int)pt.word_ent.size() / 2 : (int)pt.ent_chunk.size();
     for (int X = 0; X < PG_MAX_K1_POPS; ++X) {
@@ -2054,8 +2103,8 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
     for (int b = 0; b <= B; ++b) bound[b] = std::min<int64_t>((int64_t)b * pl.num_tiles / B * pl.T, ctx->S);
     HostSlots hs;
     slot_tables(ctx->brk, bound, nw, Q, hs);
-    size_t bytes = 4096 + pt.ent_mask.size() * 4 + pt.ent_chunk.size() * 4 + pt.word_ent.size() * 4 + ctx->brk.size() * 8 +
-                   hs.bytes() + (size_t)ctx->W * 24 + 13 * 16;
+    size_t bytes = 4096 + pt.ent_mask.size() * 4 + pt.ent_chunk.size() * 4 + pt.word_ent.size() * 4 + pt.bit_frag.size() * 4 +
+                   ctx->brk.size() * 8 + hs.bytes() + (size_t)ctx->W * 24 + 14 * 16;
     PG_TRY(c.tables.ensure(bytes));
     uint8_t* base = (uint8_t*)c.tables.p;
     size_t o = 0;
@@ -2066,6 +2115,9 @@ int prepare_windowed(pg_ctx* ctx, K1Cache& c, const std::vector<int32_t>& hap_po
     uint32_t* d_word_ent = nullptr;
     PG_TRY(push(ctx, base, o, pt.word_ent.data(), pt.word_ent.size(), &d_word_ent));
     dt.word_ent = reinterpret_cast<uint2*>(d_word_ent);
+    uint32_t* d_bit_frag = nullptr;
+    PG_TRY(push(ctx, base, o, pt.bit_frag.data(), pt.bit_frag.size(), &d_bit_frag));
+    dt.bit_frag = reinterpret_cast<uint2*>(d_bit_frag);
     PG_TRY(push(ctx, base, o, ctx->brk.data(), ctx->brk.size(), &dt.brk));
     PG_TRY(push_slots(ctx, base, o, hs, L.slots));
     PG_TRY(push(ctx, base, o, ctx->win_seg_lo.data(), ctx->win_seg_lo.size(), &dt.win_seg_lo));
@@ -2540,10 +2592,11 @@ void pg_k1_cache_free(pg_ctx* ctx) {
 // pg_popgen
 // ================================================================================================
 // Enqueue the site pass + finalize on the ctx stream WITHOUT synchronising; *h_count (pinned) holds the number of
-// windows routed to the pairwise path once the stream has been synchronised (nullptr when nothing was launched).
+// windows routed to the pairwise path once the stream has been synchronised (nullptr when nothing was launched).  A null
+// h_count (a caller that reads the routing off the records' path column) skips that counter's read-back.
 int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t force_path, void* d_rec, int** h_count) {
-    PG_CHECK(ctx && d_rec && h_count, "pg_popgen_device: null argument");
-    *h_count = nullptr;
+    PG_CHECK(ctx && d_rec, "pg_popgen_device: null argument");
+    if (h_count) *h_count = nullptr;
     PG_CHECK(ctx->P >= 1, "pg_popgen: call pg_set_pops first");
     PG_CHECK(force_path == 0 || force_path == 2, "pg_popgen: force_path must be 0 or 2");
     PG_CHECK(ctx->P <= PG_MAX_POPS, "pg_popgen: P=%d > %d populations", ctx->P, PG_MAX_POPS);
@@ -2596,9 +2649,10 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
             c.lanepop = false;
             const int nw = k1_nw_for(ctx->packed_pitch, false);
             PG_TRY(prepare_windowed(ctx, c, pop_map, Pp, Q, nw, /*force_G=*/0, /*packed=*/true));
-            u.table_bytes = table_bytes_of(c.pt);
-            u.plan = c.L.plan;
             u.one_plane = Pp < 8;
+            // the stream's kernel also keeps varied_mma's B operand in shared memory, where it has one-plane rows
+            u.table_bytes = table_bytes_of(c.pt) + (u.one_plane ? (int)c.pt.bit_frag.size() * 4 : 0);
+            u.plan = c.L.plan;
             u.wd = (ctx->H + 31) / 32;
             u.slots_epoch = 0;                                  // u.L follows c.L
         } else {
@@ -2663,6 +2717,7 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     fp.path = d_path;
     fp.n_pairwise = d_cnt;
     PG_TRY(launch_finalize<MODE_POPGEN>(ctx, fp));
+    if (!h_count) return PG_OK;
     void* hp = nullptr;
     PG_TRY(pg_pinned(ctx, (size_t)W * 4 + 256, &hp));
     int* h_cnt = (int*)hp;

@@ -213,8 +213,8 @@ extern "C" int pg_popgen_gather_begin(pg_ctx* ctx, int32_t min_sites, double min
     unsigned long long* mine = base + slot_words * (size_t)rank;
     // the finalize writes rows < W only: rows of an earlier batch with more windows must not reach the table
     PG_CUDA(cudaMemsetAsync(mine + (size_t)ctx->W * RC, 0, (size_t)(w_max - ctx->W) * RC * 8, ctx->stream));
-    int* h_cnt = nullptr;
-    PG_TRY(pg_popgen_enqueue(ctx, min_sites, min_data, 0, mine, &h_cnt));
+    // `end` reads the routed windows off the gathered path column: no counter read-back
+    PG_TRY(pg_popgen_enqueue(ctx, min_sites, min_data, 0, mine, nullptr));
     PG_CUDA(cudaEventRecord(ctx->g_rec[slot], ctx->stream));
     PG_CUDA(cudaStreamWaitEvent(ctx->gather_stream, ctx->g_rec[slot], 0));
     if (ranks > 1) {
