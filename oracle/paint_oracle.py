@@ -87,13 +87,14 @@ def pair_counts(win):
 
 def member_distances(diff, n, i, members, min_sites):
     """Alignment.pairDist(i, j) = np.mean of the mismatches at the jointly called sites (diff / n, one division), nan when
-    fewer than minSites (distPaint.py:73-76)"""
-    out = []
-    for j in members:
-        with np.errstate(all="ignore"):
-            d = np.float64(diff[i, j]) / np.float64(n[i, j])
-        out.append(d if n[i, j] >= min_sites else np.nan)
-    return out
+    fewer than minSites (distPaint.py:73-76); one float64 array in member order, which np.nanmean and ranksums read as
+    they read the reference's list of np.float64"""
+    m = np.asarray(members, dtype=np.int64)
+    nij = n[i, m]
+    with np.errstate(all="ignore"):
+        d = diff[i, m].astype(np.float64) / nij.astype(np.float64)
+    d[nij < min_sites] = np.nan
+    return d
 
 
 def paint_window(win, query_hap, pops, min_sites, delta=None, p_threshold=0.05, noresult=-1):

@@ -96,9 +96,12 @@ def test_member_limit_and_population_limit():
             ref_off = np.array([0, M // 2, M], dtype=np.int32)
             if M == 1024:
                 r = eng.distpaint(np.arange(H), ref_off, ref_hap, 1, with_stats=True)
-                a, m, _ = po.paint_window(g, list(range(H)), [list(ref_hap[:M // 2]), list(ref_hap[M // 2:])], 1)
+                a, m, p = po.paint_window(g, list(range(H)), [list(ref_hap[:M // 2]), list(ref_hap[M // 2:])], 1)
                 assert np.array_equal(r["assign"][0], a)
                 _same_bits(r["means"][0], m, M)
+                got = r["pvals"][0]                        # ranks over 512 + 512 members: 16 rounds of the lanes
+                assert np.array_equal(np.isnan(got), np.isnan(p)) and (~np.isnan(p)).sum() == H
+                np.testing.assert_allclose(got[~np.isnan(p)], p[~np.isnan(p)], rtol=1e-12, atol=0)
             else:
                 with pytest.raises(PgError, match="1025 member entries; at most 1024"):
                     eng.distpaint(np.arange(H), ref_off, ref_hap, 1)

@@ -14,9 +14,12 @@ from oracle import paint_oracle as po
 
 CASES = json.load(open(os.path.join(GOLDEN, "cases7.json")))
 DIR = os.path.join(GOLDEN, "paint7")
+# populations of 9, 130 and 300 samples (oracle/make_golden8.py)
+CASES8 = json.load(open(os.path.join(GOLDEN, "cases8.json")))
+DIR8 = os.path.join(GOLDEN, "paint8")
 
 
-def run_cli(case, tmp_path, monkeypatch=None, engine=None, extra_env=None):
+def run_cli(case, tmp_path, monkeypatch=None, engine=None, extra_env=None, directory=DIR):
     from genomics_general_b200.cli import _common, distPaint
     if engine is not None:
         monkeypatch.setattr(distPaint, "Engine", engine)
@@ -26,22 +29,28 @@ def run_cli(case, tmp_path, monkeypatch=None, engine=None, extra_env=None):
     for k, v in (extra_env or {}).items():
         monkeypatch.setenv(k, v)
     out = str(tmp_path / (case["name"] + (".tsv.gz" if case["gz"] else ".tsv")))
-    args = [os.path.join(DIR, a) if a in ("windows.txt", "pops.txt") else a for a in case["args"]]
-    distPaint.main(["-g", os.path.join(DIR, case["input"]), "-o", out] + args)
+    args = [os.path.join(directory, a) if a in ("windows.txt", "pops.txt") else a for a in case["args"]]
+    distPaint.main(["-g", os.path.join(directory, case["input"]), "-o", out] + args)
     if case["gz"]:
         with gzip.open(out, "rb") as f:
             return f.read()
     return open(out, "rb").read()
 
 
-def expected(case):
-    return open(os.path.join(DIR, case["expected"]), "rb").read()
+def expected(case, directory=DIR):
+    return open(os.path.join(directory, case["expected"]), "rb").read()
 
 
 @pytest.mark.parametrize("case", CASES, ids=[c["name"] for c in CASES])
 def test_cli_on_oracle_engine_matches_reference(case, tmp_path, monkeypatch):
     from oracle_engine_paint import PaintOracleEngine
     assert run_cli(case, tmp_path, monkeypatch, PaintOracleEngine) == expected(case)
+
+
+@pytest.mark.parametrize("case", CASES8, ids=[c["name"] for c in CASES8])
+def test_cli_on_oracle_engine_matches_reference_at_large_populations(case, tmp_path, monkeypatch):
+    from oracle_engine_paint import PaintOracleEngine
+    assert run_cli(case, tmp_path, monkeypatch, PaintOracleEngine, directory=DIR8) == expected(case, DIR8)
 
 
 def _values(rng, n):
