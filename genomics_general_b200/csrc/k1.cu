@@ -946,11 +946,11 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_lp(const __grid
 // "carries the higher of the two codes"; any other varied row is the three planes.  A tile stores its one-plane rows, then its
 // three-plane rows, each kind word-major: word x of its row j at word x * n + j of the kind's run (n rows of the kind), so
 // that the lanes reading the same word of consecutive rows read consecutive words, in distinct banks whatever the pitch.  A
-// team takes the one-plane rows in blocks of 32, a row per lane, counted on the tensor cores (varied_mma), then the
-// three-plane rows Gv lanes per row: the plan's lanes per site (1 at C2 and C5, where more measured slower; 2 for rows of
-// 1 KiB and more; PG_K1_UNI_GV forces 1 .. 32 for the tests), in blocks of 32 / Gv rows; block k of either kind goes to warp
-// (k + tile) % wpt, the three-plane blocks numbered on from the one-plane ones.  The uniform sites and every site's position
-// are not streamed: k1_finalize adds them from per-site prefix sums (UniformStream::pre).
+// team takes the one-plane rows in blocks of 32, counted on the tensor cores (varied_mma, a row per lane; or gram_counts and
+// the Gram of GRAM), then the three-plane rows Gv lanes per row: the plan's lanes per site (1 at C2 and C5, where more
+// measured slower; 2 for rows of 1 KiB and more; PG_K1_UNI_GV forces 1 .. 32 for the tests), in blocks of 32 / Gv rows; block
+// k of either kind goes to warp (k + tile) % wpt, the three-plane blocks numbered on from the one-plane ones.  The uniform
+// sites and every site's position are not streamed: k1_finalize adds them from per-site prefix sums (UniformStream::pre).
 
 // this lane's entries of population X: the first one, then steps of G (wrapping inside the population), as many as
 // walk[X] >> 16 (first | count << 16: the table holds < 6144 entries).  The G lanes of a site (gsub = 0 .. G - 1) share the
@@ -1124,6 +1124,46 @@ __device__ __forceinline__ void varied_mma(const uint2* s_bf, const uint32_t* ro
     }
 }
 
+// The counts of the one-plane rows [r, r + 32) as bytes (every population has at most 255 haplotypes), populations as M and
+// rows as N: k(X) is the binary product of the populations' member bits (A: s_bf[32 kb + lane] holds population g's words
+// 8 kb + t and 8 kb + 4 + t, A rows 8 .. 15 are zero) and the bits of 8 rows (B), in four n-tiles of 8 rows.  Lane (g, t)
+// loads words 8 kb + t and 8 kb + 4 + t of row r + 8 j + g of n-tile j, zero past n1, and ends with k(g) of the block's rows
+// 8 j + 2 t and 8 j + 2 t + 1: rows 2 t, 2 t + 1, 8 + 2 t, 9 + 2 t in the bytes of k0, the same rows + 16 in k1 (gram_row).
+__device__ __forceinline__ void gram_counts(const uint2* s_bf, const uint32_t* rows, int n1, int wd, int r, int lane,
+                                            uint32_t& k0, uint32_t& k1) {
+    const int g = lane >> 2, t = lane & 3, j = r + g;
+    const bool v0 = j < n1, v1 = j + 8 < n1, v2 = j + 16 < n1, v3 = j + 24 < n1;
+    int d[4][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}};
+    const uint32_t* w = rows + t * n1 + j;    // word 8 kb + t of row j; word 8 kb + 4 + t at w + 4 n1
+    for (int kb = 0; kb * 8 < wd; ++kb, w += 8 * n1) {
+        const bool lo = kb * 8 + t < wd, hi = kb * 8 + 4 + t < wd;
+        const uint32_t* v = w + 4 * n1;
+        const uint2 a = s_bf[kb * 32 + lane];
+        bmma_and_popc(d[0], a.x, 0u, a.y, 0u, make_uint2(lo && v0 ? w[0] : 0u, hi && v0 ? v[0] : 0u));
+        bmma_and_popc(d[1], a.x, 0u, a.y, 0u, make_uint2(lo && v1 ? w[8] : 0u, hi && v1 ? v[8] : 0u));
+        bmma_and_popc(d[2], a.x, 0u, a.y, 0u, make_uint2(lo && v2 ? w[16] : 0u, hi && v2 ? v[16] : 0u));
+        bmma_and_popc(d[3], a.x, 0u, a.y, 0u, make_uint2(lo && v3 ? w[24] : 0u, hi && v3 ? v[24] : 0u));
+    }
+    k0 = (uint32_t)d[0][0] | (uint32_t)d[0][1] << 8 | (uint32_t)d[1][0] << 16 | (uint32_t)d[1][1] << 24;
+    k1 = (uint32_t)d[2][0] | (uint32_t)d[2][1] << 8 | (uint32_t)d[3][0] << 16 | (uint32_t)d[3][1] << 24;
+}
+
+// the bytes of gram_counts' k0 (half = 0) or k1 (half = 1) in lane t whose rows are in the row mask m (bit i: row i of the block)
+__device__ __forceinline__ uint32_t gram_bytes(uint32_t m, int t, int half) {
+    const uint32_t x = m >> (2 * t + 16 * half);
+    const uint32_t b = (x & 3u) | ((x >> 6) & 0xcu);           // rows 2t, 2t + 1, 8 + 2t, 9 + 2t
+    return ((b * 0x00204081u) & 0x01010101u) * 0xffu;          // bit i to byte i
+}
+
+// d[0..1] += row g, columns 2t, 2t + 1 of the s32 product of A (16 x 32 bytes) and B (32 x 8 bytes), A rows 8 .. 15 zero
+// (IMMA.16832.U8.U8 on sm_90a)
+__device__ __forceinline__ void imma_u8(int (&d)[2], uint32_t a0, uint32_t a2, uint32_t b0, uint32_t b1) {
+    int z0, z1;
+    asm("mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %10, %10};"
+        : "+r"(d[0]), "+r"(d[1]), "=r"(z0), "=r"(z1)
+        : "r"(a0), "r"(0u), "r"(a2), "r"(0u), "r"(b0), "r"(b1), "r"(0));
+}
+
 // whether the site (of the lane that owns it) has every haplotype of every population, or some but not all of them
 template <int P, class CT>
 __device__ __forceinline__ void packed_class(const K1Params& prm, bool owner, const CT& ct, bool& pres, bool& ragged) {
@@ -1160,9 +1200,18 @@ __device__ __forceinline__ void packed_add(ACC& acc, bool pres, bool ragged, con
         }
 }
 
-template <int MODE, int P, int NW, bool UNI = false>
+// GRAM (UNI, P < 8, every population <= 255 haplotypes: K1Params::bytes): the one-plane rows are not added row by row.  A
+// complete biallelic row has every haplotype present and none ragged, and its counts are c(X, 0) = N_X - k_X, c(X, 1) = k_X,
+// so a run of n such rows in one segment adds
+//   sum c_Xa^2 = n N_X^2 - 2 N_X sum k_X + 2 sum k_X^2,   sum c_Xa c_Ya = n N_X N_Y - N_X sum k_Y - N_Y sum k_X + 2 sum k_X k_Y,
+// exact integers, equal to what the rows add one by one.  The warp keeps the Gram D = K^T K of its rows' byte counts in the
+// tensor cores' s32 accumulator (gram_counts, then one IMMA per block of 32 rows), with a column of ones per valid row
+// (lane g = 4 of the operand) for sum k_X and n, and folds D into its slot (gram_flush) when the rows move to another
+// segment or before an entry could overflow.
+template <int MODE, int P, int NW, bool UNI = false, bool GRAM = false>
 __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __grid_constant__ K1Params prm) {
     static_assert(MODE == MODE_POPGEN || MODE == MODE_POPGEN_FREQ, "packed site pass: popgen modes");
+    static_assert(!GRAM || (UNI && P <= 4), "the Gram of the one-plane rows: varied-row stream, up to 4 (padded) populations");
     constexpr int K1_THREADS = (NW + 1) * 32;
     constexpr int QI = ModeTraits<MODE, P>::QI, QU = ModeTraits<MODE, P>::QU;
     extern __shared__ __align__(128) uint8_t smem[];
@@ -1299,6 +1348,72 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             packed_add<MODE, P>(acc, pres, ragged, ct);
         };
 
+        // GRAM: the Gram's own segment (warp-uniform; the warp's one-plane rows come in site order), D[g][2t], D[g][2t + 1]
+        // in lane (g, t), the rows it holds, and per lane the rows with 0 < k_g < N_g (popFreq's segregating sites)
+        int gseg = -1, grows = 0;
+        int64_t gseg_end = -1;
+        int gd[2] = {0, 0};
+        uint32_t gfreq = 0u;
+        const uint32_t gN4 = (lane >> 2) < P ? (uint32_t)prm.popN[min(lane >> 2, P - 1)] * 0x01010101u : 0u;
+        // the entries of D are below 2^31 while the rows number at most 2^31 / maxN^2 (acc_limit is 2^32 / maxN^2)
+        const int glimit = max(prm.acc_limit / 2, 32);
+        // lane q < QU adds slot word QI + q: the sums of population X = Y (q < P), of the pair X < Y (then), or X's segregating
+        // sites; lane 31 adds the complete sites (word 0)
+        auto gram_flush = [&]() {
+            if (grows == 0) return;
+            __syncwarp();       // the lanes' read-modify-writes after warp_flush's, of the same slot
+            int X = 0, Y = 0;
+            long long NX = 0, NY = 0;
+            int k = P;
+#pragma unroll
+            for (int x = 0; x < P; ++x) {
+                if (lane == x || lane == P + P * (P - 1) / 2 + x) X = Y = x;
+#pragma unroll
+                for (int y = x + 1; y < P; ++y, ++k)
+                    if (lane == k) {
+                        X = x;
+                        Y = y;
+                    }
+            }
+#pragma unroll
+            for (int x = 0; x < P; ++x) {
+                if (X == x) NX = prm.popN[x];
+                if (Y == x) NY = prm.popN[x];
+            }
+            const int src = 4 * X + (Y >> 1);                                          // D[X][Y]
+            const int d0 = __shfl_sync(0xffffffffu, gd[0], src), d1 = __shfl_sync(0xffffffffu, gd[1], src);
+            const long long SX = __shfl_sync(0xffffffffu, gd[0], 4 * X + 2);           // D[X][4] = sum k_X
+            const long long SY = __shfl_sync(0xffffffffu, gd[0], 4 * Y + 2);
+            const long long n = __shfl_sync(0xffffffffu, gd[0], 18);                   // D[4][4] = rows
+            uint32_t f = gfreq;
+            f += __shfl_xor_sync(0xffffffffu, f, 1);
+            f += __shfl_xor_sync(0xffffffffu, f, 2);
+            f = __shfl_sync(0xffffffffu, f, 4 * X);
+            unsigned long long* dst = prm.part + slot_base + ((int64_t)(gseg - seg_first) * NW + warp) * (QI + QU);
+            if (lane < P + P * (P - 1) / 2)
+                dst[QI + lane] += (unsigned long long)(n * NX * NY - NX * SY - NY * SX + 2ll * ((Y & 1) ? d1 : d0));
+            else if (lane < QU)
+                dst[QI + lane] += (unsigned long long)f;
+            else if (lane == 31)
+                dst[0] += (unsigned long long)n;
+            __syncwarp();
+            gd[0] = gd[1] = 0;
+            gfreq = 0u;
+            grows = 0;
+        };
+        // the rows of the block in the row mask m (of the Gram's segment) into the Gram
+        auto gram_add = [&](uint32_t k0, uint32_t k1, uint32_t m) {
+            if (grows + __popc(m) > glimit) gram_flush();
+            grows += __popc(m);
+            const int t = lane & 3;
+            if ((lane >> 2) == 4) k0 = k1 = 0x01010101u;     // operand row / column 4: a one per row
+            k0 &= gram_bytes(m, t, 0);
+            k1 &= gram_bytes(m, t, 1);
+            imma_u8(gd, k0, k1, k0, k1);
+            if (MODE == MODE_POPGEN_FREQ)
+                gfreq += __popc((__vsetgtu4(k0, 0u) & __vsetltu4(k0, gN4)) | (__vsetgtu4(k1, 0u) & __vsetltu4(k1, gN4)) << 1);
+        };
+
         for (int it = team; it < ntiles; it += nteams) {
             const int stage = it % prm.stages;
             if (lane == 0)
@@ -1315,7 +1430,31 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             const int rot = (int)((t0 + it) % wpt), nb1 = (n1 + 31) / 32;
 
             // ---- one-plane rows, a row per lane (none at 8 populations: uniform_prepare streams three planes there) ----
-            if constexpr (P < 8) {
+            if constexpr (GRAM) {
+                for (int r = ((lw - rot + wpt) % wpt) * 32; r < n1; r += wpt * 32) {
+                    uint32_t k0, k1;
+                    gram_counts(s_bf, reinterpret_cast<const uint32_t*>(tile), n1, prm.wd, r, lane, k0, k1);
+                    const int nv = min(32, n1 - r);
+                    uint32_t pending = nv == 32 ? 0xffffffffu : (1u << nv) - 1u;
+                    if (tile_site0 + s_slot[r + nv - 1] < gseg_end) {
+                        gram_add(k0, k1, pending);      // the whole block lies in the Gram's segment
+                        continue;
+                    }
+                    // the block's rows segment by segment
+                    const int64_t site = tile_site0 + s_slot[r + min(lane, nv - 1)];
+                    while (pending) {
+                        const int64_t first = __shfl_sync(0xffffffffu, site, __ffs(pending) - 1);
+                        if (first >= gseg_end) {
+                            gram_flush();
+                            gseg = next_seg(prm.brk, prm.nseg, gseg + 1, first);
+                            gseg_end = __ldg(prm.brk + gseg + 1);
+                        }
+                        const uint32_t in = pending & __ballot_sync(0xffffffffu, site < gseg_end);
+                        gram_add(k0, k1, in);
+                        pending &= ~in;
+                    }
+                }
+            } else if constexpr (P < 8) {
                 for (int r = ((lw - rot + wpt) % wpt) * 32; r < n1; r += wpt * 32) {
                     const int rw = r + mma_row(lane);
                     BitCounts<P> ct;
@@ -1343,6 +1482,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, 1) k1_site_pass_packed(const __
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[stage]);
         }
+        if constexpr (GRAM) gram_flush();
     }
     warp_flush<QI, QU, 0>(acc, cur_seg, prm.part, slot_base, seg_first, warp, lane, NW);
 }
@@ -2181,8 +2321,14 @@ int launch_site_pass(pg_ctx* ctx, const K1Launch& L, const char* name) {
                : launch_kernel<k1_site_pass<MODE, P, 8, false>, 8>(ctx, L, name);
 }
 
+// The varied-row stream with one-plane rows and byte counts sums its one-plane rows as a Gram (k1_site_pass_packed's GRAM).
 template <int MODE, int P, bool UNI>
 int launch_site_pass_packed(pg_ctx* ctx, const K1Launch& L, const char* name) {
+    if constexpr (UNI && P < 8) {
+        if (L.prm.bytes)
+            return L.prm.nw == 12 ? launch_kernel<k1_site_pass_packed<MODE, P, 12, true, true>, 12>(ctx, L, name)
+                                  : launch_kernel<k1_site_pass_packed<MODE, P, 8, true, true>, 8>(ctx, L, name);
+    }
     return L.prm.nw == 12 ? launch_kernel<k1_site_pass_packed<MODE, P, 12, UNI>, 12>(ctx, L, name)
                           : launch_kernel<k1_site_pass_packed<MODE, P, 8, UNI>, 8>(ctx, L, name);
 }
