@@ -95,6 +95,7 @@ _SIGS = {
     "pg_debug_uniform_tile": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "pg_debug_uniform_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "pg_debug_uniform_ring": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
+    "pg_debug_uniform_launch": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "pg_debug_uniform_tiles": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int32)]),
     "pg_nccl_unique_id": (C.c_int, [C.c_void_p]),

@@ -1608,7 +1608,9 @@ __global__ void __launch_bounds__(64) k1_finalize(const __grid_constant__ FinPar
                     double Sx = nan_d(), tpi = nan_d(), tw = nan_d(), tD = nan_d();
                     if (Lp >= 1 && fp.with_freq) {
                         const long long N = fp.popN[x];
-                        const long long seg = (long long)sums[3 + Pp + npp + x];
+                        // a population of one haplotype: the reference's site pi is 0 / 0 = nan, which its sitePi != 0
+                        // counts (genomics.py:1016-1017), so every complete site is segregating there and thetaW = S / 0
+                        const long long seg = N == 1 ? (long long)Lp : (long long)sums[3 + Pp + npp + x];
                         const long long pairs = (N * N * Lp - (long long)sums[3 + x]) / 2;   // sum over sites of sum_{a<b} c_a c_b
                         Sx = (double)seg;
                         tpi = (double)pairs / (.5 * (double)N * (double)(N - 1));
@@ -1904,7 +1906,7 @@ int push(pg_ctx* ctx, uint8_t* base, size_t& off, const T* src, size_t n, T** ou
 struct UniformStream {
     uint64_t gen = 0;         // ctx->data_gen it describes (0: none)
     uint64_t serial = 0;      // counts the builds (the slot tables follow it)
-    int R = 0, Tmax = 0;
+    int R = 0, Tmax = 0, ctas = 0;
     bool forced = false, bits = false, wb = false;
     bool in_use = false;      // false: too few uniform sites to pay off, or no memory; the packed pass streams every row
     int64_t varied = 0;
@@ -2071,11 +2073,12 @@ __global__ void __launch_bounds__(256) k1_uni_tiles(const int64_t* __restrict__ 
     }
 }
 
-// info[0] = tiles, info[1 + b] = the first site of CTA b's tiles for b = 0 .. B (B = min(sm, tiles) CTAs, tiles b * nt / B on)
+// info[0] = tiles, info[1 + b] = the first site of CTA b's tiles for b = 0 .. B (B = min(ctas, tiles) CTAs, tiles b * nt / B
+// on)
 __global__ void __launch_bounds__(256) k1_uni_bounds(const int64_t* __restrict__ base, int64_t ng, const int64_t* __restrict__ site_lo,
-                                                     int sm, int64_t* __restrict__ info) {
+                                                     int ctas, int64_t* __restrict__ info) {
     const int64_t nt = base[ng];
-    const int64_t B = nt < sm ? (nt > 1 ? nt : 1) : sm;
+    const int64_t B = nt < ctas ? (nt > 1 ? nt : 1) : ctas;
     for (int64_t b = threadIdx.x; b <= B; b += blockDim.x) info[1 + b] = site_lo[b * nt / B];
     if (threadIdx.x == 0) info[0] = nt;
 }
@@ -2101,6 +2104,7 @@ struct UniformPass {
     int slots_Q = 0;
     K1Launch L;
     bool last = false;        // the last popgen launch was L
+    int32_t launched[3] = {0, 0, 0};   // of L's last launch: CTAs, consumer warps per CTA, 1 for the Gram kernel
     void release() {
         us.release();
         slot_buf.release();
@@ -2322,8 +2326,14 @@ int launch_site_pass(pg_ctx* ctx, const K1Launch& L, const char* name) {
 }
 
 // The varied-row stream with one-plane rows and byte counts sums its one-plane rows as a Gram (k1_site_pass_packed's GRAM).
+// launched (may be null) receives the grid, the consumer warps and whether the Gram kernel runs.
 template <int MODE, int P, bool UNI>
-int launch_site_pass_packed(pg_ctx* ctx, const K1Launch& L, const char* name) {
+int launch_site_pass_packed(pg_ctx* ctx, const K1Launch& L, const char* name, int32_t* launched = nullptr) {
+    if (launched) {
+        launched[0] = L.plan.ctas;
+        launched[1] = L.prm.nw;
+        launched[2] = UNI && P < 8 && L.prm.bytes ? 1 : 0;
+    }
     if constexpr (UNI && P < 8) {
         if (L.prm.bytes)
             return L.prm.nw == 12 ? launch_kernel<k1_site_pass_packed<MODE, P, 12, true, true>, 12>(ctx, L, name)
@@ -2405,6 +2415,13 @@ void uni_geometry(UniformPass& u) {
     u.stages = pl.stages >= 2 ? pg_k1_ring_stages(u.stage_bytes, u.table_bytes) : 0;
 }
 
+// The stream's CTAs: one per SM, or PG_K1_UNI_CTAS (1 .. SMs), which lets the tests put many rows of one segment on a few
+// warps.  It sets both the tile ranges (k1_uni_bounds) and the grid, so that the slot tables and the kernel's t0 agree.
+int uni_ctas(const pg_ctx* ctx) {
+    const char* e = getenv("PG_K1_UNI_CTAS");
+    return (e && *e) ? std::max(1, std::min(ctx->sm_count, atoi(e))) : ctx->sm_count;
+}
+
 // (Re)builds u.us for the current data and geometry when they changed: two host synchronisations per rebuild (the count of
 // varied rows, which sizes the buffers; the count of tiles with the CTAs' first sites, which size the launch and its slots),
 // nothing on a call over unchanged data.  PG_K1_UNIFORM_FORCE keeps the stream whatever the uniform fraction (tests on missing
@@ -2414,10 +2431,12 @@ int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
     UniformStream& us = u.us;
     const bool forced = getenv("PG_K1_UNIFORM_FORCE") != nullptr;
     const bool bits = u.bits, wb = u.words;
-    const int R = u.R, Tmax = u.Tmax;
-    if (us.gen == ctx->data_gen && us.R == R && us.Tmax == Tmax && us.forced == forced && us.bits == bits && us.wb == wb)
+    const int R = u.R, Tmax = u.Tmax, ctas = uni_ctas(ctx);
+    if (us.gen == ctx->data_gen && us.R == R && us.Tmax == Tmax && us.forced == forced && us.bits == bits && us.wb == wb &&
+        us.ctas == ctas)
         return PG_OK;
     us.wb = wb;
+    us.ctas = ctas;
     us.gen = ctx->data_gen;
     us.R = R;
     us.Tmax = Tmax;
@@ -2523,7 +2542,7 @@ int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
                                                           (uint16_t*)us.slots.p, d_n1, d_woff, ctx->d_packed, ppw, wd, bits,
                                                           (uint32_t*)us.rows.p);
     PG_CUDA(cudaGetLastError());
-    k1_uni_bounds<<<1, 256, 0, ctx->stream>>>(d_base, ng, d_site_lo, ctx->sm_count, d_info);
+    k1_uni_bounds<<<1, 256, 0, ctx->stream>>>(d_base, ng, d_site_lo, ctas, d_info);
     PG_CUDA(cudaGetLastError());
     PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, pre_bytes, uni_in, d_pre, S + 1, ctx->stream));
     PG_CUDA(cub::DeviceScan::ExclusiveSum(us.scan.p, pre_bytes, pos_in, d_pre + S + 1, S + 1, ctx->stream));
@@ -2532,7 +2551,7 @@ int uniform_prepare(pg_ctx* ctx, UniformPass& u) {
     PG_CUDA(cudaMemcpyAsync(info.data(), d_info, info.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
     PG_CUDA(cudaStreamSynchronize(ctx->stream));
     us.nt = info[0];
-    const int B = (int)std::max<int64_t>(1, std::min<int64_t>(ctx->sm_count, us.nt));
+    const int B = (int)std::max<int64_t>(1, std::min<int64_t>(ctas, us.nt));
     us.bound.assign(info.begin() + 1, info.begin() + 2 + B);
     us.in_use = true;
     return PG_OK;
@@ -2835,7 +2854,7 @@ int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t f
     PG_TRY(arm_slots(ctx, L, u.last ? u.us.rows.p : c.packed ? (const void*)ctx->d_packed : ctx->d_geno));
     PG_TRY(with_popgen_mode(wf, Pp, [&](auto M, auto PP) {
         constexpr int MODE = decltype(M)::value, PT = decltype(PP)::value;
-        if (u.last) return launch_site_pass_packed<MODE, PT, true>(ctx, L, "k1_popgen");
+        if (u.last) return launch_site_pass_packed<MODE, PT, true>(ctx, L, "k1_popgen", u.launched);
         if (c.packed) return launch_site_pass_packed<MODE, PT, false>(ctx, L, "k1_popgen");
         return launch_site_pass<MODE, PT>(ctx, L, "k1_popgen");
     }));
@@ -2898,6 +2917,14 @@ extern "C" int pg_debug_uniform_ring(pg_ctx* ctx, int32_t* out) {
     out[0] = read ? c->up.cap_rows : 0;
     out[1] = read ? c->up.stages : 0;
     out[2] = read ? c->up.stage_bytes : 0;
+    return PG_OK;
+}
+
+extern "C" int pg_debug_uniform_launch(pg_ctx* ctx, int32_t* out) {
+    PG_CHECK(ctx && out, "pg_debug_uniform_launch: null argument");
+    const K1Cache* c = static_cast<const K1Cache*>(ctx->k1_cache[0]);
+    const bool read = c && c->up.last;
+    for (int k = 0; k < 3; ++k) out[k] = read ? c->up.launched[k] : 0;
     return PG_OK;
 }
 

@@ -693,6 +693,13 @@ class Engine:
         check(self._lib.pg_debug_uniform_ring(self._ctx, v), "pg_debug_uniform_ring")
         return int(v[0]), int(v[1]), int(v[2])
 
+    def uniform_launch(self):
+        """(CTAs, consumer warps per CTA, 1 when the one-plane rows were summed as a Gram) of the varied-row stream's launch
+        in the last popgen call ((0, 0, 0) when it did not read the stream)."""
+        v = (C.c_int32 * 3)()
+        check(self._lib.pg_debug_uniform_launch(self._ctx, v), "pg_debug_uniform_launch")
+        return int(v[0]), int(v[1]), int(v[2])
+
     def uniform_tiles(self):
         """(R, Tmax, site_lo, row0) of the varied-row stream the last popgen call read: tile t covers the sites
         [site_lo[t], site_lo[t + 1]) and the varied rows [row0[t], row0[t + 1]); None when it did not read the stream."""

@@ -386,6 +386,10 @@ int pg_debug_uniform_tile(pg_ctx* ctx, int32_t* out);
 /* Ring of the varied-row stream's last popgen call: out[0] = varied rows a tile may hold (R), out[1] = stages, out[2] = bytes per
  * stage (all 0 when the last call did not read the stream). */
 int pg_debug_uniform_ring(pg_ctx* ctx, int32_t* out);
+/* Launch of the varied-row stream's last popgen call: out[0] = CTAs, out[1] = consumer warps per CTA, out[2] = 1 when the
+ * one-plane rows were summed as a Gram (every population of at most 255 haplotypes), else 0 (all 0 when the last call did
+ * not read the stream).  PG_K1_UNI_CTAS=n caps the stream's CTAs at n. */
+int pg_debug_uniform_launch(pg_ctx* ctx, int32_t* out);
 /* Tiles of the varied-row stream the last popgen call read: *ntiles, geometry[0] = R (varied rows per tile at most),
  * geometry[1] = Tmax (sites per tile at most); when cap >= *ntiles + 1, site_lo / row0 get each tile's first site / first
  * varied row and the totals (S, varied rows) at [ntiles].  All 0 when the last call did not read the stream. */

@@ -353,7 +353,9 @@ def test_natural_32bit_limit_on_the_stream(eng, monkeypatch):
     stream carries as one plane: the stream matches the oracle at the natural limit, but does not flush there.  A warp
     flushes after acc_limit + 1 of its row blocks in one segment, and at this width a tile holds one 32-row block (R = 4
     on a budget of words), so every warp of every CTA (132 x 8 on an H100) would need 6 tiles of its own in a segment:
-    about 200,000 varied rows, 6 billion genotypes.  The forced flushes are in test_forced_32bit_flush_in_the_stream."""
+    about 200,000 varied rows, 6 billion genotypes.  The forced flushes are in test_forced_32bit_flush_in_the_stream;
+    test_gpu_gram_bounds.py::test_natural_32bit_flush_on_one_cta reaches the natural flush on a stream capped at one CTA
+    (PG_K1_UNI_CTAS=1)."""
     spb.test_natural_32bit_flush_with_the_large_population_second(eng)
     assert_stream(eng, "natural limit")
     assert ring_R(eng, True) == stream_R(28010)[0] == 4 and eng.uniform_rows()[0] > 300
