@@ -114,6 +114,7 @@ _SIGS = {
     "pg_ingest_meta": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_ingest_release": (C.c_int, [C.c_void_p]),
     "pg_ingest_set_strict": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pg_debug_ingest": (C.c_int, [C.c_void_p, C.c_void_p]),
     "pg_filter": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_uint8)]),
     "pg_filter_emit": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64),
                                  C.POINTER(C.c_size_t)]),

@@ -32,8 +32,12 @@ inline bool is_ws(char c) { return c == ' ' || c == '\t' || c == '\r' || c == '\
 struct Lut {
     int8_t base[256];
     int8_t dip0[256], dip1[256];
+    uint8_t ws[256];
     Lut() {
-        for (int i = 0; i < 256; ++i) base[i] = dip0[i] = dip1[i] = -1;
+        for (int i = 0; i < 256; ++i) {
+            base[i] = dip0[i] = dip1[i] = -1;
+            ws[i] = is_ws((char)i) ? 1 : 0;
+        }
         base[(int)'A'] = 0;
         base[(int)'C'] = 1;
         base[(int)'G'] = 2;
@@ -190,9 +194,16 @@ extern "C" int pg_geno_parse(const char* buf, size_t len, int32_t fmt, int32_t n
                 new_scaffold[l] = ((q1 - q) != (sc1 - sc0) || memcmp(q, sc0, (size_t)(sc1 - sc0)) != 0) ? 1 : 0;
             }
             while (p < e && is_ws(*p)) ++p;
-            // position
+            if (p >= e) {
+                char b[160];
+                snprintf(b, sizeof(b), "data line %lld: no position field", (long long)l + 1);
+                errs[t] = b;
+                failed.store(1);
+                return;
+            }
+            // position: an optional sign and leading digits (the rest of the field is skipped); it must fit in int32
             bool neg = false;
-            if (p < e && (*p == '-' || *p == '+')) {
+            if (*p == '-' || *p == '+') {
                 neg = (*p == '-');
                 ++p;
             }
@@ -205,14 +216,22 @@ extern "C" int pg_geno_parse(const char* buf, size_t len, int32_t fmt, int32_t n
             }
             int64_t v = 0;
             while (p < e && *p >= '0' && *p <= '9') {
-                v = v * 10 + (*p - '0');
+                if (v <= ((int64_t)1 << 31)) v = v * 10 + (*p - '0');    // past the limit the value stays out of range
                 ++p;
             }
+            if (v > ((int64_t)1 << 31) - (neg ? 0 : 1)) {
+                char b[160];
+                snprintf(b, sizeof(b), "data line %lld: position outside the int32 range", (long long)l + 1);
+                errs[t] = b;
+                failed.store(1);
+                return;
+            }
+            while (p < e && !is_ws(*p)) ++p;
             pos[l] = (int32_t)(neg ? -v : v);
             int8_t* grow = geno + (size_t)l * H_out;
             int col = 0, found = 0;
-            // fast path: every token has the same width and single-character separators (the normal layout of
-            // .geno files) -> address the requested columns directly instead of tokenising the whole line
+            // fast path: every token has the same width and is followed by one blank (the normal layout of .geno files)
+            // -> address the requested columns directly instead of tokenising the whole line
             {
                 const char* q = p;
                 while (q < e && is_ws(*q)) ++q;
@@ -225,19 +244,15 @@ extern "C" int pg_geno_parse(const char* buf, size_t len, int32_t fmt, int32_t n
                 long ncols = fast ? (rem + 1) / (tokw + 1) : 0;
                 if (fast && max_col >= ncols) fast = false;
                 if (fast) {
-                    const char* sp = q + tokw;
-                    for (long c2 = 0; c2 + 1 < ncols; ++c2, sp += tokw + 1)
-                        if (!is_ws(*sp)) {
-                            fast = false;
-                            break;
-                        }
-                }
-                if (fast && fmt == 0) {
-                    // a 3-character token must not contain whitespace either ("A|T")
-                    for (int k = 0; k < n_out && fast; ++k) {
-                        const char* t0 = q + (long)col_take[k] * 4;
-                        if (is_ws(t0[0]) || is_ws(t0[1]) || is_ws(t0[2])) fast = false;
+                    // the grid is the whitespace split only when every separator is one blank and no token byte is blank
+                    // (branch-free over the line: one table load per byte)
+                    const unsigned char* u = (const unsigned char*)q;
+                    unsigned bad = 0;
+                    for (long c2 = 0; c2 < ncols; ++c2, u += tokw + 1) {
+                        for (int j = 0; j < tokw; ++j) bad |= LUT.ws[u[j]];
+                        if (c2 + 1 < ncols) bad |= LUT.ws[u[tokw]] ^ 1u;
                     }
+                    fast = bad == 0;
                 }
                 if (fast) {
                     for (int k = 0; k < n_out; ++k) {
@@ -269,26 +284,12 @@ extern "C" int pg_geno_parse(const char* buf, size_t len, int32_t fmt, int32_t n
                     const int k = col_to_out[col];
                     const int pl = ploidy[k];
                     int8_t* o = grow + hap_off[k];
-                    int nall;
-                    int8_t al[8];
-                    if (fmt == 0) {              // phased: characters 0,2,4,...
-                        nall = (tl + 1) / 2;
-                        if (nall > 8) nall = 8;
-                        for (int a = 0; a < nall; ++a) al[a] = LUT.base[(unsigned char)t0[2 * a]];
-                    } else if (fmt == 2) {       // pairs
-                        nall = tl > 8 ? 8 : tl;
-                        for (int a = 0; a < nall; ++a) al[a] = LUT.base[(unsigned char)t0[a]];
-                    } else if (fmt == 1) {       // diplo
-                        nall = 2;
-                        al[0] = LUT.dip0[(unsigned char)t0[0]];
-                        al[1] = LUT.dip1[(unsigned char)t0[0]];
-                    } else {                     // haplo
-                        nall = 1;
-                        al[0] = LUT.base[(unsigned char)t0[0]];
-                    }
+                    // alleles in the token: every other character (phased), every character (pairs), two (diplo), one (haplo)
+                    const int nall = fmt == 0 ? (tl + 1) / 2 : (fmt == 2 ? tl : (fmt == 1 ? 2 : 1));
                     if (pl == 1 && fmt == 1) {
                         // forceHomo (genomics.py:407): keep homozygous calls only
-                        o[0] = (al[0] == al[1]) ? al[0] : (int8_t)-1;
+                        const int8_t a0 = LUT.dip0[(unsigned char)t0[0]], a1 = LUT.dip1[(unsigned char)t0[0]];
+                        o[0] = (a0 == a1) ? a0 : (int8_t)-1;
                     } else if (nall != pl) {
                         char b[200];
                         snprintf(b, sizeof(b), "data line %lld, genotype column %d: token has %d alleles, sample ploidy is %d "
@@ -297,7 +298,10 @@ extern "C" int pg_geno_parse(const char* buf, size_t len, int32_t fmt, int32_t n
                         failed.store(1);
                         return;
                     } else {
-                        for (int a = 0; a < pl; ++a) o[a] = al[a];
+                        for (int a = 0; a < pl; ++a) {
+                            const unsigned char c = (unsigned char)t0[fmt == 0 ? 2 * a : (fmt == 2 ? a : 0)];
+                            o[a] = fmt == 1 ? (a == 0 ? LUT.dip0[c] : LUT.dip1[c]) : LUT.base[c];
+                        }
                     }
                     ++found;
                 }

@@ -116,7 +116,7 @@ struct ParseParams {
     int aux_stride;
 };
 
-enum { ERR_NONE = 0, ERR_POS = 1, ERR_PLOIDY = 2, ERR_MISSING_COLS = 3, ERR_NO_POS = 4, ERR_CHAR = 5 };
+enum { ERR_NONE = 0, ERR_POS = 1, ERR_PLOIDY = 2, ERR_MISSING_COLS = 3, ERR_NO_POS = 4, ERR_CHAR = 5, ERR_POS_RANGE = 6 };
 
 __device__ __forceinline__ bool acgtn(unsigned c) { return c == 'A' || c == 'C' || c == 'G' || c == 'T' || c == 'N'; }
 __device__ __forceinline__ bool diplotype(unsigned c) {
@@ -227,12 +227,14 @@ __global__ void __launch_bounds__(256) k_parse_lines(const __grid_constant__ Par
                         neg = (c == '-');
                         c = byte_at(pp, ++j);
                     }
-                    if (c < '0' || c > '9') report(pp, ERR_POS, line, 0);
+                    // position errors take column -1, so that they precede any genotype column's error of the line
+                    if (c < '0' || c > '9') report(pp, ERR_POS, line, -1);
                     long long v = 0;
                     while (c >= '0' && c <= '9') {
-                        v = v * 10 + (long long)(c - '0');
+                        if (v <= (1ll << 31)) v = v * 10 + (long long)(c - '0');    // past the limit it stays out of range
                         c = byte_at(pp, ++j);
                     }
+                    if (v > (1ll << 31) - (neg ? 0 : 1)) report(pp, ERR_POS_RANGE, line, -1);
                     pp.pos[line] = (int32_t)(neg ? -v : v);
                     have_pos = true;
                 } else {
@@ -309,7 +311,8 @@ __global__ void __launch_bounds__(256) k_parse_lines(const __grid_constant__ Par
         const bool any_pos = __any_sync(0xffffffffu, have_pos);
         if (lane == 0) {
             if (!any_pos) report(pp, ERR_NO_POS, line, 0);
-            else if ((int)found != pp.n_wanted) report(pp, ERR_MISSING_COLS, line, (int)fields_before - 3);
+            // one past the last genotype column: an error of any column of the line comes first
+            else if ((int)found != pp.n_wanted) report(pp, ERR_MISSING_COLS, line, (int)fields_before - 2);
         }
     }
 }
@@ -454,6 +457,10 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
             }
         }
         const int ti = pg_time_begin(ctx, "text_h2d");
+        ctx->ingest_geom[0] = (int64_t)((len + slab - 1) / slab);
+        ctx->ingest_geom[1] = (int64_t)slab;
+        ctx->ingest_geom[2] = CS_BLOCK_BYTES;
+        ctx->ingest_geom[3] = ctx->ingest_geom[4] = 0;
         int k = 0;
         for (size_t o = 0; o < len; o += slab, ++k) {
             const size_t n = std::min(slab, len - o);
@@ -549,7 +556,10 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
         k_parse_lines<<<grid, 256, 0, ctx->stream>>>(pp);
         pg_time_end(ctx, ti);
         PG_CUDA(cudaGetLastError());
-        k_scaffold_flags<<<(unsigned)std::min<int64_t>((S + 255) / 256, 4096), 256, 0, ctx->stream>>>(d_hash, S, d_flags);
+        const unsigned fgrid = (unsigned)std::min<int64_t>((S + 255) / 256, 4096);
+        k_scaffold_flags<<<fgrid, 256, 0, ctx->stream>>>(d_hash, S, d_flags);
+        ctx->ingest_geom[3] = (int64_t)grid * 8;
+        ctx->ingest_geom[4] = (int64_t)fgrid * 256;
         PG_CUDA(cudaGetLastError());
         ctx->launches += 1;
     }
@@ -563,8 +573,13 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
     switch ((int)h_err[0]) {
         case ERR_NONE: break;
         case ERR_POS:
-        case ERR_NO_POS:
             pg_set_error("pg_ingest_text: data line %llu: position is not an integer", h_err[1]);
+            return PG_ERR;
+        case ERR_NO_POS:
+            pg_set_error("pg_ingest_text: data line %llu: no position field", h_err[1]);
+            return PG_ERR;
+        case ERR_POS_RANGE:
+            pg_set_error("pg_ingest_text: data line %llu: position outside the int32 range", h_err[1]);
             return PG_ERR;
         case ERR_PLOIDY:
             pg_set_error("pg_ingest_text: data line %llu, genotype column %llu: the token's allele count does not match the "
@@ -576,7 +591,7 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
             return PG_ERR;
         default:
             pg_set_error("pg_ingest_text: data line %llu: %llu genotype columns, not every requested sample found", h_err[1],
-                         h_err[2]);
+                         h_err[2] - 1);
             return PG_ERR;
     }
     return PG_OK;
@@ -606,6 +621,12 @@ extern "C" int pg_ingest_set_strict(pg_ctx* ctx, int32_t on) {
     PG_CHECK(ctx != nullptr, "pg_ingest_set_strict: null ctx");
     PG_CHECK(on >= 0 && on <= 2, "pg_ingest_set_strict: level %d is not 0, 1 or 2", on);
     ctx->ingest_strict = on;
+    return PG_OK;
+}
+
+extern "C" int pg_debug_ingest(pg_ctx* ctx, int64_t* out) {
+    PG_CHECK(ctx && out, "pg_debug_ingest: null argument");
+    for (int k = 0; k < 5; ++k) out[k] = ctx->ingest_geom[k];
     return PG_OK;
 }
 

@@ -129,6 +129,7 @@ struct pg_ctx {
     int64_t ingest_sites = -1;
     int32_t ingest_fmt = 0;                   // format of the last text ingest
     int32_t ingest_strict = 0;                // pg_ingest_set_strict
+    int64_t ingest_geom[5] = {0, 0, 0, 0, 0}; // geometry of the last text ingest (pg_debug_ingest)
     // filterGenotypes (filter.cu): phase character per sample of the strict ingest, sample tables, per-site statistics,
     // kept rows, their byte offsets and the output slab
     PgBuf flt_aux, flt_tab, flt_stats, flt_rows, flt_off, flt_out, flt_cub;

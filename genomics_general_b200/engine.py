@@ -360,6 +360,13 @@ class Engine:
             check(self._lib.pg_ingest_release(self._ctx), "pg_ingest_release")
         return pos, newsc, off
 
+    def ingest_geometry(self):
+        """Geometry of the last ingest (pg_debug_ingest): slabs and slab bytes of the text copy, bytes per line-index block,
+        warps of the line parse grid and threads of the scaffold-flag grid."""
+        out = np.zeros(5, dtype=np.int64)
+        check(self._lib.pg_debug_ingest(self._ctx, _ptr(out)), "pg_debug_ingest")
+        return dict(zip(("slabs", "slab_bytes", "index_block_bytes", "parse_warps", "flag_threads"), (int(v) for v in out)))
+
     # ---- filterGenotypes.py ----
     FILTER_FORMATS = {"phased": 0, "diplo": 1, "bases": 2, "alleles": 3, "coded": 4, "count": 5}
 

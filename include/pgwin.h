@@ -301,6 +301,10 @@ int pg_ingest_release(pg_ctx* ctx);
  * error naming its data line.  The ingest also keeps each sample's phase character (genomics.py:335) for pg_filter_emit.
  * on = 2 keeps only the width test (distPaint.py's haploid tokens: one character; other characters read as usual). */
 int pg_ingest_set_strict(pg_ctx* ctx, int32_t on);
+/* Geometry of the last text ingest of this ctx: out[0] = slabs of the host-to-device copy of the text, out[1] = bytes per
+ * slab, out[2] = bytes per block of the line index, out[3] = warps of the line parse grid (one line per warp, grid-stride),
+ * out[4] = threads of the scaffold-flag grid (one line per thread, grid-stride).  All 0 before any ingest. */
+int pg_debug_ingest(pg_ctx* ctx, int64_t* out);
 
 /* ---- filterGenotypes.py ------------------------------------------------------------------------ */
 /* Filter settings (filterGenotypes.py:161-183 -> genomics.siteTest, genomics.py:742-799).  Samples are the selected
