@@ -9,6 +9,8 @@ import ctypes as C
 import os
 import subprocess
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpgwin.so")
 CSRC = os.path.join(_HERE, "csrc")
@@ -127,6 +129,12 @@ _SIGS = {
                                         C.c_void_p]),
     "pg_fourpop_allgather": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32,
                                        C.c_int64, C.c_void_p]),
+    "pg_vcf_set_spec": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "pg_vcf_load": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.c_char_p, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
+    "pg_vcf_lines": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    "pg_vcf_genotypes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]),
+    "pg_vcf_verdicts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pg_vcf_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_size_t)]),
     "pg_geno_count_lines": (C.c_int, [C.c_char_p, C.c_size_t, C.POINTER(C.c_int64)]),
     "pg_geno_parse": (C.c_int, [C.c_char_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                 C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),
@@ -144,6 +152,27 @@ class FilterSpec(C.Structure):
                 ("min_pop_alleles", C.c_void_p), ("max_pop_alleles", C.c_void_p), ("fixed_diffs", C.c_int32),
                 ("has_nearly_fixed", C.c_int32), ("nearly_fixed_diff", C.c_double), ("partial_to_missing", C.c_int32),
                 ("no_test", C.c_int32), ("thin_dist", C.c_int32), ("pod_size", C.c_int32)]
+
+
+class VcfSpec(C.Structure):
+    """pg_vcf_spec (include/pgwin.h)"""
+    _fields_ = [("n_cols", C.c_int32), ("col_slot", C.c_void_p), ("col_prev", C.c_void_p), ("n_keys", C.c_int32),
+                ("key_off", C.c_void_p), ("key_chars", C.c_void_p), ("n_samp", C.c_int32), ("samp_col", C.c_void_p),
+                ("samp_ploidy", C.c_void_p), ("field_key", C.c_int32), ("field_phase", C.c_int32), ("n_filt", C.c_int32),
+                ("filt_key", C.c_void_p), ("filt_min", C.c_void_p), ("filt_max", C.c_void_p), ("filt_site", C.c_void_p),
+                ("filt_gt", C.c_void_p), ("filt_samp", C.c_void_p), ("has_min_qual", C.c_int32), ("min_qual", C.c_double),
+                ("missing", C.c_void_p), ("missing_len", C.c_int32), ("sep", C.c_void_p), ("sep_len", C.c_int32),
+                ("skip_indels", C.c_int32), ("keep_partial", C.c_int32), ("ploidy_mismatch_to_missing", C.c_int32),
+                ("add_ref_track", C.c_int32)]
+
+
+# pg_vcf_line (include/pgwin.h) as a numpy record
+VCF_LINE = np.dtype([("start", np.int64), ("end", np.int64), ("pos", np.int64)] +
+                    [(n, np.uint32) for n in ("chrom_off", "chrom_len", "pos_off", "pos_len", "ref_off", "ref_len", "alt_off",
+                                              "alt_len", "qual_off", "qual_len", "fmt_off", "fmt_len")] +
+                    [("n_fields", np.int32), ("n_alt", np.int32), ("flags", np.uint32), ("reserved", np.uint32)])
+VCF_NONASCII, VCF_POS_UNRESOLVED, VCF_QUAL_DROP, VCF_QUAL_UNRESOLVED, VCF_SAME_LEN, VCF_DUPLICATE, VCF_FORMAT_WIDE = \
+    1, 2, 4, 8, 16, 32, 64
 
 
 def lib():

@@ -72,6 +72,7 @@ extern "C" int pg_ctx_destroy(pg_ctx* ctx) {
     cudaStreamSynchronize(ctx->stream);
     pg_k1_cache_free(ctx);
     pg_filter_free(ctx);
+    pg_vcf_free(ctx);
     pg_nccl_finalize(ctx);
     ctx->gather.release();
     ctx->gather_flag.release();

@@ -134,6 +134,7 @@ struct pg_ctx {
     // kept rows, their byte offsets and the output slab
     PgBuf flt_aux, flt_tab, flt_stats, flt_rows, flt_off, flt_out, flt_cub;
     void* flt_state = nullptr;                // host-side state of the last pg_filter (owned by filter.cu)
+    void* vcf_state = nullptr;                // parseVCF buffers and spec (owned by vcf.cu)
     void* h_text[2] = {nullptr, nullptr};     // pinned staging of the text
     cudaEvent_t h_text_free[2] = {nullptr, nullptr};
     // upload pipeline: copy stream + two staging buffers
@@ -239,6 +240,7 @@ int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, const in
                          int32_t min_sites, double min_data, void* d_rec, int RC);
 void pg_k1_cache_free(pg_ctx* ctx);
 void pg_filter_free(pg_ctx* ctx);        // filter.cu
+void pg_vcf_free(pg_ctx* ctx);           // vcf.cu
 int pg_nccl_allreduce_i64(pg_ctx* ctx, void* d_buf, size_t count);   // nccl_gather.cu
 int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t force_path, void* d_rec, int** h_count);
 int pg_popgen_resolve(pg_ctx* ctx, int32_t min_sites, double min_data, void* d_rec, int nk2);

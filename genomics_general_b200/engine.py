@@ -446,6 +446,103 @@ class Engine:
               "pg_filter_stats")
         return r
 
+    # ---- parseVCF.py ----
+    def vcf_set_spec(self, spec: dict):
+        """pg_vcf_set_spec: the header's column tables, the FORMAT keys looked up (GT first), the selected samples, the
+        --gtf filters and the output settings of one run (parseVCF.py:331-368)."""
+        from ._lib import VcfSpec
+        keep = []
+
+        def arr(v, dt):
+            a = np.ascontiguousarray(v if len(v) else np.zeros(1), dtype=dt)
+            keep.append(a)
+            return a.ctypes.data
+
+        def text(b):
+            keep.append(b)
+            return C.cast(C.c_char_p(b), C.c_void_p).value
+        keys = [k.encode() for k in spec["keys"]]
+        vs = VcfSpec()
+        vs.n_cols = len(spec["col_slot"])
+        vs.col_slot = arr(spec["col_slot"], np.int32)
+        vs.col_prev = arr(spec["col_prev"], np.int32)
+        vs.n_keys = len(keys)
+        vs.key_off = arr(np.concatenate([[0], np.cumsum([len(k) for k in keys])]), np.int32)
+        vs.key_chars = text(b"".join(keys) + b"\0")
+        vs.n_samp = len(spec["samp_col"])
+        vs.samp_col = arr(spec["samp_col"], np.int32)
+        vs.samp_ploidy = arr(spec["samp_ploidy"], np.int32)
+        vs.field_key = int(spec["field_key"])
+        vs.field_phase = 1 if spec.get("field_phase") else 0
+        filt = spec["filters"]
+        vs.n_filt = len(filt)
+        vs.filt_key = arr([f["key"] for f in filt], np.int32)
+        vs.filt_min = arr([f["min"] for f in filt], np.float64)
+        vs.filt_max = arr([f["max"] for f in filt], np.float64)
+        vs.filt_site = arr([f["site"] for f in filt], np.uint8)
+        vs.filt_gt = arr([f["gt"] for f in filt], np.uint8)
+        vs.filt_samp = arr(np.array([f["samples"] for f in filt], dtype=np.uint8).reshape(-1), np.uint8)
+        vs.has_min_qual = 1 if spec.get("min_qual") is not None else 0
+        vs.min_qual = float(spec.get("min_qual") or 0.0)
+        vs.missing = text(spec["missing"] + b"\0")
+        vs.missing_len = len(spec["missing"])
+        vs.sep = text(spec["sep"] + b"\0")
+        vs.sep_len = len(spec["sep"])
+        vs.skip_indels = 1 if spec.get("skip_indels") else 0
+        vs.keep_partial = 1 if spec.get("keep_partial") else 0
+        vs.ploidy_mismatch_to_missing = 1 if spec.get("p2m") else 0
+        vs.add_ref_track = 1 if spec.get("add_ref") else 0
+        check(self._lib.pg_vcf_set_spec(self._ctx, C.byref(vs)), "pg_vcf_set_spec")
+
+    def vcf_load(self, text: bytes, prev=None) -> int:
+        """pg_vcf_load: complete lines of VCF body text; prev = (CHROM, POS) bytes of the data line before it, or None.
+        Returns the number of data lines."""
+        n = C.c_int64(0)
+        pc, pp = (prev[0], prev[1]) if prev is not None else (b"", b"")
+        check(self._lib.pg_vcf_load(self._ctx, text, len(text), (pc + pp) if prev is not None else None, len(pc), len(pp),
+                                    C.byref(n)), "pg_vcf_load")
+        self._vcf_lines = int(n.value)
+        return self._vcf_lines
+
+    def vcf_lines(self, line0: int = 0, n: int | None = None):
+        """The pg_vcf_line records of the last load as a numpy record array (_lib.VCF_LINE)."""
+        from ._lib import VCF_LINE
+        if n is None:
+            n = self._vcf_lines - line0
+        out = np.zeros(n, dtype=VCF_LINE)
+        check(self._lib.pg_vcf_lines(self._ctx, int(line0), int(n), _ptr(out)), "pg_vcf_lines")
+        return out
+
+    def vcf_genotypes(self, rows, pos):
+        """pg_vcf_genotypes over the kept lines `rows` (with their POS): (genotypes left unresolved, error word)."""
+        rows = np.ascontiguousarray(rows, dtype=np.int64)
+        pos = np.ascontiguousarray(pos, dtype=np.int64)
+        nu = C.c_int64(0)
+        err = C.c_uint64(0)
+        check(self._lib.pg_vcf_genotypes(self._ctx, len(rows), _ptr(rows), _ptr(pos), C.byref(nu), C.byref(err)),
+              "pg_vcf_genotypes")
+        return int(nu.value), int(err.value)
+
+    def vcf_verdicts(self, n_rows: int, n_samp: int, put=None):
+        """The verdict bytes [n_rows, n_samp] of the last vcf_genotypes; with put, replaces them first."""
+        if put is not None:
+            put = np.ascontiguousarray(put, dtype=np.uint8)
+            check(self._lib.pg_vcf_verdicts(self._ctx, None, _ptr(put)), "pg_vcf_verdicts")
+            return put
+        out = np.zeros((n_rows, n_samp), dtype=np.uint8)
+        check(self._lib.pg_vcf_verdicts(self._ctx, _ptr(out), None), "pg_vcf_verdicts")
+        return out
+
+    def vcf_emit(self, row0: int, buf, cap: int):
+        """Rows row0.. of the last vcf_genotypes as .geno text into buf (at least cap bytes, pinned for speed):
+        (rows, bytes) written."""
+        rows = C.c_int64(0)
+        nb = C.c_size_t(0)
+        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
+        check(self._lib.pg_vcf_emit(self._ctx, int(row0), C.c_void_p(addr), int(cap), C.byref(rows), C.byref(nb)),
+              "pg_vcf_emit")
+        return int(rows.value), int(nb.value)
+
     def site_counts(self, site0: int = 0, n: int = None, out=None):
         """uint16 [n, P, 4] A,C,G,T counts per population (`out`: a caller-owned array to fill, e.g. one whose pages are
         already resident — a fresh 100 MB array costs more in page faults than the kernel and the copy together)."""

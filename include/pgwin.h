@@ -358,6 +358,77 @@ int pg_filter_emit(pg_ctx* ctx, int32_t fmt, int32_t freq_order, int64_t row0, c
 int pg_filter_stats(pg_ctx* ctx, int64_t site0, int64_t n, int32_t* called, int32_t* het, int32_t* counts,
                     int32_t* pop_called, uint8_t* pop_mask, uint8_t* flags, uint8_t* keep, uint8_t* final_);
 
+/* ---- parseVCF.py (csrc/vcf.cu) ------------------------------------------------------------------------------------- */
+/* One data line of the last pg_vcf_load (offsets of the fields are from the line's first byte). */
+typedef struct {
+    int64_t start;              /* first byte of the line in the text */
+    int64_t end;                /* its terminator ('\n' or '\r') */
+    int64_t pos;                /* POS, unless flags & PG_VCF_POS_UNRESOLVED */
+    uint32_t chrom_off, chrom_len, pos_off, pos_len, ref_off, ref_len, alt_off, alt_len, qual_off, qual_len, fmt_off, fmt_len;
+    int32_t n_fields;           /* str.split() fields of the line */
+    int32_t n_alt;              /* ALT alleles (0 for ".") */
+    uint32_t flags;             /* PG_VCF_* */
+    uint32_t reserved;
+} pg_vcf_line;
+#define PG_VCF_NONASCII 1u          /* a byte >= 0x80: the host checks str.split() against the ASCII split */
+#define PG_VCF_POS_UNRESOLVED 2u    /* POS is not sign + ASCII digits ('_' between them) of at most 18 significant digits */
+#define PG_VCF_QUAL_DROP 4u         /* float(QUAL) < min_qual */
+#define PG_VCF_QUAL_UNRESOLVED 8u   /* QUAL off the fast number path: the host decides */
+#define PG_VCF_SAME_LEN 16u         /* every ALT as long as REF (an ALT-less line has it too) */
+#define PG_VCF_DUPLICATE 32u        /* CHROM and POS text equal to the data line before */
+#define PG_VCF_FORMAT_WIDE 64u      /* a looked-up FORMAT key past the 64th */
+
+/* What a run of parseVCF.py reads and writes (parseVCF.py:257-289, 350-391). */
+typedef struct {
+    int32_t n_cols;             /* #CHROM line tokens (the nine fixed columns, then the samples) */
+    const int32_t* col_slot;    /* [n_cols] slot of a column a selected sample may read (0, 1, .. in column order), or -1 */
+    const int32_t* col_prev;    /* [n_cols] the previous column of the same sample name, or -1 (also for columns < 9) */
+    int32_t n_keys;             /* FORMAT keys looked up: key 0 is GT */
+    const int32_t* key_off;     /* [n_keys + 1] into key_chars */
+    const char* key_chars;
+    int32_t n_samp;             /* selected samples, in -s order */
+    const int32_t* samp_col;    /* [n_samp] last column of the sample's name */
+    const int32_t* samp_ploidy; /* [n_samp] expected ploidy */
+    int32_t field_key;          /* --field: its key; -1: genotypes */
+    int32_t field_phase;        /* --field phase: the GT's phase character when the sample has a GT */
+    int32_t n_filt;             /* --gtf filters, in command-line order */
+    const int32_t* filt_key;    /* [n_filt] key of the flag; -1: the filter always fails */
+    const double* filt_min;
+    const double* filt_max;
+    const uint8_t* filt_site;   /* [n_filt] site types it applies to: bit 0 MONO, 1 SNP, 2 INDEL */
+    const uint8_t* filt_gt;     /* [n_filt] genotype types: bit 0 Het, 1 HomRef, 2 Missing, 3 HomAlt */
+    const uint8_t* filt_samp;   /* [n_filt x n_samp] 1: it applies to the sample */
+    int32_t has_min_qual;
+    double min_qual;            /* drop a line whose float(QUAL) < min_qual */
+    const char* missing;        /* the missing allele / field text */
+    int32_t missing_len;
+    const char* sep;            /* --outSep */
+    int32_t sep_len;
+    int32_t skip_indels, keep_partial, ploidy_mismatch_to_missing, add_ref_track;
+} pg_vcf_spec;
+
+/* Sets the run's spec (copied; the pointers need not outlive the call). */
+int pg_vcf_set_spec(pg_ctx* ctx, const pg_vcf_spec* spec);
+/* Complete lines of VCF body text (cut at line ends) -> device: data-line index and one pg_vcf_line per data line.  prev
+ * (may be NULL) = the CHROM then POS text of the data line before this text (prev_chrom + prev_pos bytes, at most 4000), for
+ * --excludeDuplicates.  *n_lines = data lines. */
+int pg_vcf_load(pg_ctx* ctx, const char* text, size_t len, const char* prev, int32_t prev_chrom, int32_t prev_pos,
+                int64_t* n_lines);
+/* Lines [line0, line0 + n) of the last pg_vcf_load. */
+int pg_vcf_lines(pg_ctx* ctx, int64_t line0, int64_t n, pg_vcf_line* out);
+/* Replaces VcfSite.getGenotypes / getGenoField (parseVCF.py:107-190) for the kept lines rows[0..n_rows) (their POS in pos):
+ * one verdict per (row, selected sample).  Every line must hold all of the header's sample names.  *n_unresolved = genotypes
+ * whose filter values left the fast number path (verdict bit 2; settle them with pg_vcf_verdicts before pg_vcf_emit);
+ * *error = 0, or the first offending genotype: ((line + 1) << 24) | (sample << 3) | code, code 1 = no GT, 2 = ploidy. */
+int pg_vcf_genotypes(pg_ctx* ctx, int64_t n_rows, const int64_t* rows, const int64_t* pos, int64_t* n_unresolved,
+                     uint64_t* error);
+/* The verdict bytes [n_rows x n_samp] of the last pg_vcf_genotypes: copied out to get and/or replaced by put (either may be
+ * NULL).  Bits: 1 a filter failed, 2 unresolved, 4 ploidy mismatch (to missing), 8 phased GT, 16 field absent. */
+int pg_vcf_verdicts(pg_ctx* ctx, uint8_t* get, const uint8_t* put);
+/* The .geno rows of the last pg_vcf_genotypes from row0 on, as many as fit in cap bytes of out (host memory): *rows, *bytes
+ * written; a single row larger than cap is an error. */
+int pg_vcf_emit(pg_ctx* ctx, int64_t row0, char* out, size_t cap, int64_t* rows, size_t* bytes);
+
 /* ---- introspection ---------------------------------------------------------------------------- */
 /* Device time (ms, CUDA events on the ctx stream) of the kernels launched by the last statistics call:
  * names[i] -> ms[i]; returns the number of entries through *count (at most cap). */
