@@ -135,6 +135,13 @@ _SIGS = {
     "pg_vcf_genotypes": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]),
     "pg_vcf_verdicts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_vcf_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_size_t)]),
+    "pg_seq_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.c_char_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32,
+                               C.c_void_p, C.c_int32, C.POINTER(C.c_int64), C.c_void_p]),
+    "pg_seq_meta": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pg_seq_plan": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                              C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "pg_seq_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64),
+                              C.POINTER(C.c_int64), C.POINTER(C.c_size_t)]),
     "pg_geno_count_lines": (C.c_int, [C.c_char_p, C.c_size_t, C.POINTER(C.c_int64)]),
     "pg_geno_parse": (C.c_int, [C.c_char_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                 C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),

@@ -413,30 +413,12 @@ extern "C" int pg_ingest_file_range(pg_ctx* ctx, const char* path, int64_t byte_
     return rc;
 }
 
-namespace {
-int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t len, int32_t fmt, int32_t n_cols,
-                const int32_t* col_hap, const int8_t* col_ploidy, int32_t H_out, int64_t* n_sites) {
-    PG_CHECK(fmt >= 0 && fmt <= 3, "pg_ingest: unknown format %d", fmt);
-    PG_CHECK(n_cols >= 1 && H_out >= 1, "pg_ingest: no genotype columns requested");
-    int n_wanted = 0;
-    {
-        std::vector<char> used((size_t)H_out, 0);
-        for (int c = 0; c < n_cols; ++c) {
-            if (col_hap[c] < 0) continue;
-            PG_CHECK(col_ploidy[c] >= 1 && col_ploidy[c] <= 8, "pg_ingest: ploidy %d of column %d unsupported",
-                     (int)col_ploidy[c], c);
-            PG_CHECK(col_hap[c] + col_ploidy[c] <= H_out, "pg_ingest: column %d maps outside the %d output haplotypes", c, H_out);
-            for (int a = 0; a < col_ploidy[c]; ++a) {
-                PG_CHECK(!used[col_hap[c] + a], "pg_ingest: output haplotype %d is written by two columns", col_hap[c] + a);
-                used[col_hap[c] + a] = 1;
-            }
-            ++n_wanted;
-        }
-        for (int h = 0; h < H_out; ++h) PG_CHECK(used[h], "pg_ingest: output haplotype %d has no source column", h);
-    }
-    PG_CUDA(cudaSetDevice(ctx->device));
-    pg_timings_reset(ctx);
-    *n_sites = 0;
+// The text -> ctx->text (then 256 bytes of '\n'), the start of every data line -> ctx->starts, *n_lines = data lines.  The
+// source is memory (mem) or bytes [file_off, file_off + len) of the open file fd.  Shared by the .geno ingest and genoToSeq
+// (seq.cu); bumps ctx->text_gen.
+int pg_text_load(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t len, int64_t* n_lines) {
+    *n_lines = 0;
+    ctx->text_gen += 1;
     size_t free_b = 0, total_b = 0;
     PG_CUDA(cudaMemGetInfo(&free_b, &total_b));
     PG_CHECK(len + ((size_t)1 << 30) < free_b + ctx->text.cap, "pg_ingest_text: %zu bytes of text do not fit in device memory "
@@ -476,7 +458,6 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
     }
     const size_t nblk = (len + CS_BLOCK_BYTES - 1) / CS_BLOCK_BYTES;
     int64_t S = 0;
-    long long* d_starts = nullptr;
     if (nblk > 0) {
         PG_CHECK(nblk < ((size_t)1 << 31), "pg_ingest_text: text too large for one call");
         // block counts -> exclusive scan (64-bit) -> starts
@@ -502,7 +483,7 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
         PG_CUDA(cudaStreamSynchronize(ctx->stream));
         S = (int64_t)total;
         PG_TRY(ctx->starts.ensure((size_t)std::max<int64_t>(S, 1) * 8 + 64));
-        d_starts = (long long*)ctx->starts.p;
+        long long* d_starts = (long long*)ctx->starts.p;
         if (S > 0) {
             const int ti = pg_time_begin(ctx, "ingest_index");
             k_write_starts<<<(unsigned)nblk, CS_THREADS, 0, ctx->stream>>>(d_text, len, d_base, d_starts);
@@ -510,6 +491,47 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
             PG_CUDA(cudaGetLastError());
         }
     }
+    PG_TRY(ctx->starts.ensure((size_t)std::max<int64_t>(S, 1) * 8 + 64));
+    *n_lines = S;
+    return PG_OK;
+}
+
+// new_scaffold[i] = hash[i] != hash[i - 1] for S lines (ctx stream)
+int pg_scaffold_flags(pg_ctx* ctx, const unsigned long long* d_hash, int64_t S, int8_t* d_flags) {
+    const unsigned fgrid = (unsigned)std::min<int64_t>((S + 255) / 256, 4096);
+    k_scaffold_flags<<<fgrid, 256, 0, ctx->stream>>>(d_hash, S, d_flags);
+    PG_CUDA(cudaGetLastError());
+    return PG_OK;
+}
+
+namespace {
+int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t len, int32_t fmt, int32_t n_cols,
+                const int32_t* col_hap, const int8_t* col_ploidy, int32_t H_out, int64_t* n_sites) {
+    PG_CHECK(fmt >= 0 && fmt <= 3, "pg_ingest: unknown format %d", fmt);
+    PG_CHECK(n_cols >= 1 && H_out >= 1, "pg_ingest: no genotype columns requested");
+    int n_wanted = 0;
+    {
+        std::vector<char> used((size_t)H_out, 0);
+        for (int c = 0; c < n_cols; ++c) {
+            if (col_hap[c] < 0) continue;
+            PG_CHECK(col_ploidy[c] >= 1 && col_ploidy[c] <= 8, "pg_ingest: ploidy %d of column %d unsupported",
+                     (int)col_ploidy[c], c);
+            PG_CHECK(col_hap[c] + col_ploidy[c] <= H_out, "pg_ingest: column %d maps outside the %d output haplotypes", c, H_out);
+            for (int a = 0; a < col_ploidy[c]; ++a) {
+                PG_CHECK(!used[col_hap[c] + a], "pg_ingest: output haplotype %d is written by two columns", col_hap[c] + a);
+                used[col_hap[c] + a] = 1;
+            }
+            ++n_wanted;
+        }
+        for (int h = 0; h < H_out; ++h) PG_CHECK(used[h], "pg_ingest: output haplotype %d has no source column", h);
+    }
+    PG_CUDA(cudaSetDevice(ctx->device));
+    pg_timings_reset(ctx);
+    *n_sites = 0;
+    int64_t S = 0;
+    PG_TRY(pg_text_load(ctx, mem, fd, file_off, len, &S));
+    const uint8_t* d_text = (const uint8_t*)ctx->text.p;
+    const long long* d_starts = (const long long*)ctx->starts.p;
     PG_TRY(pg_alloc_sites(ctx, S, H_out));
     ctx->epoch += 1;
     *n_sites = S;
@@ -557,10 +579,9 @@ int ingest_core(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t le
         pg_time_end(ctx, ti);
         PG_CUDA(cudaGetLastError());
         const unsigned fgrid = (unsigned)std::min<int64_t>((S + 255) / 256, 4096);
-        k_scaffold_flags<<<fgrid, 256, 0, ctx->stream>>>(d_hash, S, d_flags);
+        PG_TRY(pg_scaffold_flags(ctx, d_hash, S, d_flags));
         ctx->ingest_geom[3] = (int64_t)grid * 8;
         ctx->ingest_geom[4] = (int64_t)fgrid * 256;
-        PG_CUDA(cudaGetLastError());
         ctx->launches += 1;
     }
     PG_TRY(pg_pack_rows(ctx, 0, S));
@@ -639,5 +660,6 @@ extern "C" int pg_ingest_release(pg_ctx* ctx) {
     ctx->starts.release();
     ctx->meta.release();
     ctx->ingest_sites = -1;
+    ctx->text_gen += 1;
     return PG_OK;
 }

@@ -130,11 +130,13 @@ struct pg_ctx {
     int32_t ingest_fmt = 0;                   // format of the last text ingest
     int32_t ingest_strict = 0;                // pg_ingest_set_strict
     int64_t ingest_geom[5] = {0, 0, 0, 0, 0}; // geometry of the last text ingest (pg_debug_ingest)
+    uint64_t text_gen = 0;                    // bumped by every load or release of ctx->text (pg_text_load)
     // filterGenotypes (filter.cu): phase character per sample of the strict ingest, sample tables, per-site statistics,
     // kept rows, their byte offsets and the output slab
     PgBuf flt_aux, flt_tab, flt_stats, flt_rows, flt_off, flt_out, flt_cub;
     void* flt_state = nullptr;                // host-side state of the last pg_filter (owned by filter.cu)
     void* vcf_state = nullptr;                // parseVCF buffers and spec (owned by vcf.cu)
+    void* seq_state = nullptr;                // genoToSeq token index and row plan (owned by seq.cu)
     void* h_text[2] = {nullptr, nullptr};     // pinned staging of the text
     cudaEvent_t h_text_free[2] = {nullptr, nullptr};
     // upload pipeline: copy stream + two staging buffers
@@ -241,6 +243,11 @@ int pg_k2_popgen_windows(pg_ctx* ctx, const std::vector<int64_t>& wins, const in
 void pg_k1_cache_free(pg_ctx* ctx);
 void pg_filter_free(pg_ctx* ctx);        // filter.cu
 void pg_vcf_free(pg_ctx* ctx);           // vcf.cu
+void pg_seq_free(pg_ctx* ctx);           // seq.cu
+// ingest.cu: the text (memory, or bytes [file_off, file_off + len) of the open file fd) -> ctx->text, the start of every data
+// line -> ctx->starts, *n_lines = data lines; and the new-scaffold flags of S per-line scaffold hashes (both on ctx->stream)
+int pg_text_load(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t len, int64_t* n_lines);
+int pg_scaffold_flags(pg_ctx* ctx, const unsigned long long* d_hash, int64_t S, int8_t* d_flags);
 int pg_nccl_allreduce_i64(pg_ctx* ctx, void* d_buf, size_t count);   // nccl_gather.cu
 int pg_popgen_enqueue(pg_ctx* ctx, int32_t min_sites, double min_data, int32_t force_path, void* d_rec, int** h_count);
 int pg_popgen_resolve(pg_ctx* ctx, int32_t min_sites, double min_data, void* d_rec, int nk2);

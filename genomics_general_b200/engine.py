@@ -543,6 +543,54 @@ class Engine:
               "pg_vcf_emit")
         return int(rows.value), int(nb.value)
 
+    def seq_index(self, col_slot, slot_width, exact: bool, data: bytes | None = None, path: str | None = None,
+                  body_offset: int = 0):
+        """pg_seq_index: the body (data, or bytes body_offset.. of the file path) to the device and the token start of every
+        slotted column per data line.  Returns (data lines, (code, data line, genotype column)); code 0 = no error."""
+        col_slot = np.ascontiguousarray(col_slot, dtype=np.int32)
+        slot_width = np.ascontiguousarray(slot_width, dtype=np.int32)
+        n = C.c_int64(0)
+        err = np.zeros(3, dtype=np.int64)
+        check(self._lib.pg_seq_index(self._ctx, data if path is None else None, 0 if data is None else len(data),
+                                     None if path is None else path.encode(), int(body_offset), len(col_slot), _ptr(col_slot),
+                                     len(slot_width), _ptr(slot_width), 1 if exact else 0, C.byref(n), _ptr(err)),
+              "pg_seq_index")
+        return int(n.value), tuple(int(v) for v in err)
+
+    def seq_meta(self, S: int):
+        """positions int32 [S], new-scaffold flags int8 [S] and line offsets int64 [S] of the last seq_index"""
+        pos = np.zeros(S, np.int32)
+        newsc = np.zeros(S, np.int8)
+        off = np.zeros(S, np.int64)
+        check(self._lib.pg_seq_meta(self._ctx, _ptr(pos), _ptr(newsc), _ptr(off)), "pg_seq_meta")
+        return pos, newsc, off
+
+    def seq_plan(self, fmt: str, nto_gap: bool, names, seq_slot, seq_byte, seq_width, lo, hi):
+        """pg_seq_plan: alignments over the windows [lo, hi) of the last seq_index.  Returns (rows, bytes of every window)."""
+        enc = [n.encode() for n in names]
+        name_off = np.concatenate([[0], np.cumsum([len(b) for b in enc])]).astype(np.int64)
+        seq_slot = np.ascontiguousarray(seq_slot, dtype=np.int32)
+        seq_byte = np.ascontiguousarray(seq_byte, dtype=np.int32)
+        seq_width = np.ascontiguousarray(seq_width, dtype=np.int32)
+        lo = np.ascontiguousarray(lo, dtype=np.int64)
+        hi = np.ascontiguousarray(hi, dtype=np.int64)
+        wb = np.zeros(len(lo), np.int64)
+        R = C.c_int64(0)
+        check(self._lib.pg_seq_plan(self._ctx, {"fasta": 0, "phylip": 1}[fmt], 1 if nto_gap else 0, len(enc), b"".join(enc),
+                                    _ptr(name_off), _ptr(seq_slot), _ptr(seq_byte), _ptr(seq_width), len(lo), _ptr(lo),
+                                    _ptr(hi), C.byref(R), _ptr(wb)), "pg_seq_plan")
+        return int(R.value), wb
+
+    def seq_emit(self, row0: int, part0: int, buf, cap: int):
+        """Alignment text of the last seq_plan from cell (row0, part0) into buf (cap bytes, pinned for speed):
+        (row, part) to resume at, bytes written."""
+        r1, p1 = C.c_int64(0), C.c_int64(0)
+        nb = C.c_size_t(0)
+        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
+        check(self._lib.pg_seq_emit(self._ctx, int(row0), int(part0), C.c_void_p(addr), int(cap), C.byref(r1), C.byref(p1),
+                                    C.byref(nb)), "pg_seq_emit")
+        return int(r1.value), int(p1.value), int(nb.value)
+
     def site_counts(self, site0: int = 0, n: int = None, out=None):
         """uint16 [n, P, 4] A,C,G,T counts per population (`out`: a caller-owned array to fill, e.g. one whose pages are
         already resident — a fresh 100 MB array costs more in page faults than the kernel and the copy together)."""

@@ -473,6 +473,36 @@ int pg_debug_uniform_tiles(pg_ctx* ctx, int64_t cap, int64_t* site_lo, int64_t* 
  * *words = 32-bit words of all its rows (both 0 when the last call did not read the stream). */
 int pg_debug_uniform_rows(pg_ctx* ctx, int64_t* one_plane_rows, int64_t* words);
 
+/* ---- genoToSeq.py (seq.cu) ---------------------------------------------------------------------------------------------
+ * Replaces parseGenoFile / the window generators' line reading (genomics.py:1949-1967, 1971-2108), GenoWindow.seqDict
+ * (1790-1793) and makeAlnString (2232-2251): the genotype tokens of a .geno body, transposed into alignment text. */
+
+/* The body (text[0..len), or bytes [body_offset, EOF) of the file path when path is not NULL) -> device, its data lines
+ * indexed as pg_ingest_text does, and the start of the token of every column with col_slot[c] >= 0 (n_cols genotype columns,
+ * slots 0..n_slots-1, each of one column) recorded per line.  Every slot's token must be slot_width[slot] bytes wide (the
+ * width on the first data line); with exact_cols a line holds exactly n_cols genotype columns, else at least every slot's.
+ * *n_sites = data lines.  error[3] = {0, 0, 0}, or the first offending line: {code, data line, genotype column (0: none)},
+ * both 1-based; codes 1 position not an integer, 2 no position, 3 position outside int32, 4 token width, 5 a slot's column
+ * missing, 6 column count, 7 a byte >= 0x80, 8 a '\r' that ends a line by itself.  The text replaces the one of the last
+ * pg_ingest_text on this ctx. */
+int pg_seq_index(pg_ctx* ctx, const char* text, size_t len, const char* path, int64_t body_offset, int32_t n_cols,
+                 const int32_t* col_slot, int32_t n_slots, const int32_t* slot_width, int32_t exact_cols, int64_t* n_sites,
+                 int64_t* error);
+/* pos int32 [S], new_scaffold int8 [S], line_off int64 [S] of the last pg_seq_index (any may be NULL). */
+int pg_seq_meta(pg_ctx* ctx, int32_t* pos, int8_t* new_scaffold, int64_t* line_off);
+/* The output rows of n_win alignments over data lines [lo[w], hi[w]): fmt 0 FASTA (">name\nseq\n" per sequence), 1 PHYLIP
+ * (" n L\n", then "name   seq\n" per sequence, L the longest sequence).  Sequence k is named names[name_off[k] ..
+ * name_off[k + 1]) and takes seq_width[k] bytes from byte seq_byte[k] of slot seq_slot[k]'s token at every site (the whole
+ * token, or with --splitPhased one allele: seq_byte 2a, width 1); nto_gap maps N and n to '-' in the sequences.  A length
+ * pass and a scan give every row's byte offset.  *n_rows = rows; win_bytes[w] = bytes of alignment w. */
+int pg_seq_plan(pg_ctx* ctx, int32_t fmt, int32_t nto_gap, int32_t n_seq, const char* names, const int64_t* name_off,
+                const int32_t* seq_slot, const int32_t* seq_byte, const int32_t* seq_width, int64_t n_win, const int64_t* lo,
+                const int64_t* hi, int64_t* n_rows, int64_t* win_bytes);
+/* The text of the last pg_seq_plan from cell (row0, part0) on into out (host memory, cap bytes): whole rows while they fit,
+ * else row0 alone, cut after as many sites as fit.  part0 = -1 starts a row; k >= 0 resumes after its name and k sites.
+ * (*row1, *part1) = where the next call resumes (*row1 = n_rows: done); *bytes = bytes written. */
+int pg_seq_emit(pg_ctx* ctx, int64_t row0, int64_t part0, char* out, size_t cap, int64_t* row1, int64_t* part1, size_t* bytes);
+
 #ifdef __cplusplus
 }
 #endif
