@@ -142,6 +142,14 @@ _SIGS = {
                               C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "pg_seq_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64),
                               C.POINTER(C.c_int64), C.POINTER(C.c_size_t)]),
+    "pg_g2v_ref_load": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64)]),
+    "pg_g2v_ref_starts": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "pg_g2v_ref_index": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pg_g2v_spec": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32]),
+    "pg_g2v_chunk": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "pg_g2v_runs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pg_g2v_sites": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p]),
+    "pg_g2v_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "pg_geno_count_lines": (C.c_int, [C.c_char_p, C.c_size_t, C.POINTER(C.c_int64)]),
     "pg_geno_parse": (C.c_int, [C.c_char_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                 C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),

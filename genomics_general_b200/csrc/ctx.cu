@@ -74,6 +74,7 @@ extern "C" int pg_ctx_destroy(pg_ctx* ctx) {
     pg_filter_free(ctx);
     pg_vcf_free(ctx);
     pg_seq_free(ctx);
+    pg_g2v_free(ctx);
     pg_nccl_finalize(ctx);
     ctx->gather.release();
     ctx->gather_flag.release();

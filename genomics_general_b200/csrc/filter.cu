@@ -420,16 +420,7 @@ __global__ void __launch_bounds__(256) k_filter_emit(const __grid_constant__ Emi
         {
             int c[4];
             for (int a = 0; a < 4; ++a) c[a] = ep.cnt[site * 4 + a];
-            int nr = 0;
-            for (int a = 0; a < 4; ++a) {
-                rank[a] = 4;
-                if (c[a] <= 0) continue;
-                int before = 0;
-                for (int b = 0; b < 4; ++b)
-                    if (c[b] > 0 && (c[b] > c[a] || (c[b] == c[a] && b > a))) ++before;
-                rank[a] = before;
-                ++nr;
-            }
+            const int nr = pg_freq_order(c, rank);
             for (int a = 0; a < 4; ++a)
                 if (rank[a] == nr - 1) count_allele = a;
         }

@@ -137,6 +137,7 @@ struct pg_ctx {
     void* flt_state = nullptr;                // host-side state of the last pg_filter (owned by filter.cu)
     void* vcf_state = nullptr;                // parseVCF buffers and spec (owned by vcf.cu)
     void* seq_state = nullptr;                // genoToSeq token index and row plan (owned by seq.cu)
+    void* g2v_state = nullptr;                // genoToVCF reference sequences, spec and chunk state (owned by geno2vcf.cu)
     void* h_text[2] = {nullptr, nullptr};     // pinned staging of the text
     cudaEvent_t h_text_free[2] = {nullptr, nullptr};
     // upload pipeline: copy stream + two staging buffers
@@ -235,6 +236,24 @@ int pg_k2t_seq_nonnan(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, con
 int pg_k2t_het(pg_ctx* ctx, const K2TPlanes& ps, const int64_t* d_lo, const int64_t* d_hi, int nb, const int32_t* d_ind_start,
                int n_ind, int min_sites, double* d_out);
 
+// Frequency order of a site's alleles A, C, G, T from their counts c: np.argsort(counts)[::-1] over the counted alleles
+// (genomics.py:556) as a stable sort gives it — descending count, ties to the later allele.  rank[a] = place of allele a in
+// the order (4 when its count is 0); returns the number of counted alleles.  Shared by filterGenotypes' row emission
+// (filter.cu) and genoToVCF's allele lists (geno2vcf.cu).
+__device__ __forceinline__ int pg_freq_order(const int c[4], int rank[4]) {
+    int nr = 0;
+    for (int a = 0; a < 4; ++a) {
+        rank[a] = 4;
+        if (c[a] <= 0) continue;
+        int before = 0;
+        for (int b = 0; b < 4; ++b)
+            if (c[b] > 0 && (c[b] > c[a] || (c[b] == c[a] && b > a))) ++before;
+        rank[a] = before;
+        ++nr;
+    }
+    return nr;
+}
+
 // implemented in k1.cu / k2.cu
 // pairwise statistics for the listed windows, written into the DEVICE record table (stride RC words); window w spans sites
 // [win_lo[w], win_hi[w]) of the resident matrix
@@ -244,6 +263,7 @@ void pg_k1_cache_free(pg_ctx* ctx);
 void pg_filter_free(pg_ctx* ctx);        // filter.cu
 void pg_vcf_free(pg_ctx* ctx);           // vcf.cu
 void pg_seq_free(pg_ctx* ctx);           // seq.cu
+void pg_g2v_free(pg_ctx* ctx);           // geno2vcf.cu
 // ingest.cu: the text (memory, or bytes [file_off, file_off + len) of the open file fd) -> ctx->text, the start of every data
 // line -> ctx->starts, *n_lines = data lines; and the new-scaffold flags of S per-line scaffold hashes (both on ctx->stream)
 int pg_text_load(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t len, int64_t* n_lines);

@@ -591,6 +591,58 @@ class Engine:
                                     C.byref(nb)), "pg_seq_emit")
         return int(r1.value), int(p1.value), int(nb.value)
 
+    def g2v_ref_load(self, text: bytes):
+        """pg_g2v_ref_load + pg_g2v_ref_starts: the reference FASTA to the device; returns the byte offsets of its '>' bytes"""
+        n = C.c_int64(0)
+        check(self._lib.pg_g2v_ref_load(self._ctx, text, len(text), C.byref(n)), "pg_g2v_ref_load")
+        starts = np.zeros(int(n.value), np.int64)
+        check(self._lib.pg_g2v_ref_starts(self._ctx, _ptr(starts)), "pg_g2v_ref_starts")
+        return starts
+
+    def g2v_ref_index(self, lo, hi):
+        """pg_g2v_ref_index: record k's sequence is FASTA bytes [lo[k], hi[k]) without newlines and spaces; returns the
+        sequence lengths"""
+        lo = np.ascontiguousarray(lo, dtype=np.int64)
+        hi = np.ascontiguousarray(hi, dtype=np.int64)
+        out = np.zeros(len(lo), np.int64)
+        check(self._lib.pg_g2v_ref_index(self._ctx, len(lo), _ptr(lo), _ptr(hi), _ptr(out)), "pg_g2v_ref_index")
+        return out
+
+    def g2v_spec(self, fmt: int, col_slot, col_prev, sel_col, use_ref: bool):
+        """pg_g2v_spec: format (0 phased, 1 diplo, 2 pairs), the header's column tables and the selected samples' columns"""
+        col_slot = np.ascontiguousarray(col_slot, dtype=np.int32)
+        col_prev = np.ascontiguousarray(col_prev, dtype=np.int32)
+        sel_col = np.ascontiguousarray(sel_col, dtype=np.int32)
+        check(self._lib.pg_g2v_spec(self._ctx, int(fmt), len(col_slot), _ptr(col_slot), _ptr(col_prev), len(sel_col),
+                                    _ptr(sel_col), 1 if use_ref else 0), "pg_g2v_spec")
+
+    def g2v_chunk(self, text: bytes):
+        """pg_g2v_chunk + pg_g2v_runs: complete body lines to the device, tokenised.  Returns (data lines, first line of every
+        scaffold run, its byte offset in text)."""
+        S, nr = C.c_int64(0), C.c_int64(0)
+        check(self._lib.pg_g2v_chunk(self._ctx, text, len(text), C.byref(S), C.byref(nr)), "pg_g2v_chunk")
+        run_line = np.zeros(int(nr.value), np.int64)
+        run_off = np.zeros(int(nr.value), np.int64)
+        check(self._lib.pg_g2v_runs(self._ctx, _ptr(run_line), _ptr(run_off)), "pg_g2v_runs")
+        return int(S.value), run_line, run_off
+
+    def g2v_sites(self, run_rec):
+        """pg_g2v_sites: the site pass over the last chunk, run_rec = FASTA record of every scaffold run (-1: none).  Returns
+        (rows before the first error, their bytes, (code, data line, column, line offset)); code 0 = no error."""
+        run_rec = np.ascontiguousarray(run_rec, dtype=np.int32)
+        rows, nb = C.c_int64(0), C.c_int64(0)
+        err = np.zeros(4, np.int64)
+        check(self._lib.pg_g2v_sites(self._ctx, _ptr(run_rec) if len(run_rec) else None, C.byref(rows), C.byref(nb),
+                                     _ptr(err)), "pg_g2v_sites")
+        return int(rows.value), int(nb.value), tuple(int(v) for v in err)
+
+    def g2v_emit(self, byte0: int, buf, cap: int) -> int:
+        """Bytes byte0.. (at most cap) of the last g2v_sites' VCF rows into buf (pinned for speed); returns the bytes written"""
+        nb = C.c_size_t(0)
+        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
+        check(self._lib.pg_g2v_emit(self._ctx, int(byte0), C.c_void_p(addr), int(cap), C.byref(nb)), "pg_g2v_emit")
+        return int(nb.value)
+
     def site_counts(self, site0: int = 0, n: int = None, out=None):
         """uint16 [n, P, 4] A,C,G,T counts per population (`out`: a caller-owned array to fill, e.g. one whose pages are
         already resident — a fresh 100 MB array costs more in page faults than the kernel and the copy together)."""

@@ -503,6 +503,40 @@ int pg_seq_plan(pg_ctx* ctx, int32_t fmt, int32_t nto_gap, int32_t n_seq, const 
  * (*row1, *part1) = where the next call resumes (*row1 = n_rows: done); *bytes = bytes written. */
 int pg_seq_emit(pg_ctx* ctx, int64_t row0, int64_t part0, char* out, size_t cap, int64_t* row1, int64_t* part1, size_t* bytes);
 
+/* ---- genoToVCF.py (geno2vcf.cu) ----------------------------------------------------------------------------------------
+ * Replaces VCF_processing/genoToVCF.py makeVCFline, genomics.py GenomeSite / Genotype (317-378, 500-557) and parseFasta
+ * (2256-2261): .geno genotypes -> VCF GT records, REF from a reference FASTA. */
+
+/* The reference FASTA text[0..len) -> device; *n_rec = its '>' bytes (the starts of parseFasta's pieces). */
+int pg_g2v_ref_load(pg_ctx* ctx, const char* text, size_t len, int64_t* n_rec);
+/* The n_rec byte offsets of the '>' bytes of the last pg_g2v_ref_load, in order. */
+int pg_g2v_ref_starts(pg_ctx* ctx, int64_t* starts);
+/* Record k's sequence is bytes [lo[k], hi[k]) of the FASTA without '\n', '\r' and ' ' (lo = the piece's first newline, hi =
+ * the next '>' or the end); the sequences are compacted into one resident buffer and the text is released.
+ * rec_len[k] = length of record k's sequence. */
+int pg_g2v_ref_index(pg_ctx* ctx, int64_t n_rec, const int64_t* lo, const int64_t* hi, int64_t* rec_len);
+/* The conversion: fmt 0 phased, 1 diplo, 2 pairs; n_cols genotype columns of the header, col_slot[c] = the column's token
+ * slot (the slotted columns numbered in order) or -1, col_prev[c] = the previous column of the same name or -1; selected
+ * sample k reads column sel_col[k], or on a line with fewer columns the last column of its name the line holds (every column
+ * of such a chain has a slot); use_ref: REF from the records of pg_g2v_ref_index. */
+int pg_g2v_spec(pg_ctx* ctx, int32_t fmt, int32_t n_cols, const int32_t* col_slot, const int32_t* col_prev, int32_t n_sel,
+                const int32_t* sel_col, int32_t use_ref);
+/* A chunk of complete .geno body lines (no header line; below 4 GiB) -> device, its data lines indexed as pg_ingest_text
+ * does and tokenised; *n_lines = data lines, *n_runs = runs of lines with the same scaffold name. */
+int pg_g2v_chunk(pg_ctx* ctx, const char* text, size_t len, int64_t* n_lines, int64_t* n_runs);
+/* The first data line of every scaffold run of the last pg_g2v_chunk and its byte offset in the chunk. */
+int pg_g2v_runs(pg_ctx* ctx, int64_t* run_line, int64_t* run_off);
+/* The site pass over the last chunk: with use_ref, run_rec[i] = the FASTA record of scaffold run i, or -1 (not in the FASTA).
+ * Alleles, allele lists and row lengths, a scan for the row offsets.  *n_rows = the data lines before the first error (all
+ * when none), *n_bytes = their VCF text.  error[4] = {0, 0, 0, 0}, or {code, data line (0-based in the chunk), column, byte
+ * offset of the line in the chunk}; column 0 = the line itself, k + 1 = selected sample k, n_sel + 1 = the reference lookup;
+ * codes 1 POS not [+-]?[0-9]+, 2 no POS field, 3 POS outside int64, 4 only two fields, 5 a byte >= 0x80, 6 a '\r' that ends a
+ * line by itself, 7 the sample's column missing, 8 not a diplo code, 9 scaffold not in the FASTA, 10 POS outside the contig. */
+int pg_g2v_sites(pg_ctx* ctx, const int32_t* run_rec, int64_t* n_rows, int64_t* n_bytes, int64_t* error);
+/* Bytes [byte0, byte0 + cap) (at most to *n_bytes of pg_g2v_sites) of the VCF rows of the last site pass into out (host
+ * memory); a row may be cut anywhere.  *bytes = bytes written. */
+int pg_g2v_emit(pg_ctx* ctx, int64_t byte0, char* out, size_t cap, size_t* bytes);
+
 #ifdef __cplusplus
 }
 #endif
