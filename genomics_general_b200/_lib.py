@@ -150,6 +150,15 @@ _SIGS = {
     "pg_g2v_runs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "pg_g2v_sites": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_void_p]),
     "pg_g2v_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "pg_s2g_fasta_load": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64)]),
+    "pg_s2g_fasta_starts": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "pg_s2g_fasta_index": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pg_s2g_phylip_load": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64)]),
+    "pg_s2g_phylip_lines": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "pg_s2g_phylip_pack": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]),
+    "pg_s2g_plan": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_char_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
+                              C.POINTER(C.c_int64)]),
+    "pg_s2g_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "pg_geno_count_lines": (C.c_int, [C.c_char_p, C.c_size_t, C.POINTER(C.c_int64)]),
     "pg_geno_parse": (C.c_int, [C.c_char_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                 C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),

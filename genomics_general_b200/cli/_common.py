@@ -3,6 +3,7 @@ script: windows, populations, ploidy, files).  Citations are genomics_general/<f
 from __future__ import annotations
 
 import gzip
+import re
 import sys
 
 import numpy as np
@@ -284,3 +285,27 @@ def hap_pop_vector(gd, popNames, popInds):
             samp_pop[i] = k
     per_sample = np.array([samp_pop.get(n, -1) for n in gd.names], dtype=np.int32)
     return np.repeat(per_sample, gd.ploidy.astype(np.int64))
+
+
+FASTA_TOK = re.compile(rb"[^ \t\n\r\x0b\x0c\x1c-\x1f]+")
+FASTA_NEWLINE = re.compile(rb"[\r\n]")
+
+
+def fasta_records(data, starts, fail):
+    """genomics.parseFasta's pieces (the text between '>' bytes at `starts`) after universal newlines: (names, [first
+    newline, end) of every piece's sequence).  fail(message) is called where parseFasta raises: every piece's name is taken
+    before any piece's newline, as parseFasta does."""
+    ends = list(starts[1:]) + [len(data)]
+    names = []
+    for a, b in zip(starts, ends):
+        m = FASTA_TOK.search(data, a + 1, b)
+        if m is None:
+            fail("the record at byte %d has no name (the reference fails with an IndexError)" % a)
+        names.append(m.group().decode())
+    lo = []
+    for a, b in zip(starts, ends):
+        m = FASTA_NEWLINE.search(data, a + 1, b)
+        if m is None:
+            fail("record %s has no newline (the reference fails with a ValueError)" % names[len(lo)])
+        lo.append(m.start())
+    return names, np.array(lo, np.int64), np.array(ends, np.int64)

@@ -33,7 +33,6 @@ from .parseVCF import chunks, prefetched
 FORMATS = {"phased": 0, "diplo": 1, "pairs": 2}
 TOK = re.compile(rb"[^ \t\n\r\x0b\x0c\x1c-\x1f]+")
 EOL = re.compile(rb"\r\n|\r|\n")
-NEWLINE = re.compile(rb"[\r\n]")
 # error codes of pg_g2v_sites (include/pgwin.h); %s takes the sample name where the code names one
 ERRORS = {1: "the position is not an integer of the form [+-]digits (the reference's int() fails on it, or accepts a form "
              "such as 1_000 that this engine does not)",
@@ -74,22 +73,8 @@ def read_fai(reference):
 
 
 def fasta_records(data, starts):
-    """genomics.parseFasta's pieces (the text between '>' bytes at `starts`): (names, [first newline, end) of every
-    piece's sequence), refused where parseFasta raises"""
-    ends = list(starts[1:]) + [len(data)]
-    names = []
-    for a, b in zip(starts, ends):
-        m = TOK.search(data, a + 1, b)
-        if m is None:
-            _fail("reference FASTA: the record at byte %d has no name (the reference fails with an IndexError)" % a)
-        names.append(m.group().decode())
-    lo = []
-    for a, b in zip(starts, ends):
-        m = NEWLINE.search(data, a + 1, b)
-        if m is None:
-            _fail("reference FASTA: record %s has no newline (the reference fails with a ValueError)" % names[len(lo)])
-        lo.append(m.start())
-    return names, np.array(lo, np.int64), np.array(ends, np.int64)
+    """genomics.parseFasta's pieces of the reference (_common.fasta_records), refused where parseFasta raises"""
+    return C.fasta_records(data, starts, lambda msg: _fail("reference FASTA: " + msg))
 
 
 def read_header(src):

@@ -1,10 +1,10 @@
 // genoToVCF.py on the device: .geno genotypes -> VCF GT records, with REF from a reference FASTA (VCF_processing/genoToVCF.py
 // makeVCFline, genomics.py GenomeSite / Genotype 317-378, 500-557, parseFasta 2256-2261).
 //
-// The reference FASTA is loaded once (pg_g2v_ref_load / pg_g2v_ref_index): its text goes to HBM, k_fa_marks flags the '>'
-// bytes and a CUB select gives the record starts; the host names the records from their header pieces; k_fa_keep flags the
-// sequence bytes (after a record's first newline, not '\n', '\r' or ' ') and counts them per record, and a CUB select
-// compacts them into one resident buffer.
+// The reference FASTA is loaded once (pg_g2v_ref_load / pg_g2v_ref_index) by fasta.cu's shared loader: its text goes to
+// HBM, k_fa_marks flags the '>' bytes and a CUB select gives the record starts; the host names the records from their header
+// pieces; k_fa_keep flags the sequence bytes (after a record's first newline, not '\n', '\r' or ' ') and counts them per
+// record, and a CUB select compacts them into one resident buffer.
 // The body is streamed in chunks of complete lines.  Per chunk (pg_g2v_chunk, pg_g2v_sites, pg_g2v_emit):
 //   ingest.cu's pg_text_load uploads the text and indexes its data lines;
 //   k_g2v_tokens : ONE WARP PER DATA LINE (pg_warp_fields, which classifies a line as k_seq_tokens does): field 0 -> scaffold hash and span, field 1 -> POS as int64,
@@ -24,80 +24,6 @@
 #include "pgwin_internal.h"
 
 namespace {
-
-// str.split() blanks of ASCII text ('\n' ends the line)
-__device__ __forceinline__ bool pg_sblank(unsigned c) {
-    return c == ' ' || c == '\t' || c == '\r' || c == '\v' || c == '\f' || (c >= 0x1c && c <= 0x1f);
-}
-
-// byte i of a text of len bytes, '\n' past its end
-__device__ __forceinline__ unsigned pg_byte_at(const uint8_t* buf, size_t len, size_t i) { return i < len ? buf[i] : (unsigned)'\n'; }
-
-// ONE WARP walks the line that starts at byte l0 of buf (len bytes) as str.split() reads it: each lane classifies 4 bytes per
-// step and a warp prefix sum of the token-start flags numbers the fields.  The lane that owns the start q of field f calls
-// on_field(f, q) (in field order within a lane).  Returns the line's field count to every lane; *hi = the line holds a byte
-// >= 0x80, *lone_cr = a '\r' in it is not followed by '\n' (a line end of its own under universal newlines).  The
-// classification is seq.cu's k_seq_tokens'; the caller gives every data line its own warp.
-template <class OnField>
-__device__ __forceinline__ unsigned pg_warp_fields(const uint8_t* buf, size_t len, size_t l0, bool* hi, bool* lone_cr,
-                                                   OnField&& on_field) {
-    const int lane = threadIdx.x & 31;
-    const size_t a0 = l0 & ~(size_t)3;
-    unsigned fields_before = 0;
-    bool prev_ws = true, any_hi = false, any_cr = false, done = false;
-    for (size_t step = 0; !done; ++step) {
-        const size_t wbase = a0 + step * 128 + (size_t)lane * 4;
-        uint32_t w = 0x0a0a0a0au;
-        if (wbase + 4 <= len) w = *reinterpret_cast<const uint32_t*>(buf + wbase);
-        else if (wbase < len) {
-            for (int k = 0; k < 4; ++k)
-                if (wbase + k < len) w = (w & ~(0xffu << (8 * k))) | ((uint32_t)buf[wbase + k] << (8 * k));
-        }
-        unsigned ws = 0, nl = 0, hb = 0, cr = 0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const unsigned c = (w >> (8 * k)) & 0xffu;
-            const bool before = (wbase + k) < l0;
-            if (before || pg_sblank(c)) ws |= 1u << k;
-            else if (c == '\n') nl |= 1u << k;
-            if (!before && c >= 0x80u) hb |= 1u << k;
-            if (!before && c == '\r') cr |= 1u << k;
-        }
-        const unsigned nl_lanes = __ballot_sync(0xffffffffu, nl != 0);
-        if (nl_lanes) {
-            const int first = __ffs(nl_lanes) - 1;
-            if (lane > first) ws = 0xfu, nl = 0, hb = 0, cr = 0;
-            else if (lane == first) {
-                const unsigned from = nl & (0u - nl);
-                ws |= ~(from - 1u) & 0xfu;
-                hb &= from - 1u;
-                cr &= from - 1u;
-            }
-            done = true;
-        }
-        any_hi |= hb != 0;
-        for (unsigned m = cr; m; m &= m - 1)
-            if (pg_byte_at(buf, len, wbase + __ffs(m)) != '\n') any_cr = true;
-        const unsigned last_ws = (ws >> 3) & 1u;
-        unsigned pw = __shfl_up_sync(0xffffffffu, last_ws, 1);
-        if (lane == 0) pw = prev_ws ? 1u : 0u;
-        const unsigned prevbits = ((ws << 1) | pw) & 0xfu;
-        const unsigned st = ~ws & prevbits & 0xfu;
-        unsigned cnt = __popc(st), incl = cnt;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const unsigned v = __shfl_up_sync(0xffffffffu, incl, d);
-            if (lane >= d) incl += v;
-        }
-        unsigned fidx = fields_before + incl - cnt;
-        fields_before += __shfl_sync(0xffffffffu, incl, 31);
-        prev_ws = (__shfl_sync(0xffffffffu, last_ws, 31) != 0);
-        for (unsigned m = st; m; m &= m - 1, ++fidx) on_field(fidx, wbase + (__ffs(m) - 1));
-    }
-    *hi = __any_sync(0xffffffffu, any_hi);
-    *lone_cr = __any_sync(0xffffffffu, any_cr);
-    return fields_before;
-}
 
 enum { GE_POS = 1, GE_NO_POS = 2, GE_POS_RANGE = 3, GE_TWO_FIELDS = 4, GE_BYTE = 5, GE_CR = 6, GE_MISSING = 7, GE_DIPLO = 8,
        GE_SCAFFOLD = 9, GE_OUTSIDE = 10 };
@@ -445,59 +371,6 @@ __global__ void __launch_bounds__(256) k_g2v_emit(const __grid_constant__ G2vPar
 }
 
 
-// the FASTA: flags of the '>' bytes, and their count
-__global__ void k_fa_marks(const uint8_t* __restrict__ t, size_t n, uint8_t* __restrict__ flags,
-                           unsigned long long* __restrict__ count) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const bool gt = t[i] == '>';
-        flags[i] = gt;
-        const unsigned act = __activemask();
-        const unsigned b = __ballot_sync(act, gt);
-        if (b && (threadIdx.x & 31) == __ffs(act) - 1) atomicAdd(count, (unsigned long long)__popc(b));
-    }
-}
-
-// the FASTA: flags of the bytes of a record's sequence ([lo[k], hi[k]) without '\n', '\r' and ' ': genomics.parseFasta
-// after universal newlines), and their count per record.  FA_BYTES consecutive bytes per thread.
-constexpr int FA_BYTES = 16;
-__global__ void k_fa_keep(const uint8_t* __restrict__ t, size_t n, const int64_t* __restrict__ lo,
-                          const int64_t* __restrict__ hi, int64_t n_rec, uint8_t* __restrict__ flags,
-                          unsigned long long* __restrict__ count) {
-    const size_t nb = (n + FA_BYTES - 1) / FA_BYTES;
-    for (size_t blk0 = (size_t)blockIdx.x * blockDim.x; blk0 < nb; blk0 += (size_t)gridDim.x * blockDim.x) {
-        const size_t blk = blk0 + threadIdx.x;          // warp-uniform loop: every lane takes part in the reduction below
-        long long k = -1;
-        unsigned kept = 0;
-        if (blk < nb) {
-            const size_t i0 = blk * FA_BYTES;
-            if (lo[0] <= (int64_t)i0) {                 // the last record with lo <= i0
-                int64_t a = 0, b = n_rec - 1;
-                while (a < b) {
-                    const int64_t mid = (a + b + 1) >> 1;
-                    if (lo[mid] <= (int64_t)i0) a = mid;
-                    else b = mid - 1;
-                }
-                k = a;
-            }
-            for (size_t i = i0; i < i0 + FA_BYTES && i < n; ++i) {
-                if (k + 1 < n_rec && lo[k + 1] <= (int64_t)i) {     // a record starts inside the run: flush the count
-                    if (kept) atomicAdd(count + k, (unsigned long long)kept);
-                    kept = 0;
-                    ++k;
-                }
-                const unsigned c = t[i];
-                const bool keep = k >= 0 && (int64_t)i < hi[k] && c != '\n' && c != '\r' && c != ' ';
-                flags[i] = keep;
-                kept += keep;
-            }
-        }
-        // one atomic per warp and record: the lanes that end in the same record add up their counts first
-        const unsigned same = __match_any_sync(0xffffffffu, k);
-        const unsigned sum = __reduce_add_sync(same, kept);
-        if ((int)(threadIdx.x & 31) == __ffs(same) - 1 && k >= 0 && sum) atomicAdd(count + k, (unsigned long long)sum);
-    }
-}
-
 __global__ void k_g2v_run_off(const long long* __restrict__ starts, const long long* __restrict__ run_line, int64_t n_runs,
                               long long* __restrict__ run_off) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_runs; i += (int64_t)gridDim.x * blockDim.x)
@@ -506,10 +379,8 @@ __global__ void k_g2v_run_off(const long long* __restrict__ starts, const long l
 
 struct G2vState {
     // the reference: its text and flags until pg_g2v_ref_index, then the compacted sequences and {rec_off, rec_len}
-    PgBuf fa, flags, seq, rec, scratch, cub;
-    size_t fa_len = 0;
-    int64_t n_rec = 0;
-    bool ref_indexed = false;
+    PgFasta ref;
+    PgBuf cub;
     // the spec: col_slot [n_cols], col_prev [n_cols], sel_col [n_sel]
     PgBuf spec;
     int fmt = -1, n_cols = 0, n_slots = 0, n_sel = 0, use_ref = 0;
@@ -552,9 +423,9 @@ G2vParams params(pg_ctx* ctx, G2vState* gs) {
     p.n_runs = gs->n_runs;
     p.run_line = (const long long*)gs->runs.p;
     p.run_rec = (const int32_t*)(p.run_line + 2 * (gs->S + 1));
-    p.rec_off = (const int64_t*)gs->rec.p;
-    p.rec_len = p.rec_off + gs->n_rec;
-    p.seq = (const uint8_t*)gs->seq.p;
+    p.rec_off = (const int64_t*)gs->ref.rec.p;
+    p.rec_len = p.rec_off + gs->ref.n_rec;
+    p.seq = (const uint8_t*)gs->ref.seq.p;
     return p;
 }
 
@@ -563,8 +434,8 @@ G2vParams params(pg_ctx* ctx, G2vState* gs) {
 void pg_g2v_free(pg_ctx* ctx) {
     G2vState* gs = (G2vState*)ctx->g2v_state;
     if (!gs) return;
-    PgBuf* bufs[] = {&gs->fa, &gs->flags, &gs->seq, &gs->rec, &gs->scratch, &gs->cub, &gs->spec, &gs->tok, &gs->meta,
-                     &gs->lens, &gs->runs, &gs->err, &gs->out};
+    gs->ref.release();
+    PgBuf* bufs[] = {&gs->cub, &gs->spec, &gs->tok, &gs->meta, &gs->lens, &gs->runs, &gs->err, &gs->out};
     for (PgBuf* b : bufs) b->release();
     delete gs;
     ctx->g2v_state = nullptr;
@@ -576,110 +447,29 @@ extern "C" int pg_g2v_ref_load(pg_ctx* ctx, const char* text, size_t len, int64_
     PG_CUDA(cudaSetDevice(ctx->device));
     pg_timings_reset(ctx);
     G2vState* gs = gstate(ctx);
-    gs->ref_indexed = false;
-    gs->n_rec = 0;
-    gs->fa_len = len;
-    PG_TRY(gs->fa.ensure(len + 64));
-    PG_TRY(gs->flags.ensure(len + 64));
-    PG_TRY(gs->scratch.ensure(64));
-    unsigned long long* d_n = (unsigned long long*)gs->scratch.p;
-    PG_CUDA(cudaMemsetAsync(d_n, 0, 8, ctx->stream));
-    if (len == 0) return PG_OK;
-    {
-        const int ti = pg_time_begin(ctx, "g2v_fa_h2d");
-        PG_CUDA(cudaMemcpyAsync(gs->fa.p, text, len, cudaMemcpyHostToDevice, ctx->stream));
-        pg_time_end(ctx, ti);
-    }
-    const unsigned grid = (unsigned)std::min<size_t>((len + 255) / 256, (size_t)ctx->sm_count * 32);
-    PG_TRY(pg_timed(ctx, "g2v_fa_marks", [&] {
-        k_fa_marks<<<grid, 256, 0, ctx->stream>>>((const uint8_t*)gs->fa.p, len, (uint8_t*)gs->flags.p, d_n);
-    }));
-    unsigned long long cnt = 0;
-    PG_CUDA(cudaMemcpyAsync(&cnt, d_n, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    gs->n_rec = (int64_t)cnt;
-    if (cnt) {                                          // the record starts: offsets of the flagged bytes, into gs->rec
-        PG_TRY(gs->rec.ensure((size_t)cnt * 16 + 64));
-        thrust::counting_iterator<int64_t> idx(0);
-        size_t tmp = 0;
-        PG_CUDA(cub::DeviceSelect::Flagged(nullptr, tmp, idx, (const uint8_t*)gs->flags.p, (int64_t*)gs->rec.p, (int64_t*)d_n,
-                                           (int64_t)len, ctx->stream));
-        PG_TRY(gs->cub.ensure(tmp + 64));
-        PG_TRY(pg_timed(ctx, "g2v_fa_marks", [&] {
-            cub::DeviceSelect::Flagged(gs->cub.p, tmp, idx, (const uint8_t*)gs->flags.p, (int64_t*)gs->rec.p, (int64_t*)d_n,
-                                       (int64_t)len, ctx->stream);
-        }));
-    }
-    ctx->launches += 2;
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    *n_rec = gs->n_rec;
-    return PG_OK;
+    return pg_fa_load(ctx, gs->ref, text, len, "g2v", n_rec);
 }
 
 extern "C" int pg_g2v_ref_starts(pg_ctx* ctx, int64_t* starts) {
     PG_CHECK(ctx && starts, "pg_g2v_ref_starts: null argument");
     G2vState* gs = gstate(ctx);
-    PG_CHECK(!gs->ref_indexed, "pg_g2v_ref_starts: the record starts are gone after pg_g2v_ref_index");
-    if (gs->n_rec == 0) return PG_OK;
+    PG_CHECK(!gs->ref.indexed, "pg_g2v_ref_starts: the record starts are gone after pg_g2v_ref_index");
     PG_CUDA(cudaSetDevice(ctx->device));
-    PG_CUDA(cudaMemcpyAsync(starts, gs->rec.p, (size_t)gs->n_rec * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    return PG_OK;
+    return pg_fa_starts(ctx, gs->ref, starts);
 }
 
 extern "C" int pg_g2v_ref_index(pg_ctx* ctx, int64_t n_rec, const int64_t* lo, const int64_t* hi, int64_t* rec_len) {
     PG_CHECK(ctx && (n_rec == 0 || (lo && hi && rec_len)), "pg_g2v_ref_index: null argument");
     G2vState* gs = gstate(ctx);
-    PG_CHECK(!gs->ref_indexed && n_rec == gs->n_rec && n_rec > 0,
-             "pg_g2v_ref_index: %lld records, the last pg_g2v_ref_load found %lld", (long long)n_rec, (long long)gs->n_rec);
+    PG_CHECK(!gs->ref.indexed && n_rec == gs->ref.n_rec && n_rec > 0,
+             "pg_g2v_ref_index: %lld records, the last pg_g2v_ref_load found %lld", (long long)n_rec, (long long)gs->ref.n_rec);
     for (int64_t k = 0; k < n_rec; ++k)
-        PG_CHECK(lo[k] >= 0 && lo[k] <= hi[k] && hi[k] <= (int64_t)gs->fa_len && (k == 0 || lo[k] >= hi[k - 1]),
+        PG_CHECK(lo[k] >= 0 && lo[k] <= hi[k] && hi[k] <= (int64_t)gs->ref.fa_len && (k == 0 || lo[k] >= hi[k - 1]),
                  "pg_g2v_ref_index: record %lld spans [%lld, %lld) (sorted, disjoint, inside the %zu bytes)", (long long)k,
-                 (long long)lo[k], (long long)hi[k], gs->fa_len);
+                 (long long)lo[k], (long long)hi[k], gs->ref.fa_len);
     PG_CUDA(cudaSetDevice(ctx->device));
     pg_timings_reset(ctx);
-    const size_t len = gs->fa_len;
-    PG_TRY(gs->scratch.ensure((size_t)n_rec * 24 + 64));
-    int64_t* d_lo = (int64_t*)gs->scratch.p;
-    int64_t* d_hi = d_lo + n_rec;
-    unsigned long long* d_cnt = (unsigned long long*)(d_hi + n_rec);
-    int64_t* d_n = (int64_t*)(d_cnt + n_rec);
-    PG_CUDA(cudaMemcpyAsync(d_lo, lo, (size_t)n_rec * 8, cudaMemcpyHostToDevice, ctx->stream));
-    PG_CUDA(cudaMemcpyAsync(d_hi, hi, (size_t)n_rec * 8, cudaMemcpyHostToDevice, ctx->stream));
-    PG_CUDA(cudaMemsetAsync(d_cnt, 0, (size_t)n_rec * 8, ctx->stream));
-    const size_t nb = (len + FA_BYTES - 1) / FA_BYTES;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((nb + 255) / 256, (size_t)ctx->sm_count * 16));
-    PG_TRY(pg_timed(ctx, "g2v_fa_keep", [&] {
-        k_fa_keep<<<grid, 256, 0, ctx->stream>>>((const uint8_t*)gs->fa.p, len, d_lo, d_hi, n_rec, (uint8_t*)gs->flags.p,
-                                                 d_cnt);
-    }));
-    std::vector<unsigned long long> cnt((size_t)n_rec);
-    PG_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, (size_t)n_rec * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    std::vector<int64_t> tab((size_t)n_rec * 2);        // rec_off [n_rec], rec_len [n_rec]
-    int64_t total = 0;
-    for (int64_t k = 0; k < n_rec; ++k) {
-        tab[(size_t)k] = total;
-        tab[(size_t)(n_rec + k)] = rec_len[k] = (int64_t)cnt[(size_t)k];
-        total += (int64_t)cnt[(size_t)k];
-    }
-    PG_TRY(gs->seq.ensure((size_t)total + 64));
-    size_t tmp = 0;
-    PG_CUDA(cub::DeviceSelect::Flagged(nullptr, tmp, (const uint8_t*)gs->fa.p, (const uint8_t*)gs->flags.p, (uint8_t*)gs->seq.p,
-                                       d_n, (int64_t)len, ctx->stream));
-    PG_TRY(gs->cub.ensure(tmp + 64));
-    PG_TRY(pg_timed(ctx, "g2v_fa_select", [&] {
-        cub::DeviceSelect::Flagged(gs->cub.p, tmp, (const uint8_t*)gs->fa.p, (const uint8_t*)gs->flags.p, (uint8_t*)gs->seq.p,
-                                   d_n, (int64_t)len, ctx->stream);
-    }));
-    ctx->launches += 2;
-    PG_TRY(gs->rec.ensure(tab.size() * 8 + 64));
-    PG_CUDA(cudaMemcpyAsync(gs->rec.p, tab.data(), tab.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-    PG_CUDA(cudaStreamSynchronize(ctx->stream));
-    gs->fa.release();                                   // only the sequences stay resident
-    gs->flags.release();
-    gs->ref_indexed = true;
-    return PG_OK;
+    return pg_fa_index(ctx, gs->ref, n_rec, lo, hi, "g2v", rec_len);
 }
 
 extern "C" int pg_g2v_spec(pg_ctx* ctx, int32_t fmt, int32_t n_cols, const int32_t* col_slot, const int32_t* col_prev,
@@ -688,7 +478,7 @@ extern "C" int pg_g2v_spec(pg_ctx* ctx, int32_t fmt, int32_t n_cols, const int32
     PG_CHECK(fmt >= 0 && fmt <= 2, "pg_g2v_spec: format %d is not 0 (phased), 1 (diplo) or 2 (pairs)", fmt);
     PG_CHECK(n_sel >= 1 && n_cols >= 1, "pg_g2v_spec: %d selected samples of %d columns", n_sel, n_cols);
     G2vState* gs = gstate(ctx);
-    PG_CHECK(!use_ref || gs->ref_indexed, "pg_g2v_spec: a reference lookup without pg_g2v_ref_index");
+    PG_CHECK(!use_ref || gs->ref.indexed, "pg_g2v_spec: a reference lookup without pg_g2v_ref_index");
     int n_slots = 0;
     for (int c = 0; c < n_cols; ++c) {
         PG_CHECK(col_slot[c] == -1 || col_slot[c] == n_slots, "pg_g2v_spec: column %d has slot %d (slots number the slotted "
@@ -798,8 +588,8 @@ extern "C" int pg_g2v_sites(pg_ctx* ctx, const int32_t* run_rec, int64_t* n_rows
     pg_timings_reset(ctx);
     if (gs->use_ref)
         for (int64_t i = 0; i < gs->n_runs; ++i)
-            PG_CHECK(run_rec[i] >= -1 && run_rec[i] < gs->n_rec, "pg_g2v_sites: run %lld maps to record %d of %lld",
-                     (long long)i, run_rec[i], (long long)gs->n_rec);
+            PG_CHECK(run_rec[i] >= -1 && run_rec[i] < gs->ref.n_rec, "pg_g2v_sites: run %lld maps to record %d of %lld",
+                     (long long)i, run_rec[i], (long long)gs->ref.n_rec);
     G2vParams p = params(ctx, gs);
     if (gs->use_ref && gs->n_runs)
         PG_CUDA(cudaMemcpyAsync((void*)p.run_rec, run_rec, (size_t)gs->n_runs * 4, cudaMemcpyHostToDevice, ctx->stream));

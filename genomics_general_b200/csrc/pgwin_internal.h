@@ -138,6 +138,7 @@ struct pg_ctx {
     void* vcf_state = nullptr;                // parseVCF buffers and spec (owned by vcf.cu)
     void* seq_state = nullptr;                // genoToSeq token index and row plan (owned by seq.cu)
     void* g2v_state = nullptr;                // genoToVCF reference sequences, spec and chunk state (owned by geno2vcf.cu)
+    void* s2g_state = nullptr;                // seqToGeno sequences, line table and row plan (owned by seq2geno.cu)
     void* h_text[2] = {nullptr, nullptr};     // pinned staging of the text
     cudaEvent_t h_text_free[2] = {nullptr, nullptr};
     // upload pipeline: copy stream + two staging buffers
@@ -254,6 +255,81 @@ __device__ __forceinline__ int pg_freq_order(const int c[4], int rank[4]) {
     return nr;
 }
 
+// str.split() blanks of ASCII text ('\n' ends the line)
+__device__ __forceinline__ bool pg_sblank(unsigned c) {
+    return c == ' ' || c == '\t' || c == '\r' || c == '\v' || c == '\f' || (c >= 0x1c && c <= 0x1f);
+}
+
+// byte i of a text of len bytes, '\n' past its end
+__device__ __forceinline__ unsigned pg_byte_at(const uint8_t* buf, size_t len, size_t i) { return i < len ? buf[i] : (unsigned)'\n'; }
+
+// ONE WARP walks the line that starts at byte l0 of buf (len bytes) as str.split() reads it: each lane classifies 4 bytes per
+// step and a warp prefix sum of the token-start flags numbers the fields.  The lane that owns the start q of field f calls
+// on_field(f, q) (in field order within a lane).  Returns the line's field count to every lane; *hi = the line holds a byte
+// >= 0x80, *lone_cr = a '\r' in it is not followed by '\n' (a line end of its own under universal newlines).  The
+// classification is seq.cu's k_seq_tokens'; the caller gives every line its own warp.  Shared by genoToVCF's token pass
+// (geno2vcf.cu) and seqToGeno's PHYLIP line pass (seq2geno.cu).
+template <class OnField>
+__device__ __forceinline__ unsigned pg_warp_fields(const uint8_t* buf, size_t len, size_t l0, bool* hi, bool* lone_cr,
+                                                   OnField&& on_field) {
+    const int lane = threadIdx.x & 31;
+    const size_t a0 = l0 & ~(size_t)3;
+    unsigned fields_before = 0;
+    bool prev_ws = true, any_hi = false, any_cr = false, done = false;
+    for (size_t step = 0; !done; ++step) {
+        const size_t wbase = a0 + step * 128 + (size_t)lane * 4;
+        uint32_t w = 0x0a0a0a0au;
+        if (wbase + 4 <= len) w = *reinterpret_cast<const uint32_t*>(buf + wbase);
+        else if (wbase < len) {
+            for (int k = 0; k < 4; ++k)
+                if (wbase + k < len) w = (w & ~(0xffu << (8 * k))) | ((uint32_t)buf[wbase + k] << (8 * k));
+        }
+        unsigned ws = 0, nl = 0, hb = 0, cr = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const unsigned c = (w >> (8 * k)) & 0xffu;
+            const bool before = (wbase + k) < l0;
+            if (before || pg_sblank(c)) ws |= 1u << k;
+            else if (c == '\n') nl |= 1u << k;
+            if (!before && c >= 0x80u) hb |= 1u << k;
+            if (!before && c == '\r') cr |= 1u << k;
+        }
+        const unsigned nl_lanes = __ballot_sync(0xffffffffu, nl != 0);
+        if (nl_lanes) {
+            const int first = __ffs(nl_lanes) - 1;
+            if (lane > first) ws = 0xfu, nl = 0, hb = 0, cr = 0;
+            else if (lane == first) {
+                const unsigned from = nl & (0u - nl);
+                ws |= ~(from - 1u) & 0xfu;
+                hb &= from - 1u;
+                cr &= from - 1u;
+            }
+            done = true;
+        }
+        any_hi |= hb != 0;
+        for (unsigned m = cr; m; m &= m - 1)
+            if (pg_byte_at(buf, len, wbase + __ffs(m)) != '\n') any_cr = true;
+        const unsigned last_ws = (ws >> 3) & 1u;
+        unsigned pw = __shfl_up_sync(0xffffffffu, last_ws, 1);
+        if (lane == 0) pw = prev_ws ? 1u : 0u;
+        const unsigned prevbits = ((ws << 1) | pw) & 0xfu;
+        const unsigned st = ~ws & prevbits & 0xfu;
+        unsigned cnt = __popc(st), incl = cnt;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const unsigned v = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += v;
+        }
+        unsigned fidx = fields_before + incl - cnt;
+        fields_before += __shfl_sync(0xffffffffu, incl, 31);
+        prev_ws = (__shfl_sync(0xffffffffu, last_ws, 31) != 0);
+        for (unsigned m = st; m; m &= m - 1, ++fidx) on_field(fidx, wbase + (__ffs(m) - 1));
+    }
+    *hi = __any_sync(0xffffffffu, any_hi);
+    *lone_cr = __any_sync(0xffffffffu, any_cr);
+    return fields_before;
+}
+
 // implemented in k1.cu / k2.cu
 // pairwise statistics for the listed windows, written into the DEVICE record table (stride RC words); window w spans sites
 // [win_lo[w], win_hi[w]) of the resident matrix
@@ -264,6 +340,23 @@ void pg_filter_free(pg_ctx* ctx);        // filter.cu
 void pg_vcf_free(pg_ctx* ctx);           // vcf.cu
 void pg_seq_free(pg_ctx* ctx);           // seq.cu
 void pg_g2v_free(pg_ctx* ctx);           // geno2vcf.cu
+void pg_s2g_free(pg_ctx* ctx);           // seq2geno.cu
+// fasta.cu: the FASTA loader of genoToVCF's reference and seqToGeno's input (genomics.parseFasta after universal newlines).
+// pg_fa_load: the text -> fa, the byte offsets of its '>' bytes -> rec, *n_rec = their count; pg_fa_starts reads them back.
+// pg_fa_index: record k's sequence is bytes [lo[k], hi[k]) of the text without '\n', '\r' and ' ', compacted into seq with
+// {rec_off [n_rec], rec_len [n_rec]} in rec (int64); the text is released.  `tag` prefixes the timing labels (tag_fa_h2d,
+// tag_fa_marks, tag_fa_keep, tag_fa_select); the caller resets the timings.
+struct PgFasta {
+    PgBuf fa, flags, seq, rec, scratch, cub;
+    size_t fa_len = 0;
+    int64_t n_rec = 0;
+    bool indexed = false;
+    void release();
+};
+int pg_fa_load(pg_ctx* ctx, PgFasta& fs, const char* text, size_t len, const char* tag, int64_t* n_rec);
+int pg_fa_starts(pg_ctx* ctx, PgFasta& fs, int64_t* starts);
+int pg_fa_index(pg_ctx* ctx, PgFasta& fs, int64_t n_rec, const int64_t* lo, const int64_t* hi, const char* tag,
+                int64_t* rec_len);
 // ingest.cu: the text (memory, or bytes [file_off, file_off + len) of the open file fd) -> ctx->text, the start of every data
 // line -> ctx->starts, *n_lines = data lines; and the new-scaffold flags of S per-line scaffold hashes (both on ctx->stream)
 int pg_text_load(pg_ctx* ctx, const char* mem, int fd, size_t file_off, size_t len, int64_t* n_lines);

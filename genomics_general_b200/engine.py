@@ -643,6 +643,62 @@ class Engine:
         check(self._lib.pg_g2v_emit(self._ctx, int(byte0), C.c_void_p(addr), int(cap), C.byref(nb)), "pg_g2v_emit")
         return int(nb.value)
 
+    def s2g_fasta_load(self, text: bytes):
+        """pg_s2g_fasta_load + pg_s2g_fasta_starts: a FASTA to the device; returns the byte offsets of its '>' bytes"""
+        n = C.c_int64(0)
+        check(self._lib.pg_s2g_fasta_load(self._ctx, text, len(text), C.byref(n)), "pg_s2g_fasta_load")
+        starts = np.zeros(int(n.value), np.int64)
+        check(self._lib.pg_s2g_fasta_starts(self._ctx, _ptr(starts)), "pg_s2g_fasta_starts")
+        return starts
+
+    def s2g_fasta_index(self, lo, hi):
+        """pg_s2g_fasta_index: record k's sequence is FASTA bytes [lo[k], hi[k]) without newlines and spaces; returns the
+        sequence lengths"""
+        lo = np.ascontiguousarray(lo, dtype=np.int64)
+        hi = np.ascontiguousarray(hi, dtype=np.int64)
+        out = np.zeros(len(lo), np.int64)
+        check(self._lib.pg_s2g_fasta_index(self._ctx, len(lo), _ptr(lo), _ptr(hi), _ptr(out)), "pg_s2g_fasta_index")
+        return out
+
+    def s2g_phylip_load(self, text: bytes):
+        """pg_s2g_phylip_load + pg_s2g_phylip_lines: a PHYLIP text to the device, one warp per line; returns the line table,
+        int64 [lines, 7] = {field 0 start, its length, field 1 start, its length, fields, flags, header count}"""
+        n = C.c_int64(0)
+        check(self._lib.pg_s2g_phylip_load(self._ctx, text, len(text), C.byref(n)), "pg_s2g_phylip_load")
+        lines = np.zeros((int(n.value), 7), np.int64)
+        check(self._lib.pg_s2g_phylip_lines(self._ctx, _ptr(lines)), "pg_s2g_phylip_lines")
+        return lines
+
+    def s2g_phylip_pack(self, seq_len, spans):
+        """pg_s2g_phylip_pack: the sequences (seq_len bytes each, one after another) from the field-1 spans, int64 [n, 3] =
+        {text byte, sequence byte, bytes}"""
+        seq_len = np.ascontiguousarray(seq_len, dtype=np.int64)
+        spans = np.ascontiguousarray(spans, dtype=np.int64).reshape(-1, 3)
+        check(self._lib.pg_s2g_phylip_pack(self._ctx, len(seq_len), _ptr(seq_len), len(spans), _ptr(spans)),
+              "pg_s2g_phylip_pack")
+
+    def s2g_plan(self, names, rows, members, seps):
+        """pg_s2g_plan: one block per output contig — names[b] (bytes), rows[b], members[b] (sequence indices, in output
+        order) and seps[b] (bytes, one per member: the byte that follows it).  Returns the bytes of all rows."""
+        blk = np.zeros((len(names), 4), np.int64)
+        blk[:, 1] = [len(n) for n in names]
+        blk[:, 0] = np.concatenate([[0], np.cumsum(blk[:, 1])[:-1]]) if len(names) else []
+        blk[:, 2] = rows
+        blk[:, 3] = np.concatenate([[0], np.cumsum([len(m) for m in members])[:-1]]) if len(names) else []
+        mem = np.ascontiguousarray(np.concatenate([np.asarray(m, np.int64) for m in members]) if members else [], np.int64)
+        sep = np.frombuffer(b"".join(seps), np.uint8).copy()
+        nb = C.c_int64(0)
+        check(self._lib.pg_s2g_plan(self._ctx, len(names), _ptr(blk), b"".join(names), int(blk[:, 1].sum()), len(mem),
+                                    _ptr(mem), _ptr(sep), C.byref(nb)), "pg_s2g_plan")
+        return int(nb.value)
+
+    def s2g_emit(self, byte0: int, buf, cap: int) -> int:
+        """Bytes byte0.. (at most cap) of the last s2g_plan's rows into buf (pinned for speed); returns the bytes written"""
+        nb = C.c_size_t(0)
+        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
+        check(self._lib.pg_s2g_emit(self._ctx, int(byte0), C.c_void_p(addr), int(cap), C.byref(nb)), "pg_s2g_emit")
+        return int(nb.value)
+
     def site_counts(self, site0: int = 0, n: int = None, out=None):
         """uint16 [n, P, 4] A,C,G,T counts per population (`out`: a caller-owned array to fill, e.g. one whose pages are
         already resident — a fresh 100 MB array costs more in page faults than the kernel and the copy together)."""

@@ -537,6 +537,37 @@ int pg_g2v_sites(pg_ctx* ctx, const int32_t* run_rec, int64_t* n_rows, int64_t* 
  * memory); a row may be cut anywhere.  *bytes = bytes written. */
 int pg_g2v_emit(pg_ctx* ctx, int64_t byte0, char* out, size_t cap, size_t* bytes);
 
+/* ---- seqToGeno.py (seq2geno.cu, fasta.cu) ---------------------------------------------------------------------------------
+ * Replaces seqToGeno.py:37-98 and genomics.py parseFasta / parsePhylip / haploToPhased (2256-2283, 412-446): FASTA / PHYLIP
+ * alignments -> .geno rows.  The input must fit in device memory with 1 GiB to spare. */
+
+/* A FASTA text[0..len) -> device; *n_rec = its '>' bytes (the starts of parseFasta's pieces). */
+int pg_s2g_fasta_load(pg_ctx* ctx, const char* text, size_t len, int64_t* n_rec);
+/* The n_rec byte offsets of the '>' bytes of the last pg_s2g_fasta_load, in order. */
+int pg_s2g_fasta_starts(pg_ctx* ctx, int64_t* starts);
+/* Record k's sequence is bytes [lo[k], hi[k]) of the FASTA without '\n', '\r' and ' '; the sequences are compacted into the
+ * resident layout and the text is released.  rec_len[k] = length of record k's sequence. */
+int pg_s2g_fasta_index(pg_ctx* ctx, int64_t n_rec, const int64_t* lo, const int64_t* hi, int64_t* rec_len);
+/* A PHYLIP text[0..len) -> device, its lines indexed as pg_ingest_text does (so a line that starts with '#' is skipped: the
+ * caller refuses such text) and classified, one warp per line; *n_lines = indexed lines. */
+int pg_s2g_phylip_load(pg_ctx* ctx, const char* text, size_t len, int64_t* n_lines);
+/* The line table of the last pg_s2g_phylip_load: 7 int64 per line, {field 0's first byte (-1: none), its length, field 1's
+ * first byte (-1: none), its length, field count, flags (1 a byte >= 0x80, 2 a '\r' that ends a line by itself, 4 a header:
+ * fields 0 and 1 pass Python's int()), the header's count (clamped to int64; 0 when not a header)}. */
+int pg_s2g_phylip_lines(pg_ctx* ctx, int64_t* lines);
+/* The resident layout of n_seq sequences of seq_len[k] bytes, one after another: span[3i .. 3i + 2] = {text byte, sequence
+ * byte (in the concatenation), bytes} copies a field-1 span; the spans must fill the sequences exactly. */
+int pg_s2g_phylip_pack(pg_ctx* ctx, int64_t n_seq, const int64_t* seq_len, int64_t n_span, const int64_t* span);
+/* The rows: n_blk blocks, blk[4b .. 4b + 3] = {name offset in names, name length, rows, first member}; block b's members are
+ * [first, next block's first or n_mem), mem_rec[m] = the member's sequence (at least `rows` long), mem_sep[m] = the byte
+ * after it ('|', '\t' or '\n').  Row x of block b is "name\t<x + 1>\t" then every member's byte x and its mem_sep.
+ * *n_bytes = the bytes of all rows. */
+int pg_s2g_plan(pg_ctx* ctx, int64_t n_blk, const int64_t* blk, const char* names, int64_t names_len, int64_t n_mem,
+                const int64_t* mem_rec, const uint8_t* mem_sep, int64_t* n_bytes);
+/* Bytes [byte0, byte0 + cap) (at most to *n_bytes of pg_s2g_plan) of the rows into out (host memory); a row may be cut
+ * anywhere.  *bytes = bytes written. */
+int pg_s2g_emit(pg_ctx* ctx, int64_t byte0, char* out, size_t cap, size_t* bytes);
+
 #ifdef __cplusplus
 }
 #endif
