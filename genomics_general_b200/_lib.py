@@ -159,6 +159,14 @@ _SIGS = {
     "pg_s2g_plan": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_char_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                               C.POINTER(C.c_int64)]),
     "pg_s2g_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "pg_ws_spec": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32]),
+    "pg_ws_chunk": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                              C.POINTER(C.c_int64), C.c_void_p]),
+    "pg_ws_chunk_info": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pg_ws_set_values": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pg_ws_meta": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "pg_ws_stats": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
+                              C.c_void_p, C.c_void_p]),
     "pg_geno_count_lines": (C.c_int, [C.c_char_p, C.c_size_t, C.POINTER(C.c_int64)]),
     "pg_geno_parse": (C.c_int, [C.c_char_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                 C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),

@@ -643,6 +643,56 @@ class Engine:
         check(self._lib.pg_g2v_emit(self._ctx, int(byte0), C.c_void_p(addr), int(cap), C.byref(nb)), "pg_g2v_emit")
         return int(nb.value)
 
+    def ws_spec(self, col_slot, n_slots: int, n_fields: int):
+        """pg_ws_spec: value column c is parsed into slot col_slot[c] (-1: not read); n_fields >= 0: every line has exactly
+        that many value fields, -1: every line holds every slot's column"""
+        col_slot = np.ascontiguousarray(col_slot, dtype=np.int32)
+        check(self._lib.pg_ws_spec(self._ctx, len(col_slot), _ptr(col_slot), int(n_slots), int(n_fields)), "pg_ws_spec")
+
+    def ws_chunk(self, text: bytes):
+        """pg_ws_chunk + pg_ws_chunk_info: complete body lines appended to the resident values.  Returns (data lines, first
+        line of every scaffold run, its byte offset in text, flagged tokens as slot * lines + line, their records (offset << 32
+        | length << 2 | status), (code, data line, slot) of the first bad line)."""
+        S, nr, nf = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        err = np.zeros(3, np.int64)
+        check(self._lib.pg_ws_chunk(self._ctx, text, len(text), C.byref(S), C.byref(nr), C.byref(nf), _ptr(err)),
+              "pg_ws_chunk")
+        run_line = np.zeros(int(nr.value), np.int64)
+        run_off = np.zeros(int(nr.value), np.int64)
+        fidx = np.zeros(int(nf.value), np.int64)
+        ftok = np.zeros(int(nf.value), np.uint64)
+        check(self._lib.pg_ws_chunk_info(self._ctx, _ptr(run_line), _ptr(run_off), _ptr(fidx), _ptr(ftok)), "pg_ws_chunk_info")
+        return int(S.value), run_line, run_off, fidx, ftok, tuple(int(v) for v in err)
+
+    def ws_set_values(self, line, slot, v):
+        """pg_ws_set_values: slot[i]'s value on data line line[i] (over all chunks) = v[i]"""
+        line = np.ascontiguousarray(line, dtype=np.int64)
+        slot = np.ascontiguousarray(slot, dtype=np.int32)
+        v = np.ascontiguousarray(v, dtype=np.float64)
+        check(self._lib.pg_ws_set_values(self._ctx, len(line), _ptr(line), _ptr(slot), _ptr(v)), "pg_ws_set_values")
+
+    def ws_meta(self):
+        """pg_ws_meta: the positions of every data line so far (int64)"""
+        S = C.c_int64(0)
+        check(self._lib.pg_ws_meta(self._ctx, C.byref(S), None), "pg_ws_meta")
+        pos = np.zeros(int(S.value), np.int64)
+        check(self._lib.pg_ws_meta(self._ctx, C.byref(S), _ptr(pos)), "pg_ws_meta")
+        return pos
+
+    def ws_stats(self, lo, hi, codes, qs, n_slots: int, sort_budget: int = 1 << 30):
+        """pg_ws_stats: windows [lo[w], hi[w]) of data lines -> (float64 [W x n_slots x K], non-NaN counts [W x n_slots]);
+        codes: 0 mean, 1 median, 2 min, 3 max, 4 sd, 5 sum, 6 quantile qs[k]"""
+        lo = np.ascontiguousarray(lo, dtype=np.int64)
+        hi = np.ascontiguousarray(hi, dtype=np.int64)
+        codes = np.ascontiguousarray(codes, dtype=np.int32)
+        qs = np.ascontiguousarray(qs, dtype=np.float64)
+        W, K = len(lo), len(codes)
+        out = np.zeros((W, n_slots, K), np.float64)
+        n = np.zeros((W, n_slots), np.int64)
+        check(self._lib.pg_ws_stats(self._ctx, W, _ptr(lo), _ptr(hi), K, _ptr(codes), _ptr(qs), int(sort_budget), _ptr(out),
+                                    _ptr(n)), "pg_ws_stats")
+        return out, n
+
     def s2g_fasta_load(self, text: bytes):
         """pg_s2g_fasta_load + pg_s2g_fasta_starts: a FASTA to the device; returns the byte offsets of its '>' bytes"""
         n = C.c_int64(0)

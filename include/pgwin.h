@@ -568,6 +568,31 @@ int pg_s2g_plan(pg_ctx* ctx, int64_t n_blk, const int64_t* blk, const char* name
  * anywhere.  *bytes = bytes written. */
 int pg_s2g_emit(pg_ctx* ctx, int64_t byte0, char* out, size_t cap, size_t* bytes);
 
+/* ---- windowStats.py (wstats.cu): per-window statistics of numeric columns ----
+ * Spec: value column c (field 2 + c of a line) is parsed into slot col_slot[c] (-1: not read); every slot is read by exactly
+ * one column.  n_fields >= 0: every data line must have exactly n_fields value fields (error 4); n_fields = -1: every line
+ * must hold the columns of all slots (error 7 names the slot).  Drops the values of any earlier spec. */
+int pg_ws_spec(pg_ctx* ctx, int32_t n_cols, const int32_t* col_slot, int32_t n_slots, int32_t n_fields);
+/* Complete body lines (ASCII; '#' and blank lines skipped) appended to the resident values and positions.  *n_lines = data
+ * lines, *n_runs = scaffold runs, *n_flag = tokens the parser rejected or left to the host; error = {code, data line of the
+ * chunk, slot} of the first bad line (code 0: none; 1 position not [+-]?[0-9]+, 2 no position, 3 position outside int64,
+ * 4 field count, 5 byte >= 0x80, 6 lone '\r', 7 missing column). */
+int pg_ws_chunk(pg_ctx* ctx, const char* text, size_t len, int64_t* n_lines, int64_t* n_runs, int64_t* n_flag, int64_t* error);
+/* Of the last pg_ws_chunk: the first data line of every scaffold run and its byte offset in the chunk; the flagged tokens as
+ * slot * n_lines + line and {offset in the chunk << 32 | length << 2 | status (1 rejected, 2 left to the host)}.  Any NULL
+ * pair is skipped. */
+int pg_ws_chunk_info(pg_ctx* ctx, int64_t* run_line, int64_t* run_off, int64_t* flag_idx, uint64_t* flag_tok);
+/* Set n values: slot[i]'s value on data line line[i] (counted over all chunks) = v[i]. */
+int pg_ws_set_values(pg_ctx* ctx, int64_t n, const int64_t* line, const int32_t* slot, const double* v);
+/* *n_lines = data lines so far; pos (may be NULL) = their positions. */
+int pg_ws_meta(pg_ctx* ctx, int64_t* n_lines, int64_t* pos);
+/* Window w = data lines [lo[w], hi[w]).  out[(w * n_slots + c) * K + k] = statistic code[k] of slot c's non-NaN values in the
+ * window (0 mean, 1 median, 2 min, 3 max, 4 sd rounded to 6 decimals, 5 sum, 6 quantile q[k], numpy's linear method);
+ * n_out[w * n_slots + c] = their count.  The first call compacts the values (no pg_ws_chunk after it); median and quantiles
+ * sort the windows' values in batches of at most sort_budget bytes (one window at least). */
+int pg_ws_stats(pg_ctx* ctx, int64_t W, const int64_t* lo, const int64_t* hi, int32_t K, const int32_t* code, const double* q,
+                int64_t sort_budget, double* out, int64_t* n_out);
+
 #ifdef __cplusplus
 }
 #endif
