@@ -167,6 +167,12 @@ _SIGS = {
     "pg_ws_meta": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "pg_ws_stats": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
                               C.c_void_p, C.c_void_p]),
+    "pg_merge_setup": (C.c_int, [C.c_void_p, C.c_int64, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                 C.c_void_p, C.c_char_p, C.c_int32, C.c_char_p, C.c_int32, C.c_int32, C.c_int64, C.c_int64,
+                                 C.POINTER(C.c_int32)]),
+    "pg_merge_load": (C.c_int, [C.c_void_p, C.c_int32, C.c_char_p, C.c_size_t, C.c_void_p]),
+    "pg_merge_rows": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "pg_merge_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "pg_geno_count_lines": (C.c_int, [C.c_char_p, C.c_size_t, C.POINTER(C.c_int64)]),
     "pg_geno_parse": (C.c_int, [C.c_char_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
                                 C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),

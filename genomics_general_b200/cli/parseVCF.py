@@ -231,9 +231,10 @@ def _env_int(name, default):
     return int(v) if v else default
 
 
-def chunks(stream, target):
+def chunks(stream, target, cut_at_cr=True):
     """Complete lines in chunks of about `target` bytes, cut after the last '\\n' or '\\r' (a '\\r\\n' cut in two leaves
-    a blank line, which is skipped)"""
+    a blank line, which is skipped).  cut_at_cr=False cuts after the last '\\n' only, for callers to whom a blank line
+    matters."""
     rest = b""
     eof = False
     while True:
@@ -249,7 +250,7 @@ def chunks(stream, target):
         if eof:
             yield buf
             return
-        cut = max(buf.rfind(b"\n"), buf.rfind(b"\r")) + 1
+        cut = max(buf.rfind(b"\n"), buf.rfind(b"\r") if cut_at_cr else -1) + 1
         if cut == 0:                        # one line longer than the target: read on
             blk = stream.read(target)
             if not blk:

@@ -77,6 +77,7 @@ extern "C" int pg_ctx_destroy(pg_ctx* ctx) {
     pg_g2v_free(ctx);
     pg_s2g_free(ctx);
     pg_ws_free(ctx);
+    pg_merge_free(ctx);
     pg_nccl_finalize(ctx);
     ctx->gather.release();
     ctx->gather_flag.release();

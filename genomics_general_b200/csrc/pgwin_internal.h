@@ -140,6 +140,7 @@ struct pg_ctx {
     void* g2v_state = nullptr;                // genoToVCF reference sequences, spec and chunk state (owned by geno2vcf.cu)
     void* s2g_state = nullptr;                // seqToGeno sequences, line table and row plan (owned by seq2geno.cu)
     void* ws_state = nullptr;                 // windowStats values, positions and chunk state (owned by wstats.cu)
+    void* merge_state = nullptr;              // mergeGeno scaffold table, per-file chunks and the rows (owned by merge.cu)
     void* h_text[2] = {nullptr, nullptr};     // pinned staging of the text
     cudaEvent_t h_text_free[2] = {nullptr, nullptr};
     // upload pipeline: copy stream + two staging buffers
@@ -343,6 +344,7 @@ void pg_seq_free(pg_ctx* ctx);           // seq.cu
 void pg_g2v_free(pg_ctx* ctx);           // geno2vcf.cu
 void pg_s2g_free(pg_ctx* ctx);           // seq2geno.cu
 void pg_ws_free(pg_ctx* ctx);            // wstats.cu
+void pg_merge_free(pg_ctx* ctx);         // merge.cu
 // fasta.cu: the FASTA loader of genoToVCF's reference and seqToGeno's input (genomics.parseFasta after universal newlines).
 // pg_fa_load: the text -> fa, the byte offsets of its '>' bytes -> rec, *n_rec = their count; pg_fa_starts reads them back.
 // pg_fa_index: record k's sequence is bytes [lo[k], hi[k]) of the text without '\n', '\r' and ' ', compacted into seq with

@@ -693,6 +693,42 @@ class Engine:
                                     _ptr(n)), "pg_ws_stats")
         return out, n
 
+    def merge_setup(self, names, lengths, out, n_dummy, sep: bytes, missing: bytes, method: int, union_min: int,
+                    must_include_first: int) -> bool:
+        """pg_merge_setup: the .fai walk (names as bytes, lengths), per file whether its columns are written and its dummy
+        genotype count, the separator, the missing genotype and the rule (method 0 intersect, 1 union, 2 all).  Returns
+        True when every walk index is a row (the dense rule)."""
+        name_off = np.zeros(len(names) + 1, np.int64)
+        name_off[1:] = np.cumsum([len(n) for n in names])
+        lengths = np.ascontiguousarray(lengths, dtype=np.int64)
+        out = np.ascontiguousarray(out, dtype=np.int32)
+        n_dummy = np.ascontiguousarray(n_dummy, dtype=np.int64)
+        dense = C.c_int32(0)
+        check(self._lib.pg_merge_setup(self._ctx, len(names), b"".join(names), _ptr(name_off), _ptr(lengths), len(out),
+                                       _ptr(out), _ptr(n_dummy), sep, len(sep), missing, len(missing), int(method),
+                                       int(union_min), int(must_include_first), C.byref(dense)), "pg_merge_setup")
+        return bool(dense.value)
+
+    def merge_load(self, file: int, text: bytes):
+        """pg_merge_load: the next chunk of complete lines of a file's body.  Returns (lines, the first line that stalls the
+        file (lines when none), 0 no stall / 1 stall / 2 that line is refused, walk index of the line before the stall)."""
+        info = np.zeros(4, np.int64)
+        check(self._lib.pg_merge_load(self._ctx, int(file), text, len(text), _ptr(info)), "pg_merge_load")
+        return tuple(int(v) for v in info)
+
+    def merge_rows(self, hi: int):
+        """pg_merge_rows: the rows of walk indices (previous bound, hi]; returns (rows, bytes)"""
+        n, nb = C.c_int64(0), C.c_int64(0)
+        check(self._lib.pg_merge_rows(self._ctx, int(hi), C.byref(n), C.byref(nb)), "pg_merge_rows")
+        return int(n.value), int(nb.value)
+
+    def merge_emit(self, byte0: int, buf, cap: int) -> int:
+        """Bytes byte0.. (at most cap) of the last merge_rows' rows into buf (pinned for speed); returns the bytes written"""
+        nb = C.c_size_t(0)
+        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
+        check(self._lib.pg_merge_emit(self._ctx, int(byte0), C.c_void_p(addr), int(cap), C.byref(nb)), "pg_merge_emit")
+        return int(nb.value)
+
     def s2g_fasta_load(self, text: bytes):
         """pg_s2g_fasta_load + pg_s2g_fasta_starts: a FASTA to the device; returns the byte offsets of its '>' bytes"""
         n = C.c_int64(0)

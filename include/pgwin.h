@@ -593,6 +593,33 @@ int pg_ws_meta(pg_ctx* ctx, int64_t* n_lines, int64_t* pos);
 int pg_ws_stats(pg_ctx* ctx, int64_t W, const int64_t* lo, const int64_t* hi, int32_t K, const int32_t* code, const double* q,
                 int64_t sort_budget, double* out, int64_t* n_out);
 
+/* ---- mergeGeno.py (merge.cu): .geno files joined by position in the order of the .fai's walk ----
+ * Replaces mergeGeno.py:41-88.  The walk visits every site 1..len of every scaffold in .fai order; walk index = the offset
+ * of the scaffold (the lengths of the positive-length scaffolds before it) + site - 1.  A file's merged lines are the longest
+ * prefix of its body whose lines have >= 2 fields, name a scaffold, hold its site as str(n) with 1 <= n <= len and lie
+ * strictly after the line before in the walk. */
+
+/* The walk and the rule.  n_scaf scaffolds: name s is bytes [name_off[s], name_off[s + 1]) of names (distinct), len[s] its
+ * length (<= 0: no sites).  n_files inputs: out[x] = file x's columns are written, n_dummy[x] = its dummy genotypes (the
+ * header's fields - 2).  Rows are sep-joined; a file that did not match adds n_dummy times sep + missing.  method 0
+ * intersect, 1 union, 2 all, with the reference's unionMin and mustIncludeFirst.  *dense = 1 when every walk index is a row
+ * (`all`, or `union` with max(unionMin, mustIncludeFirst) <= 0, and mustIncludeFirst <= 0).  Drops any earlier merge. */
+int pg_merge_setup(pg_ctx* ctx, int64_t n_scaf, const char* names, const int64_t* name_off, const int64_t* len,
+                   int32_t n_files, const int32_t* out, const int64_t* n_dummy, const char* sep, int32_t sep_len,
+                   const char* missing, int32_t miss_len, int32_t method, int64_t union_min, int64_t must_include_first,
+                   int32_t* dense);
+/* The next chunk (complete '\n' lines; the last one may lack its '\n') of file `file`'s body, which must have merged every
+ * line of its previous chunk.  info = {lines of the chunk, its first line that stalls the file (the line count when none),
+ * 0 no stall / 1 the file stalls there / 2 that line is refused (a byte >= 0x80 or a lone '\r'), the walk index of the line
+ * before the stall (that of the file's last line so far, -1 none)}. */
+int pg_merge_load(pg_ctx* ctx, int32_t file, const char* text, size_t len, int64_t* info);
+/* The rows of walk indices (previous bound, hi] (hi < the walk's length), from every file's waiting lines up to hi.
+ * *n_rows = rows written, *n_bytes = their bytes. */
+int pg_merge_rows(pg_ctx* ctx, int64_t hi, int64_t* n_rows, int64_t* n_bytes);
+/* Bytes [byte0, byte0 + cap) (at most to *n_bytes of pg_merge_rows) of those rows into out (host memory); a row may be cut
+ * anywhere.  *bytes = bytes written. */
+int pg_merge_emit(pg_ctx* ctx, int64_t byte0, char* out, size_t cap, size_t* bytes);
+
 #ifdef __cplusplus
 }
 #endif
