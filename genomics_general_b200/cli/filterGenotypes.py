@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Drop-in for the reference's filterGenotypes.py (flags 124-183), on the GPU: every chunk of the input is tokenised on the
 device (strict tokens), the contig lists, --thinDist and genomics.siteTest run as site passes over the resident matrix, and
-the kept rows are formatted on the device (GenomeSite.asList) and written slab by slab.
+the kept rows are formatted on the device (GenomeSite.asList) and written slab by slab (_stream.py).
 
 Refused up front: -of randomAllele (unseeded random.sample, genomics.py:376), --HWE (inHWE calls an undefined `unique`,
 genomics.py:729), --samples that leave out a population member (siteTest raises a KeyError), -of diplo with a non-diploid
@@ -11,7 +11,7 @@ ploidy and characters outside A C G T N are reported with their data line."""
 from __future__ import annotations
 
 import argparse
-import os
+import io
 import string
 import sys
 
@@ -19,6 +19,7 @@ import numpy as np
 
 from ..engine import Engine, PinnedArray
 from . import _common as C
+from ._stream import Chain, SlabWriter, env_int, open_input, open_output
 
 FMT_CODE = {"phased": 0, "diplo": 1, "alleles": 2}
 
@@ -200,11 +201,6 @@ def plan(args, headers, first_line):
                 head=head, col_hap=col_hap, col_pl=col_pl, H=int(sum(pl)), spec=spec)
 
 
-def _env_int(name, default):
-    v = os.environ.get(name)
-    return int(v) if v else default
-
-
 def chunks(stream, target, pod_lines):
     """Complete data lines in chunks of about `target` bytes (cut at line starts).  With pod_lines, every chunk but the
     last holds a whole number of pods, so that each chunk starts a pod."""
@@ -273,32 +269,24 @@ def _first_data_line(src):
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
-    if args.infile:
-        import gzip
-        src = gzip.open(args.infile, "rb") if args.infile.endswith(".gz") else open(args.infile, "rb")
-    else:
-        src = sys.stdin.buffer
+    src = open_input(args.infile)
     head_line = src.readline()
     headers = head_line.decode().split()
     body0, first = _first_data_line(src)
     pl = plan(args, headers, first.decode())
-    import io
-    stream = io.BufferedReader(_Chain(body0, src), buffer_size=1 << 20)
+    stream = io.BufferedReader(Chain(body0, src), buffer_size=1 << 20)
     spec = pl["spec"]
     fmt = args.outputGenoFormat
     freq_order = args.alleleOrder == "freq"
-    out = C.open_out(args.outfile)
-    out.write("\t".join(pl["head"]) + "\n")
-    out.flush()
-    raw = out.buffer if hasattr(out, "buffer") else None
     tm = C.Timing(args.timing)
-    target = _env_int("PG_FILTER_CHUNK_BYTES", 1 << 30)
-    slab = _env_int("PG_FILTER_SLAB_BYTES", 64 << 20)
+    target = env_int("PG_FILTER_CHUNK_BYTES", 1 << 30)
+    slab = env_int("PG_FILTER_SLAB_BYTES", 64 << 20)
     pod_lines = args.podSize if args.thinDist else 0
     n_sites = n_kept = n_lines = 0
-    with Engine(args.device) as eng:
+    with (open_output(args.outfile) as out, Engine(args.device) as eng,
+          SlabWriter(out.write, slab, PinnedArray) as w):
+        out.write(("\t".join(pl["head"]) + "\n").encode())
         eng.set_strict_ingest(True)
-        buf = None
         for chunk in chunks(stream, target, pod_lines):
             S = eng.ingest_text(chunk, FMT_CODE[args.inputGenoFormat], pl["col_hap"], pl["col_pl"], pl["H"])
             tm.mark("ingest", eng)
@@ -332,47 +320,16 @@ def main(argv=None):
             if flags & 1 and (fmt in ("coded", "count") or freq_order) and args.verbose:
                 sys.stderr.write("filterGenotypes: kept sites with tied allele counts: their frequency order is the one a "
                                  "stable sort gives (numpy may break such ties otherwise)\n")
-            if buf is None:
-                buf = PinnedArray((slab,), np.uint8)
             row = 0
             while row < nk:
-                rows, nb = eng.filter_emit(fmt, freq_order, row, buf.array, slab)
-                if raw is not None:
-                    raw.write(memoryview(buf.array)[:nb])
-                else:
-                    out.write(bytes(buf.array[:nb]).decode())
+                rows, nb = eng.filter_emit(fmt, freq_order, row, w.slab(), w.cap)
+                w.write(nb)
                 row += rows
             n_kept += nk
             tm.mark("emit", eng)
             if args.verbose:
                 sys.stderr.write("%d lines read, %d written\n" % (n_sites, n_kept))
-        if buf is not None:
-            buf.close()
     tm.write(sites=n_sites, kept=n_kept)
-    if out is not sys.stdout:
-        out.close()
-    else:
-        out.flush()
-
-
-class _Chain(__import__("io").RawIOBase):
-    """the bytes already read from the stream, then the rest of it"""
-
-    def __init__(self, head, stream):
-        self.head, self.stream = head, stream
-
-    def readable(self):
-        return True
-
-    def readinto(self, b):
-        if self.head:
-            n = min(len(b), len(self.head))
-            b[:n] = self.head[:n]
-            self.head = self.head[n:]
-            return n
-        data = self.stream.read(len(b))
-        b[:len(data)] = data
-        return len(data)
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Drop-in for the reference's genoToSeq.py (flags 8-30), on the GPU: the .geno body goes to the device, every data line's
 token starts are indexed there, and the alignments (FASTA or PHYLIP, for the whole file, per window or per contig) are
-transposed out of the device copy of the text slab by slab, the next slab being produced while the last one is written.
+transposed out of the device copy of the text slab by slab (_stream.py).
 
 Refused before any work, where the reference crashes: --seqNameFormat other than `sample` (a KeyError), -S with -M windows or
 contigs (the generators iterate the string's characters), --windType sites without --maxDist or --overlap, --separateFiles
@@ -13,19 +13,17 @@ sample's ceil(width / 2) equals its ploidy, and the text is ASCII with '\\n' or 
 from __future__ import annotations
 
 import argparse
-import gzip
+import contextlib
 import mmap
-import os
 import re
 import string
-import sys
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
 from .. import windows as W
 from ..engine import Engine, PgError, PinnedArray
 from . import _common as C
+from ._stream import SlabWriter, env_int, open_input, open_output
 
 TOK = re.compile(rb"[^ \t\n\r\x0b\x0c\x1c-\x1f]+")
 CONTIG_WINDOW = 10 ** 7          # -M contigs: coordinate windows of 1e7 bp, step 1e7 (genoToSeq.py:74-79)
@@ -243,17 +241,13 @@ class _Writer:
         self.args = args
         self.cum = np.concatenate([[0], np.cumsum(win_bytes)]).astype(np.int64)
         self.scaffolds, self.lo, self.hi, self.pos = scaffolds, lo, hi, pos
-        self.cur, self.f = -1, None
+        self.at, self.cur, self.f = 0, -1, None
+        self.files = contextlib.ExitStack()
         if not args.separateFiles:
-            if args.seqFile:
-                if args.seqFile[-3:] == ".gz":
-                    self.f = gzip.open(args.seqFile, "wb")
-                elif args.gzip:
-                    self.f = gzip.open(args.seqFile + ".gz", "wb")
-                else:
-                    self.f = open(args.seqFile, "wb")
-            else:
-                self.f = sys.stdout.buffer
+            name = args.seqFile
+            if name and args.gzip and not name.endswith(".gz"):
+                name += ".gz"
+            self.f = self.files.enter_context(open_output(name))
 
     def _name(self, w):
         """seqFile.scaffold[_first_last].fa|.phy[.gz] (genoToSeq.py:91-100)"""
@@ -263,7 +257,8 @@ class _Writer:
         name += ".fa" if self.args.format == "fasta" else ".phy"
         return name + (".gz" if self.args.gzip else "")
 
-    def write(self, g0, view):
+    def write(self, view):
+        g0, self.at = self.at, self.at + len(view)
         if not self.args.separateFiles:
             self.f.write(view)
             return
@@ -271,9 +266,8 @@ class _Writer:
         w = int(np.searchsorted(self.cum, g0, side="right")) - 1
         while at < len(view):
             if w != self.cur:
-                self._close()
-                name = self._name(w)
-                self.f = gzip.open(name, "wb") if self.args.gzip else open(name, "wb")
+                self.files.close()
+                self.f = self.files.enter_context(open_output(self._name(w)))
                 self.cur = w
             n = min(len(view) - at, int(self.cum[w + 1]) - (g0 + at))
             self.f.write(view[at:at + n])
@@ -281,16 +275,8 @@ class _Writer:
             if g0 + at == self.cum[w + 1]:
                 w += 1
 
-    def _close(self):
-        if self.f is not None and self.f is not sys.stdout.buffer:
-            self.f.close()
-        self.f = None
-
     def close(self):
-        if self.f is sys.stdout.buffer:
-            self.f.flush()
-        else:
-            self._close()
+        self.files.close()
 
 
 def main(argv=None):
@@ -310,7 +296,7 @@ def main(argv=None):
                     first = ln
                     break
     else:
-        raw = (gzip.open(args.genoFile, "rb") if args.genoFile else sys.stdin.buffer).read()
+        raw = open_input(args.genoFile).read()
         nl = raw.find(b"\n")
         head = raw if nl < 0 else raw[:nl + 1]
         body_offset = len(head)
@@ -320,7 +306,7 @@ def main(argv=None):
     first_tokens = [t.decode("latin-1") for t in TOK.findall(first)[2:]] if first is not None else None
     pl = plan(args, all_names, first_tokens)
     tm.mark("plan")
-    slab = int(os.environ.get("PG_SEQ_SLAB_BYTES") or (64 << 20))
+    slab = env_int("PG_SEQ_SLAB_BYTES", 64 << 20)
     with Engine(args.device) as eng:
         try:
             S, err = eng.seq_index(pl["col_slot"], pl["slot_width"], pl["exact"], data=data, path=path, body_offset=body_offset)
@@ -358,28 +344,15 @@ def main(argv=None):
                                     lo, hi)
         tm.mark("plan_rows", eng)
         out = _Writer(args, scaffolds, lo, hi, pos, win_bytes)
-        total = 0
-        if R:
-            bufs = [PinnedArray((slab,), np.uint8) for _ in range(2)]
-            pending = [None, None]
-            with ThreadPoolExecutor(1) as ex:
-                row, part, k = 0, -1, 0
-                while row < R:
-                    if pending[k] is not None:
-                        pending[k].result()
-                    row, part, nb = eng.seq_emit(row, part, bufs[k].array, slab)
-                    tm.mark("emit", eng)
-                    pending[k] = ex.submit(out.write, total, memoryview(bufs[k].array)[:nb])
-                    total += nb
-                    k ^= 1
-                for f in pending:
-                    if f is not None:
-                        f.result()
-            for b in bufs:
-                b.close()
+        with SlabWriter(out.write, slab, PinnedArray) as w:
+            row, part = 0, -1
+            while row < R:
+                row, part, nb = eng.seq_emit(row, part, w.slab(), w.cap)
+                tm.mark("emit", eng)
+                w.write(nb)
         out.close()
         tm.mark("write")
-    tm.write(sites=S, alignments=len(lo), bytes=total)
+    tm.write(sites=S, alignments=len(lo), bytes=out.at)
 
 
 if __name__ == "__main__":

@@ -1,10 +1,9 @@
 #!/usr/bin/env python
 """Drop-in for the reference's VCF_processing/genoToVCF.py (flags 29-33) on the GPU: .geno genotypes become VCF GT records,
-with REF from a reference FASTA.  The body is read in chunks cut at line ends (the next chunk is read and decompressed on a
-host thread while the device works on the current one); the device indexes each chunk's lines and tokens, counts every
-site's alleles, orders them, looks up the reference base and writes the VCF rows into slabs, and the host writes (and
-gzip-compresses) one slab while the device fills the next.  The FASTA is loaded once: its sequences are compacted on the
-device and stay there.
+with REF from a reference FASTA.  The body is read in chunks cut at line ends and the rows are written slab by slab
+(_stream.py); the device indexes each chunk's lines and tokens, counts every site's alleles, orders them, looks up the
+reference base and writes the VCF rows into the slabs.  The FASTA is loaded once: its sequences are compacted on the device
+and stay there.
 
 Refused before any output, where the reference crashes or writes something else: no -f, a -s name that is not in the
 header, no selected samples, --devices N, --hostParse and --cache, a .fai line with fewer than 2 fields, a FASTA piece with
@@ -17,22 +16,17 @@ from __future__ import annotations
 
 import argparse
 import gzip
-import io
-import os
 import re
 import sys
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
 from ..engine import Engine, PinnedArray
 from . import _common as C
-from .filterGenotypes import _Chain
-from .parseVCF import chunks, prefetched
+from ._stream import SlabWriter, body_chunks, env_int, first_line, open_input, open_output
 
 FORMATS = {"phased": 0, "diplo": 1, "pairs": 2}
 TOK = re.compile(rb"[^ \t\n\r\x0b\x0c\x1c-\x1f]+")
-EOL = re.compile(rb"\r\n|\r|\n")
 # error codes of pg_g2v_sites (include/pgwin.h); %s takes the sample name where the code names one
 ERRORS = {1: "the position is not an integer of the form [+-]digits (the reference's int() fails on it, or accepts a form "
              "such as 1_000 that this engine does not)",
@@ -77,21 +71,6 @@ def fasta_records(data, starts):
     return C.fasta_records(data, starts, lambda msg: _fail("reference FASTA: " + msg))
 
 
-def read_header(src):
-    """the first line (universal newlines) and the bytes read after it"""
-    buf = b""
-    while True:
-        m = EOL.search(buf)
-        if m is not None and not (m.group() == b"\r" and m.end() == len(buf)):
-            return buf[:m.start()], buf[m.end():]
-        blk = src.read(1 << 16)
-        if not blk:
-            if not buf:
-                _fail("the input is empty: it has no header line (the reference fails with a StopIteration)")
-            return (buf[:m.start()], buf[m.end():]) if m is not None else (buf, b"")
-        buf += blk
-
-
 def plan(args, names):
     """the selected samples and the spec tables: col_slot / col_prev over the header's genotype columns, sel_col the column
     of every selected sample (dict(zip(names, GTs)) keeps the last column of a name, genomics.py:1896)"""
@@ -124,11 +103,6 @@ def header_text(args, samples, fai, has_records):
     return "".join(out).encode()
 
 
-def _env_int(name, default):
-    v = os.environ.get(name)
-    return int(v) if v else default
-
-
 def main(argv=None):
     args = build_parser().parse_args(argv)
     if args.devices not in (None, 1):
@@ -146,15 +120,15 @@ def main(argv=None):
             fa = f.read()
         if not fa.isascii():
             _fail("reference FASTA: a byte outside ASCII (this engine reads ASCII sequences only)")
-    if args.genoFile:
-        src = gzip.open(args.genoFile, "rb") if args.genoFile.endswith(".gz") else open(args.genoFile, "rb")
-    else:
-        src = sys.stdin.buffer
-    head, body0 = read_header(src)
+    src = open_input(args.genoFile)
+    first = first_line(src)
+    if first is None:
+        _fail("the input is empty: it has no header line (the reference fails with a StopIteration)")
+    head, body0 = first
     names = head.decode().split()[2:]
     samples, spec = plan(args, names)
-    target = _env_int("PG_G2V_CHUNK_BYTES", 256 << 20)
-    slab = _env_int("PG_G2V_SLAB_BYTES", 64 << 20)
+    target = env_int("PG_G2V_CHUNK_BYTES", 256 << 20)
+    slab = env_int("PG_G2V_SLAB_BYTES", 64 << 20)
     with Engine(args.device) as eng:
         rec = {}
         if fa is not None:
@@ -172,56 +146,31 @@ def main(argv=None):
             del fa
             tm.mark("reference", eng)
         eng.g2v_spec(FORMATS[args.genoFormat], spec["col_slot"], spec["col_prev"], spec["sel_col"], bool(rec))
-        if args.outFile:
-            # gzip's own default level: Python's default (9) compresses little better at a third of the speed
-            out = gzip.open(args.outFile, "wb", compresslevel=6) if args.outFile.endswith(".gz") else open(args.outFile, "wb")
-        else:
-            out = sys.stdout.buffer
-        out.write(header_text(args, samples, fai, bool(rec)))
-        sys.stderr.write("Converting...\n")
-        n_lines, n_rows, lines_before = 0, 0, 1
-        bufs = [PinnedArray((slab,), np.uint8) for _ in range(2)]
-        pending = [None, None]
-        k = 0
-        stream = io.BufferedReader(_Chain(body0, src), buffer_size=1 << 20)
-        try:
-            with ThreadPoolExecutor(1) as ex:
-                for chunk in prefetched(chunks(stream, target)):
-                    tm.mark("read")
-                    S, run_line, run_off = eng.g2v_chunk(chunk)
-                    tm.mark("tokens", eng)
-                    run_rec = np.array([rec.get(TOK.search(chunk, int(o)).group().decode(), -1) for o in run_off]
-                                       if rec else [], np.int32)
-                    rows, nbytes, err = eng.g2v_sites(run_rec)
-                    tm.mark("sites", eng)
-                    at = 0
-                    while at < nbytes:
-                        if pending[k] is not None:
-                            pending[k].result()
-                        nb = eng.g2v_emit(at, bufs[k].array, slab)
-                        tm.mark("emit", eng)
-                        pending[k] = ex.submit(out.write, memoryview(bufs[k].array)[:nb])
-                        at += nb
-                        k ^= 1
-                    if err[0]:
-                        for f in pending:
-                            if f is not None:
-                                f.result()
-                        _fail(_message(err, chunk, samples, lines_before))
-                    n_lines += S
-                    n_rows += rows
-                    lines_before += chunk.count(b"\n")
-                    sys.stderr.write("{} lines converted...\n".format(n_lines))
-                for f in pending:
-                    if f is not None:
-                        f.result()
-        finally:
-            for b in bufs:
-                b.close()
-            if out is not sys.stdout.buffer:
-                out.close()
-            else:
-                out.flush()
+        with open_output(args.outFile) as out, SlabWriter(out.write, slab, PinnedArray) as w:
+            out.write(header_text(args, samples, fai, bool(rec)))
+            sys.stderr.write("Converting...\n")
+            n_lines, n_rows, lines_before = 0, 0, 1
+            for chunk in body_chunks(body0, src, target):
+                tm.mark("read")
+                S, run_line, run_off = eng.g2v_chunk(chunk)
+                tm.mark("tokens", eng)
+                run_rec = np.array([rec.get(TOK.search(chunk, int(o)).group().decode(), -1) for o in run_off]
+                                   if rec else [], np.int32)
+                rows, nbytes, err = eng.g2v_sites(run_rec)
+                tm.mark("sites", eng)
+                at = 0
+                while at < nbytes:
+                    nb = eng.g2v_emit(at, w.slab(), w.cap)
+                    tm.mark("emit", eng)
+                    w.write(nb)
+                    at += nb
+                if err[0]:
+                    w.wait()
+                    _fail(_message(err, chunk, samples, lines_before))
+                n_lines += S
+                n_rows += rows
+                lines_before += chunk.count(b"\n")
+                sys.stderr.write("{} lines converted...\n".format(n_lines))
         tm.mark("write")
     tm.write(lines=n_lines, rows=n_rows)
 

@@ -2,13 +2,13 @@
 """Drop-in for the reference's mergeGeno.py on the GPU: several .geno files joined into one table keyed by position, in the
 order of the .fai's walk (every site 1..length of every scaffold), by --method intersect, union or all.
 
-The host reads the .fai, the headers and the flags; each body is read in chunks of complete lines (the next chunk is read and
-decompressed on a host thread), and the device indexes each chunk's lines, finds where the file stalls (the first line that
-the reference's walk would never consume: fewer than two fields, a scaffold not in the .fai, a site that is not str(n) for
-1 <= n <= length, or a position not after the line before), merges the files' positions up to a bound and writes the rows
-into slabs; the host writes (and gzip-compresses) one slab while the device fills the next.  The bound of each round is the
-smallest last loaded position over the files still reading, so only the file(s) that set it read their next chunk and the
-device holds about one chunk per file: inputs larger than device memory stream through.
+The host reads the .fai, the headers and the flags; each body is read in chunks of complete lines, cut at '\\n' only
+(_stream.py), and the device indexes each chunk's lines, finds where the file stalls (the first line that the reference's
+walk would never consume: fewer than two fields, a scaffold not in the .fai, a site that is not str(n) for 1 <= n <=
+length, or a position not after the line before), merges the files' positions up to a bound and writes the rows into
+slabs.  The bound of each round is the smallest last loaded position over the files still reading, so only the file(s)
+that set it read their next chunk and the device holds about one chunk per file: inputs larger than device memory stream
+through.
 
 Refused before any output, where the reference crashes: an input that cannot be opened or read, a .fai line with fewer than
 2 fields or a length int() rejects, an --outputOnly index outside the files.  Narrowed (DESIGN.md section 8): a .fai that
@@ -18,22 +18,14 @@ line found after rows were written removes the -o file.  --verbose reports each 
 from __future__ import annotations
 
 import argparse
-import gzip
-import io
 import os
-import re
 import sys
-from concurrent.futures import ThreadPoolExecutor
-
-import numpy as np
 
 from ..engine import Engine, PinnedArray
 from . import _common as C
-from .filterGenotypes import _Chain
-from .parseVCF import chunks, prefetched
+from ._stream import SlabWriter, body_chunks, env_int, first_line, open_input, open_output
 
 METHODS = {"intersect": 0, "union": 1, "all": 2}
-EOL = re.compile(rb"\r\n|\r|\n")
 WALK_LIMIT = 1 << 62
 
 
@@ -56,11 +48,6 @@ def build_parser():
 
 def _fail(msg):
     raise SystemExit("mergeGeno: " + msg)
-
-
-def _env_int(name, default):
-    v = os.environ.get(name)
-    return int(v) if v else default
 
 
 def read_fai(path):
@@ -91,22 +78,9 @@ def read_fai(path):
     return scafs
 
 
-def read_header(src):
-    """the first line (universal newlines, as the reference's readline) and the bytes read after it"""
-    buf = b""
-    while True:
-        m = EOL.search(buf)
-        if m is not None and not (m.group() == b"\r" and m.end() == len(buf)):
-            return buf[:m.start()], buf[m.end():]
-        blk = src.read(1 << 16)
-        if not blk:
-            return (buf[:m.start()], buf[m.end():]) if m is not None else (buf, b"")
-        buf += blk
-
-
-def open_input(path):
+def _open(path):
     try:
-        return gzip.open(path, "rb") if path.endswith(".gz") else open(path, "rb")
+        return open_input(path)
     except OSError as e:
         _fail("cannot open input %s: %s" % (path, e))
 
@@ -118,13 +92,13 @@ def main(argv=None):
     if args.hostParse or args.cache:
         _fail("--hostParse and --cache do not apply: the merge streams the text through the GPU")
     tm = C.Timing(args.timing)
-    srcs = [open_input(p) for p in args.inputFile]
+    srcs = [_open(p) for p in args.inputFile]
     nF = len(srcs)
     scafs = read_fai(args.fai)
     heads, bodies = [], []
     for path, src in zip(args.inputFile, srcs):
         try:
-            h, rest = read_header(src)
+            h, rest = first_line(src) or (b"", b"")
             heads.append(h.decode().split())
         except (OSError, EOFError, UnicodeDecodeError) as e:
             _fail("cannot read the header of %s: %s" % (path, e))
@@ -135,9 +109,9 @@ def main(argv=None):
             _fail("--outputOnly %d: there are %d input files (the reference fails with an IndexError)" % (i + 1, nF))
     sep = args.outSep
     header = sep.join([sep.join(heads[0][0:2]), sep.join([sep.join(heads[x][2:]) for x in out_idx])]) + "\n"
-    target = _env_int("PG_MERGE_CHUNK_BYTES", 64 << 20)
-    slab = _env_int("PG_MERGE_SLAB_BYTES", 64 << 20)
-    dense_rows = _env_int("PG_MERGE_DENSE_ROWS", 1 << 22)
+    target = env_int("PG_MERGE_CHUNK_BYTES", 64 << 20)
+    slab = env_int("PG_MERGE_SLAB_BYTES", 64 << 20)
+    dense_rows = env_int("PG_MERGE_DENSE_ROWS", 1 << 22)
     total = sum(max(n, 0) for _, n in scafs)
     tm.mark("setup")
     with Engine(args.device) as eng:
@@ -145,12 +119,11 @@ def main(argv=None):
                                 [1 if x in out_idx else 0 for x in range(nF)], [max(len(h) - 2, 0) for h in heads],
                                 sep.encode(), args.missing.encode(), METHODS[args.method], args.unionMin,
                                 args.mustIncludeFirst)
-        gens = [prefetched(chunks(io.BufferedReader(_Chain(b, s), buffer_size=1 << 20), target, cut_at_cr=False))
-                for b, s in zip(bodies, srcs)]
+        gens = [body_chunks(b, s, target, cut_at_cr=False) for b, s in zip(bodies, srcs)]
         last = [-1] * nF                        # walk index of each file's last loaded line
         done = [False] * nF                     # stalled or at its end: sets no bound
         lines_before = [0] * nF
-        out = None
+        out = w = None
 
         def load(x):
             chunk = next(gens[x], None)
@@ -161,7 +134,7 @@ def main(argv=None):
             n, stall, state, key = eng.merge_load(x, chunk)
             tm.mark("lines", eng)
             if state == 2:
-                _refuse(args, out, "%s line %d: a byte outside ASCII or a '\\r' that ends a line by itself (the reference "
+                _refuse(args, out, w, "%s line %d: a byte outside ASCII or a '\\r' that ends a line by itself (the reference "
                         "reads characters and universal newlines, which this engine does not)"
                         % (args.inputFile[x], lines_before[x] + stall + 2))
             lines_before[x] += n
@@ -174,59 +147,33 @@ def main(argv=None):
 
         for x in range(nF):
             load(x)
-        if args.outputFile:
-            # gzip's own default level: Python's default (9) compresses little better at a third of the speed
-            out = gzip.open(args.outputFile, "wb", compresslevel=6) if args.outputFile.endswith(".gz") \
-                else open(args.outputFile, "wb")
-        else:
-            out = sys.stdout.buffer
-        out.write(header.encode())
-        sys.stderr.write("Merging...\n")
-        n_rows = 0
-        bufs = [PinnedArray((slab,), np.uint8) for _ in range(2)]
-        pending = [None, None]
-        k = 0
-        try:
-            with ThreadPoolExecutor(1) as ex:
-                prev = -1
-                while total > 0:
-                    live = [last[x] for x in range(nF) if not done[x]]
-                    bound = min(live) if live else total - 1
-                    while prev < bound:
-                        hi = min(bound, prev + dense_rows) if dense else bound
-                        rows, nbytes = eng.merge_rows(hi)
-                        tm.mark("rows", eng)
-                        at = 0
-                        while at < nbytes:
-                            if pending[k] is not None:
-                                pending[k].result()
-                            nb = eng.merge_emit(at, bufs[k].array, slab)
-                            tm.mark("emit", eng)
-                            pending[k] = ex.submit(out.write, memoryview(bufs[k].array)[:nb])
-                            at += nb
-                            k ^= 1
-                        n_rows += rows
-                        prev = hi
-                    if args.verbose:
-                        sys.stderr.write("Merged to walk position {}: {} lines written.\n".format(prev + 1, n_rows))
-                    if not live:
-                        break
-                    for x in range(nF):
-                        if not done[x] and last[x] == bound:
-                            for f in pending:
-                                if f is not None:
-                                    f.result()
-                            load(x)
-                for f in pending:
-                    if f is not None:
-                        f.result()
-        finally:
-            for b in bufs:
-                b.close()
-            if out is sys.stdout.buffer:
-                out.flush()
-            elif not out.closed:
-                out.close()
+        with open_output(args.outputFile) as out, SlabWriter(out.write, slab, PinnedArray) as w:
+            out.write(header.encode())
+            sys.stderr.write("Merging...\n")
+            n_rows = 0
+            prev = -1
+            while total > 0:
+                live = [last[x] for x in range(nF) if not done[x]]
+                bound = min(live) if live else total - 1
+                while prev < bound:
+                    hi = min(bound, prev + dense_rows) if dense else bound
+                    rows, nbytes = eng.merge_rows(hi)
+                    tm.mark("rows", eng)
+                    at = 0
+                    while at < nbytes:
+                        nb = eng.merge_emit(at, w.slab(), w.cap)
+                        tm.mark("emit", eng)
+                        w.write(nb)
+                        at += nb
+                    n_rows += rows
+                    prev = hi
+                if args.verbose:
+                    sys.stderr.write("Merged to walk position {}: {} lines written.\n".format(prev + 1, n_rows))
+                if not live:
+                    break
+                for x in range(nF):
+                    if not done[x] and last[x] == bound:
+                        load(x)
         tm.mark("write")
         for g in gens:
             g.close()
@@ -234,9 +181,11 @@ def main(argv=None):
     tm.write(files=nF, rows=n_rows, walk=total)
 
 
-def _refuse(args, out, msg):
-    """refuse the run: an output file already begun is removed"""
-    if out is not None and out is not sys.stdout.buffer:
+def _refuse(args, out, w, msg):
+    """refuse the run: every submitted write finishes, and an output file already begun is removed"""
+    if w is not None:
+        w.wait()
+    if out is not None and args.outputFile:
         out.close()
         os.remove(args.outputFile)
     _fail(msg)

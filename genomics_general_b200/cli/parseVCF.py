@@ -1,10 +1,9 @@
 #!/usr/bin/env python
 """Drop-in for the reference's VCF_processing/parseVCF.py (flags 257-289, 327) on the GPU: the VCF body is read in chunks
-cut at line ends (the next chunk is read and decompressed on a host thread while the device works on the current one),
-each chunk is indexed and tokenised on the device (k_vcf_records), the genotypes are evaluated there (k_vcf_genotypes) and
-the .geno rows are formatted there and written slab by slab (k_vcf_emit).  The host parses the header, applies the contig
-lists, settles the few tokens the device's number parser leaves unresolved with Python's own int() / float(), and checks
-every line with a byte >= 0x80 against str.split().
+cut at line ends (_stream.py), each chunk is indexed and tokenised on the device (k_vcf_records), the genotypes are
+evaluated there (k_vcf_genotypes) and the .geno rows are formatted there and written slab by slab (k_vcf_emit).  The host
+parses the header, applies the contig lists, settles the few tokens the device's number parser leaves unresolved with
+Python's own int() / float(), and checks every line with a byte >= 0x80 against str.split().
 
 Refused up front: --simplifyALT and --expandMulti (INFO CIGAR parsing; the reference raises a KeyError on any record
 without CIGAR), --field alleles (the reference joins a tuple and raises a TypeError), --devices N, a #CHROM line that does
@@ -16,17 +15,15 @@ from __future__ import annotations
 
 import argparse
 import math
-import os
 import re
 import sys
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
 from .. import _lib as L
 from ..engine import Engine, PinnedArray
 from . import _common as C
-from .filterGenotypes import _Chain
+from ._stream import SlabWriter, body_chunks, env_int, open_input, open_output
 
 FIXED = ["#CHROM", "POS", "ID", "REF", "ALT", "QUAL", "FILTER", "INFO", "FORMAT"]
 ASCII_WS = re.compile(rb"[ \t\n\r\x0b\x0c\x1c-\x1f]+")
@@ -226,53 +223,6 @@ def plan(args, head_line):
     return dict(headers=headers, samples=samples, min_fields=min_fields, spec=spec)
 
 
-def _env_int(name, default):
-    v = os.environ.get(name)
-    return int(v) if v else default
-
-
-def chunks(stream, target, cut_at_cr=True):
-    """Complete lines in chunks of about `target` bytes, cut after the last '\\n' or '\\r' (a '\\r\\n' cut in two leaves
-    a blank line, which is skipped).  cut_at_cr=False cuts after the last '\\n' only, for callers to whom a blank line
-    matters."""
-    rest = b""
-    eof = False
-    while True:
-        buf = rest
-        while len(buf) < target and not eof:
-            blk = stream.read(max(target - len(buf), 1))
-            if not blk:
-                eof = True
-                break
-            buf += blk
-        if not buf:
-            return
-        if eof:
-            yield buf
-            return
-        cut = max(buf.rfind(b"\n"), buf.rfind(b"\r") if cut_at_cr else -1) + 1
-        if cut == 0:                        # one line longer than the target: read on
-            blk = stream.read(target)
-            if not blk:
-                eof = True
-            rest = buf + blk
-            continue
-        yield buf[:cut]
-        rest = buf[cut:]
-
-
-def prefetched(gen):
-    """the items of gen, each read on a host thread while the caller works on the one before"""
-    with ThreadPoolExecutor(1) as ex:
-        fut = ex.submit(next, gen, None)
-        while True:
-            item = fut.result()
-            if item is None:
-                return
-            fut = ex.submit(next, gen, None)
-            yield item
-
-
 def _gt_type(alleles):
     s = set(alleles)
     return "Het" if len(s) > 1 else ("HomRef" if "0" in s else ("Missing" if "." in s else "HomAlt"))
@@ -384,11 +334,7 @@ def main(argv=None):
         _fail("--field alleles is not supported: the reference joins a tuple there and raises a TypeError")
     if args.devices not in (None, 1):
         _fail("--devices is not supported; the conversion runs on one GPU")
-    if args.inFile:
-        import gzip
-        src = gzip.open(args.inFile, "rb") if args.inFile.endswith(".gz") else open(args.inFile, "rb")
-    else:
-        src = sys.stdin.buffer
+    src = open_input(args.inFile)
     pre, head_line, body0 = read_header(src)
     for ln in pre:
         if ln.startswith("##contig"):
@@ -396,22 +342,17 @@ def main(argv=None):
     pl = plan(args, head_line)
     inc, exc = _contigs(args)
     samples = pl["samples"]
-    out = C.open_out(args.outFile)
-    if not args.noHeader:
-        out.write(args.outSep.join(["#CHROM", "POS"] + (["REF"] if args.addRefTrack else []) + samples) + "\n")
-    out.flush()
-    raw = out.buffer if hasattr(out, "buffer") else None
     tm = C.Timing(args.timing)
-    target = _env_int("PG_VCF_CHUNK_BYTES", 256 << 20)
-    slab = _env_int("PG_VCF_SLAB_BYTES", 64 << 20)
+    target = env_int("PG_VCF_CHUNK_BYTES", 256 << 20)
+    slab = env_int("PG_VCF_SLAB_BYTES", 64 << 20)
     n_lines = n_rows = 0
     prev = None
-    import io
-    stream = io.BufferedReader(_Chain(body0, src), buffer_size=1 << 20)
-    with Engine(args.device) as eng:
+    with (open_output(args.outFile) as out, Engine(args.device) as eng,
+          SlabWriter(out.write, slab, PinnedArray) as w):
+        if not args.noHeader:
+            out.write((args.outSep.join(["#CHROM", "POS"] + (["REF"] if args.addRefTrack else []) + samples) + "\n").encode())
         eng.vcf_set_spec(pl["spec"])
-        buf = None
-        for chunk in prefetched(chunks(stream, target)):
+        for chunk in body_chunks(body0, src, target):
             tm.mark("read")
             S = eng.vcf_load(chunk, prev)
             if S == 0:
@@ -440,15 +381,10 @@ def main(argv=None):
                         v[r, s] |= V_FAIL
                 eng.vcf_verdicts(len(rows), len(samples), put=v)
                 tm.mark("settle")
-            if buf is None:
-                buf = PinnedArray((slab,), np.uint8)
             row = 0
             while row < len(rows):
-                k, nb = eng.vcf_emit(row, buf.array, slab)
-                if raw is not None:
-                    raw.write(memoryview(buf.array)[:nb])
-                else:
-                    out.write(bytes(buf.array[:nb]).decode())
+                k, nb = eng.vcf_emit(row, w.slab(), w.cap)
+                w.write(nb)
                 row += k
             tm.mark("emit", eng)
             last = recs[-1]
@@ -458,13 +394,7 @@ def main(argv=None):
                         chunk[s0 + last["pos_off"]:s0 + last["pos_off"] + last["pos_len"]])
             n_lines += S
             n_rows += len(rows)
-        if buf is not None:
-            buf.close()
     tm.write(lines=n_lines, rows=n_rows)
-    if out is not sys.stdout:
-        out.close()
-    else:
-        out.flush()
 
 
 if __name__ == "__main__":

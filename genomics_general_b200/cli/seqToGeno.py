@@ -3,8 +3,7 @@
 per site and one column per sequence (-M samples), one row per site of every sequence (-M contigs), or one contig per
 alignment of a multi-PHYLIP file.  The text goes to the device once: a FASTA through the loader genoToVCF uses for its
 reference, a PHYLIP file through a warp-per-line pass whose line table the host turns into the sequences' field-1 spans.
-The transpose of the resident sequences into rows runs on the device, slab by slab, and the host writes (and
-gzip-compresses) one slab while the device fills the next.
+The transpose of the resident sequences into rows runs on the device, slab by slab (_stream.py).
 
 Refused before any output, where the reference crashes: a single -P value > 1 (a list multiplied by a float), -P values
 below 1 where a ploidy > 1 groups the sequences, a -P list that does not sum to the number of sequences (an assertion),
@@ -21,16 +20,13 @@ path, as the reference reads the whole file)."""
 from __future__ import annotations
 
 import argparse
-import gzip
-import os
 import re
-import sys
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
 from ..engine import Engine, PgError, PinnedArray
 from . import _common as C
+from ._stream import SlabWriter, env_int, open_input, open_output
 
 LF_HI, LF_CR, LF_HEAD = 1, 2, 4       # flags of the PHYLIP line table (include/pgwin.h pg_s2g_phylip_lines)
 
@@ -72,13 +68,6 @@ def check_args(args):
         if args.randomPhase:
             _fail("--randomPhase with a ploidy above 1 is not supported: the reference takes len() of a zip "
                   "(genomics.py:437) and fails with a TypeError")
-
-
-def read_input(path):
-    if path:
-        with (gzip.open(path, "rb") if path.endswith(".gz") else open(path, "rb")) as f:
-            return f.read()
-    return sys.stdin.buffer.read()
 
 
 def _line_of(data, at):
@@ -227,12 +216,12 @@ def main(argv=None):
     args = build_parser().parse_args(argv)
     check_args(args)
     tm = C.Timing(args.timing)
-    data = read_input(args.seqFile)
+    data = open_input(args.seqFile).read()
     tm.mark("read")
     if not data.isascii():
         _fail("a byte outside ASCII at line %d (the reference reads characters, which this engine does not)" %
               _line_of(data, re.search(rb"[\x80-\xff]", data).start()))
-    slab = int(os.environ.get("PG_S2G_SLAB_BYTES") or (64 << 20))
+    slab = env_int("PG_S2G_SLAB_BYTES", 64 << 20)
     with Engine(args.device) as eng:
         try:
             if args.format == "fasta":
@@ -250,36 +239,14 @@ def main(argv=None):
         total = eng.s2g_plan([b[0] for b in blocks], [b[1] for b in blocks], [b[2] for b in blocks],
                              [b[3] for b in blocks])
         tm.mark("plan", eng)
-        if args.genoFile:
-            # gzip's own default level: Python's default (9) compresses little better at a third of the speed
-            out = gzip.open(args.genoFile, "wb", compresslevel=6) if args.genoFile.endswith(".gz") else \
-                open(args.genoFile, "wb")
-        else:
-            out = sys.stdout.buffer
-        bufs = [PinnedArray((slab,), np.uint8) for _ in range(2)]
-        pending = [None, None]
-        try:
+        with open_output(args.genoFile) as out, SlabWriter(out.write, slab, PinnedArray) as w:
             out.write(head)
-            with ThreadPoolExecutor(1) as ex:
-                at, k = 0, 0
-                while at < total:
-                    if pending[k] is not None:
-                        pending[k].result()
-                    nb = eng.s2g_emit(at, bufs[k].array, slab)
-                    tm.mark("emit", eng)
-                    pending[k] = ex.submit(out.write, memoryview(bufs[k].array)[:nb])
-                    at += nb
-                    k ^= 1
-                for f in pending:
-                    if f is not None:
-                        f.result()
-        finally:
-            for b in bufs:
-                b.close()
-            if out is not sys.stdout.buffer:
-                out.close()
-            else:
-                out.flush()
+            at = 0
+            while at < total:
+                nb = eng.s2g_emit(at, w.slab(), w.cap)
+                tm.mark("emit", eng)
+                w.write(nb)
+                at += nb
         tm.mark("write")
     tm.write(sequences=int(len(lens)), rows=int(sum(b[1] for b in blocks)), bytes=int(total))
 

@@ -1,27 +1,23 @@
 #!/usr/bin/env python
 """Drop-in for the reference's windowStats.py on the GPU: per-window mean, median, min, max, sd, sum and quantiles of the
 numeric columns of a per-site table (scaffold, position, value columns), in sliding coordinate, sliding sites or predefined
-windows.  The text is read in chunks cut at line ends (the next chunk is read on a host thread while the device parses the
-current one); the device parses every value to float64, keeps them column-major with the positions, and reduces every
-(window, column) pair in one warp with numpy's own summation order.  The windows come from windows.py, the rows are printed
-by the native row formatter.
+windows.  The text is read in chunks cut at line ends (_stream.py); the device parses every value to float64, keeps them
+column-major with the positions, and reduces every (window, column) pair in one warp with numpy's own summation order.  The
+windows come from windows.py, the rows are printed by the native row formatter.
 
 Where the reference crashes under Python 3 the command line does what the script evidently means (DESIGN.md section 8): -o
 writes the file (gzip for .gz), .gz input is read as text, --include / --exclude read one scaffold per line, and failed
 windows and quantiles of an empty column are written as nan.  Refused before any output: a value float() rejects inside an
 evaluated window, min or max of an evaluated window whose column has no value, a line whose field count differs from the
-header (without --columns) or that lacks a named column (with --columns), a --columns name not in the header.  Narrowed:
+header (without --columns) or that lacks a named column (with --columns), a --columns name not in the header, an empty
+input without --headers.  Narrowed:
 ASCII only, a lone '\\r' line end, positions other than [+-]?[0-9]+ within int64, and coordinate or predefined windows over
 positions that decrease within a scaffold run.  Blank lines are skipped.  --verbose and --writeFailedWindows have no effect,
 as in the reference."""
 from __future__ import annotations
 
 import argparse
-import gzip
-import io
-import os
 import re
-import sys
 
 import numpy as np
 
@@ -29,9 +25,7 @@ from .. import geno_io
 from .. import windows as W
 from ..engine import Engine
 from . import _common as C
-from .filterGenotypes import _Chain
-from .genoToVCF import read_header
-from .parseVCF import chunks, prefetched
+from ._stream import body_chunks, env_int, first_line, open_input, open_output
 
 STATS = ("mean", "median", "min", "max", "sd", "sum", "q5", "q10", "q25", "q75", "q90", "q95")
 CODES = {"mean": (0, 0.0), "median": (1, 0.0), "min": (2, 0.0), "max": (3, 0.0), "sd": (4, 0.0), "sum": (5, 0.0),
@@ -133,11 +127,6 @@ def plan(names, columns):
     return out_names, col_slot, len(cols), [slot_of[c] for c in read]
 
 
-def _env_int(name, default):
-    v = os.environ.get(name)
-    return int(v) if v else default
-
-
 def main(argv=None):
     args = build_parser().parse_args(argv)
     if args.devices not in (None, 1):
@@ -147,28 +136,27 @@ def main(argv=None):
     codes = [CODES[s][0] for s in args.stats]
     qs = [CODES[s][1] for s in args.stats]
     tm = C.Timing(args.timing)
-    if args.inFile:
-        src = gzip.open(args.inFile, "rb") if args.inFile.endswith(".gz") else open(args.inFile, "rb")
-    else:
-        src = sys.stdin.buffer
+    src = open_input(args.inFile)
     if args.headers:
         head, body0 = " ".join(args.headers).encode(), b""
     else:
-        head, body0 = read_header(src)
+        first = first_line(src)
+        if first is None:
+            _fail("the input is empty: it has no header line (the reference fails with a StopIteration)")
+        head, body0 = first
     try:
         names = head.decode("ascii").split()[2:]
     except UnicodeDecodeError:
         _fail("the header has a byte outside ASCII (this engine reads ASCII text only)")
     out_names, col_slot, n_slots, out_slot = plan(names, args.columns)
-    target = _env_int("PG_WS_CHUNK_BYTES", 256 << 20)
-    budget = _env_int("PG_WS_SORT_BYTES", 1 << 30)
+    target = env_int("PG_WS_CHUNK_BYTES", 256 << 20)
+    budget = env_int("PG_WS_SORT_BYTES", 1 << 30)
     with Engine(args.device) as eng:
         eng.ws_spec(col_slot, n_slots, -1 if args.columns else len(names))
         run_names, run_start = [], []       # scaffold runs over all data lines
         rejected = []                       # (data line, slot, file line) of tokens float() rejects
         n_lines, lines_before, n_host = 0, 1 if not args.headers else 0, 0
-        stream = io.BufferedReader(_Chain(body0, src), buffer_size=1 << 20)
-        for chunk in prefetched(chunks(stream, target)):
+        for chunk in body_chunks(body0, src, target):
             tm.mark("read")
             S, run_line, run_off, fidx, ftok, err = eng.ws_chunk(chunk)
             tm.mark("parse", eng)
@@ -265,11 +253,7 @@ def main(argv=None):
             start, end = ws.start[w], ws.end[w]
         mid = W.mid_pos(int(p.sum()), n)
         prefixes.append("%s,%s,%s,%s,%d," % (ws.scaffold[w], start, end, mid, n))
-    if args.outFile:
-        out = gzip.open(args.outFile, "wb") if args.outFile.endswith(".gz") else open(args.outFile, "wb")
-    else:
-        out = sys.stdout.buffer
-    try:
+    with open_output(args.outFile) as out:
         out.write(b"scaffold,start,end,mid,sites")
         if len(ws):
             out.write("".join("," + ",".join(n + "_" + s for s in args.stats) for n in out_names).encode() + b"\n")
@@ -277,11 +261,6 @@ def main(argv=None):
                 out.write(geno_io.format_matrix_rows(M, sep=",", prefixes=prefixes).encode())
             else:
                 out.write("".join(p + "\n" for p in prefixes).encode())
-    finally:
-        if out is not sys.stdout.buffer:
-            out.close()
-        else:
-            out.flush()
     tm.mark("write")
     tm.write(lines=n_lines, windows=len(ws), host_tokens=n_host)
 

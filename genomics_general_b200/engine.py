@@ -18,6 +18,11 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+def _addr(buf):
+    """the address of a numpy array or of any other writable buffer (the *_emit slabs)"""
+    return C.c_void_p(buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf)))
+
+
 class PinnedArray:
     """numpy view over cudaHostAlloc'd memory (freed on close/GC)."""
 
@@ -428,8 +433,7 @@ class Engine:
         (rows, bytes) written."""
         rows = C.c_int64(0)
         nb = C.c_size_t(0)
-        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
-        check(self._lib.pg_filter_emit(self._ctx, self.FILTER_FORMATS[fmt], 1 if freq_order else 0, int(row0), C.c_void_p(addr),
+        check(self._lib.pg_filter_emit(self._ctx, self.FILTER_FORMATS[fmt], 1 if freq_order else 0, int(row0), _addr(buf),
                                        int(cap), C.byref(rows), C.byref(nb)), "pg_filter_emit")
         return int(rows.value), int(nb.value)
 
@@ -538,8 +542,7 @@ class Engine:
         (rows, bytes) written."""
         rows = C.c_int64(0)
         nb = C.c_size_t(0)
-        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
-        check(self._lib.pg_vcf_emit(self._ctx, int(row0), C.c_void_p(addr), int(cap), C.byref(rows), C.byref(nb)),
+        check(self._lib.pg_vcf_emit(self._ctx, int(row0), _addr(buf), int(cap), C.byref(rows), C.byref(nb)),
               "pg_vcf_emit")
         return int(rows.value), int(nb.value)
 
@@ -586,8 +589,7 @@ class Engine:
         (row, part) to resume at, bytes written."""
         r1, p1 = C.c_int64(0), C.c_int64(0)
         nb = C.c_size_t(0)
-        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
-        check(self._lib.pg_seq_emit(self._ctx, int(row0), int(part0), C.c_void_p(addr), int(cap), C.byref(r1), C.byref(p1),
+        check(self._lib.pg_seq_emit(self._ctx, int(row0), int(part0), _addr(buf), int(cap), C.byref(r1), C.byref(p1),
                                     C.byref(nb)), "pg_seq_emit")
         return int(r1.value), int(p1.value), int(nb.value)
 
@@ -639,8 +641,7 @@ class Engine:
     def g2v_emit(self, byte0: int, buf, cap: int) -> int:
         """Bytes byte0.. (at most cap) of the last g2v_sites' VCF rows into buf (pinned for speed); returns the bytes written"""
         nb = C.c_size_t(0)
-        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
-        check(self._lib.pg_g2v_emit(self._ctx, int(byte0), C.c_void_p(addr), int(cap), C.byref(nb)), "pg_g2v_emit")
+        check(self._lib.pg_g2v_emit(self._ctx, int(byte0), _addr(buf), int(cap), C.byref(nb)), "pg_g2v_emit")
         return int(nb.value)
 
     def ws_spec(self, col_slot, n_slots: int, n_fields: int):
@@ -725,8 +726,7 @@ class Engine:
     def merge_emit(self, byte0: int, buf, cap: int) -> int:
         """Bytes byte0.. (at most cap) of the last merge_rows' rows into buf (pinned for speed); returns the bytes written"""
         nb = C.c_size_t(0)
-        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
-        check(self._lib.pg_merge_emit(self._ctx, int(byte0), C.c_void_p(addr), int(cap), C.byref(nb)), "pg_merge_emit")
+        check(self._lib.pg_merge_emit(self._ctx, int(byte0), _addr(buf), int(cap), C.byref(nb)), "pg_merge_emit")
         return int(nb.value)
 
     def s2g_fasta_load(self, text: bytes):
@@ -781,8 +781,7 @@ class Engine:
     def s2g_emit(self, byte0: int, buf, cap: int) -> int:
         """Bytes byte0.. (at most cap) of the last s2g_plan's rows into buf (pinned for speed); returns the bytes written"""
         nb = C.c_size_t(0)
-        addr = buf.ctypes.data if hasattr(buf, "ctypes") else C.addressof(C.c_char.from_buffer(buf))
-        check(self._lib.pg_s2g_emit(self._ctx, int(byte0), C.c_void_p(addr), int(cap), C.byref(nb)), "pg_s2g_emit")
+        check(self._lib.pg_s2g_emit(self._ctx, int(byte0), _addr(buf), int(cap), C.byref(nb)), "pg_s2g_emit")
         return int(nb.value)
 
     def site_counts(self, site0: int = 0, n: int = None, out=None):

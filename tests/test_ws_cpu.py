@@ -114,6 +114,16 @@ def test_narrowings_are_refused(tmp_path, monkeypatch, body, what):
     assert what in str(e.value), str(e.value)
 
 
+def test_empty_input_is_refused_as_window_stats(tmp_path, monkeypatch):
+    from oracle_engine_ws import WsOracleEngine
+    p = tmp_path / "empty.tsv"
+    p.write_bytes(b"")
+    with pytest.raises(SystemExit) as e:
+        run_cli(["-i", str(p), "-w", "10"], tmp_path, monkeypatch, WsOracleEngine)
+    assert str(e.value).startswith("windowStats: the input is empty"), str(e.value)
+    assert run_cli.got == b""
+
+
 def test_blank_lines_skipped_and_flags_without_effect(tmp_path, monkeypatch):
     from oracle_engine_ws import WsOracleEngine
     p = tmp_path / "t.tsv"
